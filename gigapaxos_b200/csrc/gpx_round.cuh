@@ -360,6 +360,10 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
    * memory by ONE TMA bulk copy */
   __shared__ __align__(128) gpx_request_rec s_req[TPB + 2];
   __shared__ __align__(8) unsigned long long s_bar;
+  /* the ACCEPT and DECISION log images of a warp's teams, [kind][lane][team] x 32 B: staged here and written to the
+   * rings by the whole warp as contiguous 16 B per thread, so every store instruction fills whole sectors (written by
+   * their own threads, the 32-byte images at a 32-byte stride were two half-sector stores per image) */
+  __shared__ __align__(16) int4 s_img[GPX_RBLOCK / 32u][2 * L * (32u / LP) * 2];
   if (threadIdx.x < C_NCTR) s_ctr[threadIdx.x] = 0;
   if (threadIdx.x == 0) mbar_init(&s_bar, 1);
   __syncthreads();
@@ -534,9 +538,10 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
     /* my lane's two log segments are linear inside the ring (a launch never straddles the wrap) */
     uint8_t* const seg_p = ring_ptr(S, sub, seg);
     const unsigned frame_ref = (unsigned)(((seg + pay_rel + poff) & (S.ring_cap - 1)) >> 4);
-    /* ACCEPT log image + my lane's copy of the blob (AbstractPaxosLogger.logAndMessage) */
-    st256_stream(seg_p + 64 + (size_t)i * 32, q0,
-                 make_int4(median, (int)(GPX_F_ACCEPT | ((1u << sub) << 16)), rq0.z, rq0.w));
+    /* ACCEPT log image (staged, written below) + my lane's copy of the blob (AbstractPaxosLogger.logAndMessage) */
+    int4* const img = &s_img[threadIdx.x >> 5][(sub * TPW + team_in_warp) * 2];
+    img[0] = q0;
+    img[1] = make_int4(median, (int)(GPX_F_ACCEPT | ((1u << sub) << 16)), rq0.z, rq0.w);
     st_stream4(seg_p + 64 + (size_t)n * 32 + (size_t)i * 16, make_int4((int)poff, (int)plen, 1, crow.y));
     if (plen) {
       uint8_t* dst = seg_p + pay_rel + poff;
@@ -550,9 +555,10 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
     }
     /* commit (handleBatchedCommit :1488-1501 + extractExecuteAndCheckpoint): the accept is the decision */
     const bool metaf = cf_logmeta;
-    st256_stream(seg_p + res_a + 64 + (size_t)i * 32, q0,
-                 make_int4(metaf ? -1 : dmed, (int)((GPX_F_DECISION | (metaf ? GPX_F_META : 0u)) | ((1u << sub) << 16)),
-                           rq0.z, rq0.w));
+    img[2 * L * TPW] = q0; /* the DECISION image, staged */
+    img[2 * L * TPW + 1] =
+        make_int4(metaf ? -1 : dmed, (int)((GPX_F_DECISION | (metaf ? GPX_F_META : 0u)) | ((1u << sub) << 16)), rq0.z,
+                  rq0.w);
     gc_step(row, dmed);
     { /* EXEC record (PISM.execute hands the request to the app); shouldCheckpoint :2037-2041 */
       const bool ckpt = (slot % cpi) == 0;
@@ -594,6 +600,22 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
     RA.todo[k] = i; /* the run goes to k_round_slow */
     if (k == 0 && RA.tail_launch) /* the first left-over run of the round brings the second kernel in */
       k_round_slow<L, LP><<<RA.slow_grid, GPX_BLOCK, 0, cudaStreamTailLaunch>>>(S, RA);
+  }
+  { /* the staged log images of the warp's fast teams, in runs of contiguous 16 B: s_img index k is half k & 1 of the
+     * image of team (k >> 1) % TPW, kind x lane (k >> 1) / TPW; the segment base of lane l comes from warp lane l */
+    const uint32_t sfm = __ballot_sync(FULL, sf && sub == 0); /* bit tbase: the team took the fast path */
+    __syncwarp();
+    const uint32_t i0 = (blockIdx.x * (GPX_RBLOCK / 32u) + (threadIdx.x >> 5)) * TPW; /* request of the warp's team 0 */
+    constexpr uint32_t NIMG = 4u * L * TPW;
+#pragma unroll
+    for (uint32_t k0 = 0; k0 < NIMG; k0 += 32u) {
+      const uint32_t k = k0 + lane_id, r = k >> 1, team = r % TPW, kl = r / TPW, l = kl % L;
+      const unsigned long long seg_l = __shfl_sync(FULL, seg, l);
+      if (k < NIMG && ((sfm >> (team * LP)) & 1u))
+        st_stream4(ring_ptr(S, l, seg_l + (kl >= (uint32_t)L ? res_a : 0ull) + 64ull +
+                                      (unsigned long long)(i0 + team) * 32ull + (k & 1u) * 16u),
+                   s_img[threadIdx.x >> 5][k]);
+    }
   }
   if (valid && sub == 0) RA.mark[i] = sf ? 0 : 1;
   if (sf && pal && plen > 16u) { /* bodies longer than one chunk: four independent 128-bit loads in flight */
