@@ -46,6 +46,10 @@ reply_dtype = np.dtype([("gid", "<u4"), ("slot", "<i4"), ("bnum", "<i4"), ("bcoo
                         ("who", "<u4"), ("req_id", "<i8")])
 exec_dtype = np.dtype([("gid", "<u4"), ("slot", "<i4"), ("req_id", "<i8"), ("payload_off", "<u4"), ("flags", "<u4")])
 batch_ent_dtype = np.dtype([("req_id", "<i8"), ("len", "<u4"), ("flags", "<u4")])
+wire_ref_dtype = np.dtype([("off", "<u4"), ("len", "<u4"), ("gid", "<u4"), ("node", "<i4")])  # gpx_wire_ref
+# per-packet status of gpx_wire_decode_batch, per-record outcome of gpx_wire_encode_*
+WS_OK, WS_UNKNOWN_NAME, WS_VERSION, WS_MALFORMED, WS_UNHANDLED, WS_NOT_LOCAL = 0, 1, 2, 3, 4, 5
+WE_SENT, WE_VOID, WE_LOCAL, WE_NACK, WE_NO_NAME = 0, 1, 2, 3, 4
 accepted_pvalue_dtype = np.dtype([("slot", "<i4"), ("bnum", "<i4"), ("bcoord", "<i4"), ("frame_ref", "<u4"),
                                   ("req_id", "<i8"), ("payload_len", "<u4"), ("flags", "<u4")])
 prepare_reply_dtype = np.dtype([("gid", "<u4"), ("first_slot", "<i4"), ("bnum", "<i4"), ("bcoord", "<i4"), ("who", "<u4"),

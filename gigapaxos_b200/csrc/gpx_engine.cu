@@ -26,6 +26,9 @@
 #include "gpx_phase1b.cuh"
 #include "gpx_pause.cuh"
 #include "gpx_logfind.cuh"
+#include "gpx_wire_dev.cuh"
+
+#include <cub/cub.cuh>
 
 static thread_local std::string g_err;
 static int fail(int code, const std::string& msg) {
@@ -113,6 +116,13 @@ struct gpx_engine {
   bool compact_fused = false; /* round_on_stream(fused = false): k_propose + k_act instead of the four phase kernels */
   cudaEvent_t ev[5];
   gpx_kernel_times kt;
+  /* phase-2 wire calls (gpx_wire_host.inc): group names, allocated by the first call that needs them */
+  WireNames wn{};
+  bool names_on = false;
+  std::vector<uint8_t> h_named; /* [G] the gid has a table entry */
+  uint64_t names_live = 0, names_used = 0; /* entries; cells taken since the last rebuild (live + removed) */
+  void* d_wire = nullptr;
+  size_t wire_bytes = 0;
 
   template <typename T>
   int dalloc(T** p, size_t n) {
@@ -321,6 +331,7 @@ void gpx_engine_destroy(gpx_engine* e) {
   cudaDeviceSynchronize();
   for (void* p : e->allocs) cudaFree(p);
   if (e->d_misc) cudaFree(e->d_misc);
+  if (e->d_wire) cudaFree(e->d_wire);
   if (e->h_ctl) cudaFreeHost(e->h_ctl);
   for (auto& ps : e->pipe) {
     if (ps.h_ctl) cudaFreeHost(ps.h_ctl);
@@ -340,6 +351,8 @@ void gpx_engine_destroy(gpx_engine* e) {
 }
 
 /* ---- groups ----------------------------------------------------------------------- */
+static int names_drop(gpx_engine* e, uint32_t n, const uint32_t* gids, const uint8_t* only); /* gpx_wire_host.inc */
+
 static int intern_mset(gpx_engine* e, std::vector<int32_t> m, uint32_t* id, bool* added) {
   std::sort(m.begin(), m.end()); /* PISM ctor sorts groupMembers :205 */
   auto it = e->mset_ids.find(m);
@@ -410,6 +423,11 @@ int gpx_create_groups(gpx_engine* e, uint32_t n, const gpx_group_desc* d) {
   k_init_groups<<<cdiv(n, 256), 256, 0, e->stream>>>(e->S, (const InitRec*)e->d_misc, n);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(e->stream));
+  if (e->names_on) {
+    std::vector<uint32_t> g(n);
+    for (uint32_t k = 0; k < n; k++) g[k] = d[k].gid;
+    return names_drop(e, n, g.data(), nullptr);
+  }
   return GPX_OK;
 }
 
@@ -424,7 +442,7 @@ int gpx_destroy_groups(gpx_engine* e, uint32_t n, const uint32_t* gids) {
   k_destroy_groups<<<cdiv(n, 256), 256, 0, e->stream>>>(e->S, (const uint32_t*)e->d_misc, n);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(e->stream));
-  return GPX_OK;
+  return names_drop(e, n, gids, nullptr);
 }
 
 int gpx_dump_rows(gpx_engine* e, uint32_t n, const uint32_t* gids, uint32_t lane, gpx_row* out) {
@@ -477,6 +495,11 @@ int gpx_load_rows(gpx_engine* e, uint32_t n, const gpx_row* rows) {
   k_load_rows<<<cdiv(n, 128), 128, 0, e->stream>>>(e->S, (const LoadRec*)e->d_misc, n);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(e->stream));
+  if (e->names_on) {
+    std::vector<uint32_t> g(n);
+    for (uint32_t k = 0; k < n; k++) g[k] = rows[k].gid;
+    return names_drop(e, n, g.data(), nullptr);
+  }
   return GPX_OK;
 }
 
@@ -1773,9 +1796,10 @@ int gpx_pause_groups(gpx_engine* e, uint32_t n, const uint32_t* gids, gpx_row* o
     }
     e->h_name_hash[gids[i]] = e->h_version[gids[i]] = 0;
   }
-  return GPX_OK;
+  return names_drop(e, n, gids, out_paused);
 }
 
 #include "gpx_spread_host.inc"
+#include "gpx_wire_host.inc"
 
 } /* extern "C" */

@@ -1,0 +1,704 @@
+/*
+ * gpx_wire_dev.cuh -- the phase-2 wire codec on the device: a batch of received AcceptPacket / BatchedAcceptReply /
+ * BatchedCommit bytes becomes engine records, and the engine's reply and decision records become BATCHED_ACCEPT_REPLY
+ * and BATCHED_COMMIT bytes, coalesced as one PaxosPacketBatcher per node does (PaxosPacketBatcher.java:97-179,
+ * 345-454).  Byte layouts: include/gpx_wire.h; the host codec there (gpx_wire.cpp) is the reference these kernels are
+ * tested against.
+ *
+ * Names: a packet names its group by (paxosID, version) (PaxosPacket.java:459-476).  gpx_set_group_names stores, per
+ * gid, the paxosID bytes and the version, and an open-addressing table from the bytes to the gid, probed from the Java
+ * String.hashCode of the name; a hit is confirmed by comparing the bytes.
+ *
+ * Every kernel here is scalar -- one thread per packet, per record or per coalesced run, plain loads and stores over
+ * gpx_dev.cuh's state -- so tests/emu compiles this file for the host.  The scans that size the outputs and the stable
+ * sorts by gid run between the launches (CUB on the device, the standard library in the emulation).
+ */
+#pragma once
+#include "gpx_dev.cuh"
+#include "gpx_wire.h"
+
+#define GPX_NAME_BYTES 128u           /* per gid: length byte + up to GPX_WIRE_MAX_ID bytes */
+#define GPX_NAME_EMPTY 0u             /* table key: never used */
+#define GPX_NAME_TOMB 0xffffffffu     /* table key: removed */
+#define GPX_NAME_NONE 0xffffffffu     /* WireNames.slot: the gid has no name */
+#define GPX_WIRE_NOKEY 0xffffffffu    /* sort key of a record that is not encoded */
+
+struct WireNames {
+  uint2* tab;       /* [mask + 1] {gid + 1 (GPX_NAME_EMPTY / GPX_NAME_TOMB), String.hashCode} */
+  uint32_t mask;
+  uint8_t* name;    /* [G][GPX_NAME_BYTES] */
+  int32_t* version; /* [G] */
+  uint32_t* slot;   /* [G] table index of the gid's entry, GPX_NAME_NONE if it has none */
+};
+
+/* ---- big-endian reads (java.nio.ByteBuffer) ---------------------------------------------------------------------- */
+struct WireRd {
+  const uint8_t* p;
+  uint32_t len, n;
+  bool ok;
+};
+__device__ __forceinline__ bool wr_need(WireRd& r, uint32_t k) {
+  if (!r.ok || k > r.len - r.n) {
+    r.ok = false;
+    return false;
+  }
+  return true;
+}
+__device__ __forceinline__ uint32_t wr_u8(WireRd& r) {
+  if (!wr_need(r, 1)) return 0;
+  return r.p[r.n++];
+}
+__device__ __forceinline__ int32_t wr_i32(WireRd& r) {
+  if (!wr_need(r, 4)) return 0;
+  const uint8_t* q = r.p + r.n;
+  r.n += 4;
+  return (int32_t)(((uint32_t)q[0] << 24) | ((uint32_t)q[1] << 16) | ((uint32_t)q[2] << 8) | (uint32_t)q[3]);
+}
+__device__ __forceinline__ int64_t wr_i64(WireRd& r) {
+  const uint32_t hi = (uint32_t)wr_i32(r), lo = (uint32_t)wr_i32(r);
+  return (int64_t)(((uint64_t)hi << 32) | lo);
+}
+__device__ __forceinline__ void wr_skip(WireRd& r, uint32_t k) {
+  if (wr_need(r, k)) r.n += k;
+}
+/* a length field followed by that many bytes; a negative length is malformed */
+__device__ __forceinline__ uint32_t wr_bytes(WireRd& r, uint32_t* at) {
+  const int32_t l = wr_i32(r);
+  if (l < 0) r.ok = false;
+  *at = r.n;
+  wr_skip(r, (uint32_t)l);
+  return r.ok ? (uint32_t)l : 0u;
+}
+
+/* PaxosPacket header :459-476 */
+struct WireHdr {
+  int32_t type, version;
+  uint32_t id_at, id_len;
+};
+__device__ __forceinline__ bool wr_header(WireRd& r, WireHdr& h) {
+  const int32_t pp = wr_i32(r);
+  h.type = wr_i32(r);
+  h.version = wr_i32(r);
+  h.id_len = wr_u8(r);
+  h.id_at = r.n;
+  wr_skip(r, h.id_len);
+  return r.ok && pp == GPX_PT_PAXOS_PACKET && h.id_len <= GPX_WIRE_MAX_ID;
+}
+
+/* RequestPacket(ByteBuffer) :956-1024 up to the batched requests: the fields the engine keeps */
+struct WireReq {
+  int64_t req_id;
+  uint32_t stop;
+  int32_t entry;
+  uint32_t val_at, val_len;
+  int32_t n_batched;
+};
+__device__ __forceinline__ void wr_request_body(WireRd& r, WireReq& q) {
+  q.req_id = wr_i64(r);
+  q.stop = wr_u8(r) == 1u;
+  wr_skip(r, 4 + 2 + 4 + 2); /* client and listen addresses */
+  q.entry = wr_i32(r);
+  wr_skip(r, 8 + 1 + 4 + 1); /* entryTime, shouldReturnRequestValue, forwardCount, broadcasted */
+  uint32_t at;
+  wr_bytes(r, &at); /* digest */
+  q.val_len = wr_bytes(r, &q.val_at);
+  wr_bytes(r, &at); /* responseValue */
+  q.n_batched = wr_i32(r);
+  if (q.n_batched < 0) r.ok = false;
+}
+
+__device__ __forceinline__ void wire_copy(uint8_t* d, const uint8_t* s, uint32_t n) {
+  for (uint32_t i = 0; i < n; i++) d[i] = s[i];
+}
+
+__device__ __forceinline__ uint32_t wire_popc(uint32_t m) { /* scalar: the emulation has no __popc */
+  uint32_t c = 0;
+  for (; m; m &= m - 1) c++;
+  return c;
+}
+
+/* ---- names ----------------------------------------------------------------------------------------------------- */
+__device__ __forceinline__ int32_t wire_name_hash(const uint8_t* s, uint32_t n) { /* String.hashCode (ISO-8859-1) */
+  uint32_t h = 0;
+  for (uint32_t i = 0; i < n; i++) h = 31u * h + s[i];
+  return (int32_t)h;
+}
+__device__ __forceinline__ bool wire_name_eq(const WireNames& W, uint32_t gid, const uint8_t* s, uint32_t n) {
+  const uint8_t* m = W.name + (size_t)gid * GPX_NAME_BYTES;
+  if (m[0] != n) return false;
+  for (uint32_t i = 0; i < n; i++)
+    if (m[1 + i] != s[i]) return false;
+  return true;
+}
+/* gid named s[0..n), or GPX_NAME_NONE */
+__device__ __forceinline__ uint32_t wire_name_find(const WireNames& W, const uint8_t* s, uint32_t n) {
+  const uint32_t h = (uint32_t)wire_name_hash(s, n);
+  uint32_t i = h & W.mask;
+  for (uint32_t probe = 0; probe <= W.mask; probe++, i = (i + 1) & W.mask) {
+    const uint2 e = W.tab[i];
+    if (e.x == GPX_NAME_EMPTY) break;
+    if (e.x != GPX_NAME_TOMB && e.y == h && wire_name_eq(W, e.x - 1u, s, n)) return e.x - 1u;
+  }
+  return GPX_NAME_NONE;
+}
+
+/* enters gid (its bytes already stored) at the first free or removed cell of its probe sequence */
+__device__ __forceinline__ void wire_name_put(const WireNames& W, uint32_t gid, bool reuse_tomb) {
+  const uint8_t* m = W.name + (size_t)gid * GPX_NAME_BYTES;
+  const uint32_t h = (uint32_t)wire_name_hash(m + 1, m[0]);
+  uint32_t i = h & W.mask;
+  for (;;) {
+    const uint32_t cur = W.tab[i].x;
+    if (cur == GPX_NAME_EMPTY || (reuse_tomb && cur == GPX_NAME_TOMB)) {
+      if (atomicCAS(&W.tab[i].x, cur, gid + 1u) == cur) {
+        W.tab[i].y = h;
+        W.slot[gid] = i;
+        return;
+      }
+      continue; /* another insert took the cell: look at it again */
+    }
+    i = (i + 1) & W.mask;
+  }
+}
+
+/* one name per thread: the gid's bytes and version are already stored (host copy); the caller guarantees that no live
+ * gid has the same name and that the table has free cells */
+struct NameSetArgs {
+  const uint32_t* gids;
+  uint32_t n;
+};
+__global__ void k_names_insert(const __grid_constant__ WireNames W, const __grid_constant__ NameSetArgs A) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k < A.n) wire_name_put(W, A.gids[k], true);
+}
+/* removes the entries of the given gids (gids without one are skipped) */
+__global__ void k_names_remove(const __grid_constant__ WireNames W, const __grid_constant__ NameSetArgs A) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= A.n) return;
+  const uint32_t gid = A.gids[k];
+  const uint32_t s = W.slot[gid];
+  if (s == GPX_NAME_NONE) return;
+  W.tab[s].x = GPX_NAME_TOMB;
+  W.slot[gid] = GPX_NAME_NONE;
+}
+/* with the table cleared: re-enters every named gid (the removed cells become free again) */
+__global__ void k_names_rehash(const __grid_constant__ WireNames W, uint32_t G) {
+  const uint32_t gid = blockIdx.x * blockDim.x + threadIdx.x;
+  if (gid < G && W.slot[gid] != GPX_NAME_NONE) wire_name_put(W, gid, false);
+}
+/* a batch of names staged as [n][GPX_NAME_BYTES] (length byte + bytes): found[k] = the gid that has name k now, or
+ * GPX_NAME_NONE (gpx_set_group_names refuses a name another live gid holds before it changes anything) */
+__global__ void k_names_find(const __grid_constant__ WireNames W, const uint8_t* staged, uint32_t n, uint32_t* found) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= n) return;
+  const uint8_t* m = staged + (size_t)k * GPX_NAME_BYTES;
+  found[k] = wire_name_find(W, m + 1, m[0]);
+}
+/* stores name k and version k of the batch at gids[k] */
+__global__ void k_names_store(const __grid_constant__ WireNames W, const __grid_constant__ NameSetArgs A,
+                              const uint8_t* staged, const int32_t* version) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= A.n) return;
+  wire_copy(W.name + (size_t)A.gids[k] * GPX_NAME_BYTES, staged + (size_t)k * GPX_NAME_BYTES, GPX_NAME_BYTES);
+  W.version[A.gids[k]] = version[k];
+}
+
+/* ---- decode ---------------------------------------------------------------------------------------------------- */
+enum { WD_ACC = 0, WD_BLOB = 1, WD_REP = 2, WD_DEC = 3, WD_NCNT = 4 };
+
+struct WireDecodeArgs {
+  const uint8_t* bytes;
+  const gpx_wire_ref* pkts;
+  uint64_t n_bytes;
+  uint32_t n;
+  uint32_t* cnt;  /* [WD_NCNT][n]: pass 0 writes the packet's output sizes (blob bytes padded to 16) */
+  uint32_t* off;  /* [WD_NCNT][n]: pass 1 reads their exclusive prefix sums */
+  int32_t* status;
+  /* pass 1: staging in packet order, and the sort keys (gids) beside it */
+  gpx_accept_rec* acc;
+  uint8_t* blob;
+  gpx_accept_reply_rec* rep;
+  gpx_decision_rec* dec;
+  uint32_t* acc_key;
+  uint32_t* rep_key;
+  uint32_t* dec_key;
+  int emit;
+};
+
+__device__ __forceinline__ uint8_t wire_member_idx(const MsetInfo* ms, uint32_t R, int32_t node) {
+  for (uint32_t i = 0; i < R; i++)
+    if (ms->nodes[i] == node) return (uint8_t)i;
+  return 0xffu;
+}
+/* entry-lane bits of gpx_request_rec.flags: the lane serving the entry replica, 0xf when that node is not local */
+__device__ __forceinline__ uint32_t wire_entry_bits(const DevState& S, int32_t entry) {
+  for (uint32_t l = 0; l < S.L; l++)
+    if (S.lane_node[l] == entry) return l << 8;
+  return 0xfu << 8;
+}
+
+/* one thread per packet.  Pass 0 (emit == 0) parses and validates the packet, looks its name up and writes its status
+ * and output sizes; pass 1 parses it again and writes its records at the scanned offsets. */
+__global__ void k_wire_decode(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                              const __grid_constant__ WireDecodeArgs A) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= A.n) return;
+  if (A.emit && A.status[k] != GPX_WS_OK) return;
+  const gpx_wire_ref ref = A.pkts[k];
+  uint32_t c[WD_NCNT] = {0, 0, 0, 0};
+  int32_t st = GPX_WS_OK;
+  WireRd r;
+  r.p = A.bytes + ref.off;
+  r.len = ref.len;
+  r.n = 0;
+  r.ok = (uint64_t)ref.off + ref.len <= A.n_bytes;
+  WireHdr h;
+  uint32_t gid = GPX_NAME_NONE, R = 0;
+  const MsetInfo* ms = nullptr;
+  if (r.ok && ref.len > 0 && r.p[0] == '{') {
+    st = GPX_WS_UNHANDLED; /* JSON packet */
+  } else if (!wr_header(r, h)) {
+    st = GPX_WS_MALFORMED;
+  } else if (h.type != GPX_PT_ACCEPT && h.type != GPX_PT_BATCHED_ACCEPT_REPLY && h.type != GPX_PT_BATCHED_COMMIT) {
+    st = GPX_WS_UNHANDLED;
+  }
+  /* body: parsed in full before anything is looked up, so a malformed packet is malformed whatever its name */
+  WireReq q;
+  uint32_t sub_at = 0, n_sub = 0, val_total = 0, stop_any = 0;
+  int32_t slot = 0, bnum = 0, bcoord = 0, median = 0, sender = 0, acceptor = 0, max_cp = 0, cnt_slots = 0, n_group = 0;
+  uint32_t slots_at = 0;
+  if (st == GPX_WS_OK) {
+    if (h.type == GPX_PT_ACCEPT) { /* AcceptPacket :95-138 */
+      wr_request_body(r, q);
+      sub_at = r.n;
+      n_sub = r.ok ? (uint32_t)q.n_batched : 0u;
+      val_total = q.val_len;
+      stop_any = q.stop;
+      for (uint32_t b = 0; b < n_sub && r.ok; b++) { /* {int length}{REQUEST packet} :929-936 */
+        const int32_t l = wr_i32(r);
+        if (l < 0 || !wr_need(r, (uint32_t)l)) {
+          r.ok = false;
+          break;
+        }
+        WireRd s;
+        s.p = r.p + r.n;
+        s.len = (uint32_t)l;
+        s.n = 0;
+        s.ok = true;
+        WireHdr sh;
+        WireReq sq;
+        const bool hok = wr_header(s, sh);
+        wr_request_body(s, sq);
+        /* a latched request carries no latched requests of its own (RequestBatcher latches one level) */
+        if (!hok || !s.ok || sq.n_batched != 0 || s.n != s.len) r.ok = false;
+        val_total += sq.val_len;
+        stop_any |= sq.stop;
+        r.n += (uint32_t)l;
+      }
+      slot = wr_i32(r);
+      bnum = wr_i32(r);
+      bcoord = wr_i32(r);
+      wr_u8(r); /* recovery */
+      median = wr_i32(r);
+      wr_u8(r); /* noCoalesce */
+      sender = wr_i32(r);
+    } else if (h.type == GPX_PT_BATCHED_ACCEPT_REPLY) { /* BatchedAcceptReply :103-173 */
+      acceptor = wr_i32(r);
+      bnum = wr_i32(r);
+      bcoord = wr_i32(r);
+      wr_i32(r); /* slotNumber of the first reply: also in the map */
+      max_cp = wr_i32(r);
+      wr_skip(r, 8 + 1); /* requestID, undigestRequest */
+      cnt_slots = wr_i32(r);
+      if (cnt_slots < 0 || (r.ok && (uint64_t)cnt_slots * 12u > r.len - r.n)) r.ok = false;
+      slots_at = r.n;
+      if (r.ok) wr_skip(r, (uint32_t)cnt_slots * 12u);
+    } else { /* BatchedCommit :184-252 */
+      bnum = wr_i32(r);
+      bcoord = wr_i32(r);
+      median = wr_i32(r);
+      cnt_slots = wr_i32(r);
+      if (cnt_slots < 0 || (r.ok && (uint64_t)cnt_slots * 4u > r.len - r.n)) r.ok = false;
+      slots_at = r.n;
+      if (r.ok) wr_skip(r, (uint32_t)cnt_slots * 4u);
+      n_group = wr_i32(r);
+      if (n_group < 0 || (r.ok && (uint64_t)n_group * 4u > r.len - r.n)) r.ok = false;
+      if (r.ok) wr_skip(r, (uint32_t)n_group * 4u);
+    }
+    if (!r.ok || r.n != r.len) st = GPX_WS_MALFORMED;
+  }
+  uint8_t acc_idx = 0xffu, dst_idx = 0xffu;
+  if (st == GPX_WS_OK) {
+    gid = wire_name_find(W, r.p + h.id_at, h.id_len);
+    const GroupCtx g = group_ctx(S, gid);
+    if (gid == GPX_NAME_NONE || !g.live) {
+      st = GPX_WS_UNKNOWN_NAME;
+    } else if (W.version[gid] != h.version) {
+      st = GPX_WS_VERSION; /* PISM :441-447 */
+    } else {
+      ms = g.ms;
+      R = g.R;
+      if (h.type == GPX_PT_BATCHED_ACCEPT_REPLY) {
+        acc_idx = wire_member_idx(ms, R, acceptor);
+        dst_idx = wire_member_idx(ms, R, bcoord);
+        if (acc_idx == 0xffu || dst_idx == 0xffu) st = GPX_WS_MALFORMED; /* acceptor / coordinator not a member */
+        else if (ms->lane_of_idx[dst_idx] == 0xffu) st = GPX_WS_NOT_LOCAL;
+      } else if (ms->lane_mask == 0) {
+        st = GPX_WS_NOT_LOCAL;
+      }
+    }
+  }
+  if (st == GPX_WS_OK) {
+    if (h.type == GPX_PT_ACCEPT) {
+      c[WD_ACC] = 1;
+      const uint32_t nreq = 1u + n_sub;
+      c[WD_BLOB] = ((nreq > 1 ? 16u * nreq : 0u) + val_total + 15u) & ~15u;
+    } else if (h.type == GPX_PT_BATCHED_ACCEPT_REPLY) {
+      c[WD_REP] = (uint32_t)cnt_slots;
+    } else {
+      c[WD_DEC] = (uint32_t)cnt_slots;
+    }
+  }
+  if (!A.emit) {
+    A.status[k] = st;
+    for (int j = 0; j < WD_NCNT; j++) A.cnt[(size_t)j * A.n + k] = c[j];
+    return;
+  }
+  if (h.type == GPX_PT_ACCEPT) {
+    const uint32_t o = A.off[(size_t)WD_ACC * A.n + k], bo = A.off[(size_t)WD_BLOB * A.n + k];
+    const uint32_t nreq = 1u + n_sub;
+    uint8_t* blob = A.blob + bo;
+    if (nreq == 1) {
+      wire_copy(blob, r.p + q.val_at, q.val_len);
+    } else { /* [nreq x gpx_batch_ent][values] as gpx_propose builds it (k_build_blobs) */
+      uint32_t vo = 16u * nreq;
+      gpx_batch_ent be;
+      be.req_id = q.req_id;
+      be.len = q.val_len;
+      be.flags = (q.stop ? GPX_F_STOP : 0u) | wire_entry_bits(S, q.entry);
+      wire_copy(blob, reinterpret_cast<const uint8_t*>(&be), 16);
+      wire_copy(blob + vo, r.p + q.val_at, q.val_len);
+      vo += q.val_len;
+      WireRd rr;
+      rr.p = r.p;
+      rr.len = r.len;
+      rr.n = sub_at;
+      rr.ok = true;
+      for (uint32_t b = 0; b < n_sub; b++) {
+        const int32_t l = wr_i32(rr);
+        WireRd s;
+        s.p = rr.p + rr.n;
+        s.len = (uint32_t)l;
+        s.n = 0;
+        s.ok = true;
+        WireHdr sh;
+        WireReq sq;
+        wr_header(s, sh);
+        wr_request_body(s, sq);
+        be.req_id = sq.req_id;
+        be.len = sq.val_len;
+        be.flags = (sq.stop ? GPX_F_STOP : 0u) | wire_entry_bits(S, sq.entry);
+        wire_copy(blob + 16u * (1u + b), reinterpret_cast<const uint8_t*>(&be), 16);
+        wire_copy(blob + vo, s.p + sq.val_at, sq.val_len);
+        vo += sq.val_len;
+        rr.n += (uint32_t)l;
+      }
+    }
+    const uint32_t used = (nreq > 1 ? 16u * nreq : 0u) + val_total;
+    for (uint32_t b = used; b < c[WD_BLOB]; b++) blob[b] = 0;
+    gpx_accept_rec a;
+    a.h.gid = gid;
+    a.h.slot = slot;
+    a.h.bnum = bnum;
+    a.h.bcoord = bcoord;
+    a.h.median_cp = median;
+    a.h.flags = (uint16_t)(GPX_F_ACCEPT | (stop_any ? GPX_F_STOP : 0u));
+    a.h.dst_mask = ms->lane_mask;
+    a.h.req_id = q.req_id;
+    a.payload_off = bo;
+    a.payload_len = used;
+    a.nreq = nreq;
+    a.sender = sender;
+    A.acc[o] = a;
+    A.acc_key[o] = gid;
+  } else if (h.type == GPX_PT_BATCHED_ACCEPT_REPLY) {
+    const uint32_t o = A.off[(size_t)WD_REP * A.n + k];
+    WireRd s;
+    s.p = r.p;
+    s.len = r.len;
+    s.n = slots_at;
+    s.ok = true;
+    for (uint32_t j = 0; j < (uint32_t)cnt_slots; j++) {
+      gpx_accept_reply_rec x;
+      x.gid = gid;
+      x.slot = wr_i32(s);
+      x.bnum = bnum;
+      x.bcoord = bcoord;
+      x.max_cp = max_cp;
+      x.who = GPX_WHO(acc_idx, dst_idx, 0u);
+      x.req_id = wr_i64(s);
+      A.rep[o + j] = x;
+      A.rep_key[o + j] = gid;
+    }
+  } else {
+    const uint32_t o = A.off[(size_t)WD_DEC * A.n + k];
+    WireRd s;
+    s.p = r.p;
+    s.len = r.len;
+    s.n = slots_at;
+    s.ok = true;
+    for (uint32_t j = 0; j < (uint32_t)cnt_slots; j++) {
+      gpx_decision_rec d;
+      d.gid = gid;
+      d.slot = wr_i32(s);
+      d.bnum = bnum;
+      d.bcoord = bcoord;
+      d.median_cp = median;
+      d.flags = GPX_F_DECISION;
+      d.dst_mask = ms->lane_mask;
+      d.req_id = 0; /* a BatchedCommit carries slots only: the value is the accept the acceptor holds */
+      A.dec[o + j] = d;
+      A.dec_key[o + j] = gid;
+    }
+  }
+}
+
+/* launch glue of the host side (gpx_wire_host.inc) */
+__global__ void k_wire_iota(uint32_t* p, uint32_t n) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) p[i] = i;
+}
+/* tot[j] = the total of counter row j of [rows][n] from its exclusive prefix sums */
+__global__ void k_wire_totals(const uint32_t* cnt, const uint32_t* off, uint32_t n, uint32_t rows, uint32_t* tot) {
+  const uint32_t j = threadIdx.x;
+  if (j < rows) tot[j] = off[(size_t)j * n + n - 1] + cnt[(size_t)j * n + n - 1];
+}
+
+/* records (or their indices) into the order of a stable sort: dst[i] = src[perm[i]] */
+template <typename T>
+__global__ void k_wire_gather(const T* src, const uint32_t* perm, uint32_t n, T* dst) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = src[perm[i]];
+}
+
+/* ---- encode ---------------------------------------------------------------------------------------------------- */
+struct WireEncodeArgs {
+  const void* recs;     /* gpx_accept_reply_rec[n] or gpx_decision_rec[n] */
+  uint32_t n;
+  uint32_t n_lanes;     /* replies: record i * n_lanes + l belongs to lane l */
+  uint8_t* rstatus;     /* [n] GPX_WE_* per record */
+  uint32_t* key;        /* [n] sort key: (lane, gid) / gid, GPX_WIRE_NOKEY if not encoded */
+  const uint32_t* perm; /* [n] record indices in stable key order (GPX_WIRE_NOKEY keys last) */
+  const uint32_t* skey; /* [n] the keys in that order */
+  uint32_t* cnt;        /* [2][n] pass 0, per sorted position that starts a run: packet bytes, index entries */
+  const uint32_t* off;  /* [2][n] their exclusive prefix sums */
+  uint8_t* out;
+  gpx_wire_ref* refs;
+  int emit;
+};
+
+/* one thread per record: what happens to it and its sort key */
+__global__ void k_wire_enc_keys_replies(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                                        const __grid_constant__ WireEncodeArgs A) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= A.n) return;
+  const gpx_accept_reply_rec x = reinterpret_cast<const gpx_accept_reply_rec*>(A.recs)[i];
+  const uint32_t fl = GPX_WHO_FLAGS(x.who), lane = i % A.n_lanes;
+  uint8_t st = GPX_WE_SENT;
+  const GroupCtx g = group_ctx(S, x.gid);
+  if (fl & GPX_F_VOID) st = GPX_WE_VOID;
+  else if (fl & GPX_F_NACK) st = GPX_WE_NACK; /* allPositiveAcceptReplies :423-430: the host sends it alone */
+  else if (!g.live || GPX_WHO_DST(x.who) >= g.R || GPX_WHO_ACC(x.who) >= g.R) st = GPX_WE_VOID;
+  else if (g.ms->lane_of_idx[GPX_WHO_DST(x.who)] != 0xffu) st = GPX_WE_LOCAL; /* SHORT_CIRCUIT_LOCAL */
+  else if (W.slot == nullptr || W.slot[x.gid] == GPX_NAME_NONE) st = GPX_WE_NO_NAME;
+  A.rstatus[i] = st;
+  A.key[i] = st == GPX_WE_SENT ? lane * S.G + x.gid : GPX_WIRE_NOKEY;
+}
+__global__ void k_wire_enc_keys_decisions(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                                          const __grid_constant__ WireEncodeArgs A) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= A.n) return;
+  const gpx_decision_rec d = reinterpret_cast<const gpx_decision_rec*>(A.recs)[i];
+  uint8_t st = GPX_WE_SENT;
+  const GroupCtx g = group_ctx(S, d.gid);
+  if ((d.flags & GPX_F_VOID) || !g.live) st = GPX_WE_VOID;
+  else if (wire_popc(g.ms->lane_mask) >= g.R) st = GPX_WE_LOCAL; /* every member is a local lane */
+  else if (W.slot == nullptr || W.slot[d.gid] == GPX_NAME_NONE) st = GPX_WE_NO_NAME;
+  A.rstatus[i] = st;
+  A.key[i] = st == GPX_WE_SENT ? d.gid : GPX_WIRE_NOKEY;
+}
+
+__device__ __forceinline__ void ww_i32(uint8_t* p, int32_t v) {
+  const uint32_t u = (uint32_t)v;
+  p[0] = (uint8_t)(u >> 24);
+  p[1] = (uint8_t)(u >> 16);
+  p[2] = (uint8_t)(u >> 8);
+  p[3] = (uint8_t)u;
+}
+__device__ __forceinline__ void ww_i64(uint8_t* p, int64_t v) {
+  ww_i32(p, (int32_t)(uint32_t)((uint64_t)v >> 32));
+  ww_i32(p + 4, (int32_t)(uint32_t)(uint64_t)v);
+}
+/* PaxosPacket.toBytes :459-476; returns the bytes written */
+__device__ __forceinline__ uint32_t ww_header(uint8_t* p, int32_t type, const WireNames& W, uint32_t gid) {
+  const uint8_t* m = W.name + (size_t)gid * GPX_NAME_BYTES;
+  ww_i32(p, GPX_PT_PAXOS_PACKET);
+  ww_i32(p + 4, type);
+  ww_i32(p + 8, W.version[gid]);
+  p[12] = m[0];
+  wire_copy(p + 13, m + 1, m[0]);
+  return 13u + m[0];
+}
+
+/* the run of sorted positions [p, end) that share the key and ballot of position p; false if p does not start one */
+template <typename T>
+__device__ __forceinline__ bool wire_run(const WireEncodeArgs& A, uint32_t p, uint32_t& end) {
+  const T* recs = reinterpret_cast<const T*>(A.recs);
+  const uint32_t key = A.skey[p];
+  if (key == GPX_WIRE_NOKEY) return false;
+  const T x = recs[A.perm[p]];
+  if (p > 0 && A.skey[p - 1] == key) {
+    const T y = recs[A.perm[p - 1]];
+    if (y.bnum == x.bnum && y.bcoord == x.bcoord) return false;
+  }
+  end = p + 1;
+  while (end < A.n && A.skey[end] == key) {
+    const T y = recs[A.perm[end]];
+    if (y.bnum != x.bnum || y.bcoord != x.bcoord) break;
+    end++;
+  }
+  return true;
+}
+
+/* the run's distinct slots in ascending signed order (TreeMap / TreeSet); `last` = sorted position of the entry that
+ * wins a repeated slot (the last put).  Returns the number of distinct slots; with out != nullptr writes them. */
+template <typename T, bool WITH_REQ>
+__device__ __forceinline__ uint32_t wire_slots(const WireEncodeArgs& A, uint32_t p, uint32_t end, uint8_t* out) {
+  const T* recs = reinterpret_cast<const T*>(A.recs);
+  uint32_t n = 0;
+  bool have = false;
+  int32_t prev = 0;
+  for (;;) { /* selection: the smallest slot above the previous one, O(run^2) -- runs are a window's worth */
+    bool found = false;
+    int32_t best = 0;
+    uint32_t bi = 0;
+    for (uint32_t q = p; q < end; q++) {
+      const int32_t s = recs[A.perm[q]].slot;
+      if (have && s <= prev) continue;
+      if (!found || s <= best) { /* s == best: the same slot again, the later record wins */
+        best = s;
+        bi = q;
+        found = true;
+      }
+    }
+    if (!found) break;
+    if (out) {
+      uint8_t* o = out + (size_t)n * (WITH_REQ ? 12u : 4u);
+      ww_i32(o, best);
+      if (WITH_REQ) ww_i64(o + 4, reinterpret_cast<const gpx_accept_reply_rec*>(recs)[A.perm[bi]].req_id);
+    }
+    n++;
+    have = true;
+    prev = best;
+  }
+  return n;
+}
+
+/* one thread per sorted position; a position that starts a (lane, gid, ballot) run writes one BatchedAcceptReply
+ * (BatchedAcceptReply(AcceptReplyPacket) :53-58 takes the header of the first reply, addAcceptReply :179-184 adds
+ * slot -> requestID) addressed to the ballot's coordinator */
+__global__ void k_wire_enc_replies(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                                   const __grid_constant__ WireEncodeArgs A) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= A.n) return;
+  uint32_t end = 0;
+  const bool head = wire_run<gpx_accept_reply_rec>(A, p, end);
+  if (!A.emit) {
+    uint32_t bytes = 0;
+    if (head) {
+      const uint32_t gid = reinterpret_cast<const gpx_accept_reply_rec*>(A.recs)[A.perm[p]].gid;
+      bytes = 13u + W.name[(size_t)gid * GPX_NAME_BYTES] + 29u + 4u +
+              12u * wire_slots<gpx_accept_reply_rec, true>(A, p, end, nullptr);
+    }
+    A.cnt[p] = bytes;
+    A.cnt[A.n + p] = head ? 1u : 0u;
+    return;
+  }
+  if (!head) return;
+  const gpx_accept_reply_rec x = reinterpret_cast<const gpx_accept_reply_rec*>(A.recs)[A.perm[p]];
+  const MsetInfo* ms = group_ctx(S, x.gid).ms;
+  uint8_t* o = A.out + A.off[p];
+  uint32_t b = ww_header(o, GPX_PT_BATCHED_ACCEPT_REPLY, W, x.gid);
+  ww_i32(o + b, ms->nodes[GPX_WHO_ACC(x.who)]);
+  ww_i32(o + b + 4, x.bnum);
+  ww_i32(o + b + 8, x.bcoord);
+  ww_i32(o + b + 12, x.slot);
+  ww_i32(o + b + 16, x.max_cp);
+  ww_i64(o + b + 20, x.req_id);
+  o[b + 28] = 0; /* undigestRequest */
+  b += 29;
+  const uint32_t ns = wire_slots<gpx_accept_reply_rec, true>(A, p, end, o + b + 4);
+  ww_i32(o + b, (int32_t)ns);
+  b += 4 + 12u * ns;
+  gpx_wire_ref r;
+  r.off = A.off[p];
+  r.len = b;
+  r.gid = x.gid;
+  r.node = ms->nodes[GPX_WHO_DST(x.who)];
+  A.refs[A.off[A.n + p]] = r;
+}
+
+/* one thread per sorted position; a position that starts a (gid, ballot) run writes one BatchedCommit
+ * (PaxosPacketBatcher.fuseBatchedCommits :389-417, BatchedCommit.addCommit :113-121: medianCheckpointedSlot is the
+ * wrap-aware maximum, gpx_wire_fuse_commits' rule), stored once and indexed once per member node that no local lane
+ * serves */
+__global__ void k_wire_enc_decisions(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                                     const __grid_constant__ WireEncodeArgs A) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= A.n) return;
+  uint32_t end = 0;
+  const bool head = wire_run<gpx_decision_rec>(A, p, end);
+  const gpx_decision_rec* recs = reinterpret_cast<const gpx_decision_rec*>(A.recs);
+  const GroupCtx g = group_ctx(S, head ? recs[A.perm[p]].gid : 0u);
+  const uint32_t n_remote = head ? g.R - wire_popc(g.ms->lane_mask) : 0u;
+  if (!A.emit) {
+    uint32_t bytes = 0;
+    if (head) {
+      const uint32_t gid = recs[A.perm[p]].gid;
+      bytes = 13u + W.name[(size_t)gid * GPX_NAME_BYTES] + 12u + 4u +
+              4u * wire_slots<gpx_decision_rec, false>(A, p, end, nullptr) + 4u + 4u * g.R;
+    }
+    A.cnt[p] = bytes;
+    A.cnt[A.n + p] = n_remote;
+    return;
+  }
+  if (!head) return;
+  const gpx_decision_rec d = recs[A.perm[p]];
+  int32_t median = d.median_cp;
+  for (uint32_t q = p + 1; q < end; q++) {
+    const int32_t m = recs[A.perm[q]].median_cp;
+    if (jsub(m, median) > 0) median = m;
+  }
+  uint8_t* o = A.out + A.off[p];
+  uint32_t b = ww_header(o, GPX_PT_BATCHED_COMMIT, W, d.gid);
+  ww_i32(o + b, d.bnum);
+  ww_i32(o + b + 4, d.bcoord);
+  ww_i32(o + b + 8, median);
+  b += 12;
+  const uint32_t ns = wire_slots<gpx_decision_rec, false>(A, p, end, o + b + 4);
+  ww_i32(o + b, (int32_t)ns);
+  b += 4 + 4u * ns;
+  ww_i32(o + b, (int32_t)g.R);
+  b += 4;
+  for (uint32_t m = 0; m < g.R; m++, b += 4) ww_i32(o + b, g.ms->nodes[m]);
+  uint32_t ri = A.off[A.n + p];
+  for (uint32_t m = 0; m < g.R; m++) {
+    if (g.ms->lane_of_idx[m] != 0xffu) continue;
+    gpx_wire_ref r;
+    r.off = A.off[p];
+    r.len = b;
+    r.gid = d.gid;
+    r.node = g.ms->nodes[m];
+    A.refs[ri++] = r;
+  }
+}

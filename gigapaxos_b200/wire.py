@@ -225,3 +225,80 @@ def fuse_commits(decs: np.ndarray):
     k = L.gpx_wire_fuse_commits(C.c_uint32(len(d)), d.ctypes.data_as(C.c_void_p), rs.ctypes.data_as(C.c_void_p),
                                 rm.ctypes.data_as(C.c_void_p))
     return rs[:k].copy(), rm[:k].copy()
+
+
+# ---- phase-2 packets on the device (gpx_set_group_names, gpx_wire_decode_batch, gpx_wire_encode_*) -------------------
+def pack_packets(packets: Sequence[bytes]):
+    """(bytes arena, gpx_wire_ref[n]) for a list of packets"""
+    refs = np.zeros(len(packets), dtype=abi.wire_ref_dtype)
+    lens = np.array([len(p) for p in packets], dtype=np.uint64)
+    offs = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.uint64) if len(packets) else lens
+    refs["off"], refs["len"] = offs, lens
+    arena = np.frombuffer(b"".join(packets), dtype=np.uint8) if packets else np.zeros(0, np.uint8)
+    return np.ascontiguousarray(arena), refs
+
+
+def unpack_packets(arena: np.ndarray, refs: np.ndarray) -> list:
+    """[(gid, node, bytes)] of an encoder's output"""
+    return [(int(r["gid"]), int(r["node"]), bytes(arena[int(r["off"]): int(r["off"]) + int(r["len"])])) for r in refs]
+
+
+def set_group_names(engine, gids, names: Sequence[str]):
+    """gpx_set_group_names: gids[k] is called names[k] (ISO-8859-1) at the version it was created / loaded with"""
+    gids = np.ascontiguousarray(gids, dtype=np.uint32)
+    enc = [s.encode("iso-8859-1") for s in names]
+    lens = np.array([len(b) for b in enc], dtype=np.uint32)
+    offs = np.concatenate([[0], np.cumsum(lens)[:-1]]).astype(np.uint32) if len(enc) else lens
+    arena = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8)
+    L = engine.L
+    L.check(L.fn("set_group_names")(engine.handle, C.c_uint32(len(gids)), abi._ptr(gids), abi._ptr(arena),
+                                    abi._ptr(offs), abi._ptr(lens)))
+
+
+def decode_batch(engine, packets: Sequence[bytes]):
+    """gpx_wire_decode_batch -> (status[n], accepts, blob, replies, decisions); outputs grouped by gid"""
+    L = engine.L
+    arena, refs = pack_packets(packets)
+    n = len(packets)
+    status = np.zeros(max(n, 1), np.int32)
+    caps = [C.c_uint32(0), C.c_uint64(0), C.c_uint32(0), C.c_uint32(0)]
+    args = lambda acc, blob, rep, dec: (engine.handle, C.c_uint32(n), abi._ptr(arena), C.c_uint64(len(arena)),
+                                        abi._ptr(refs), abi._ptr(status), abi._ptr(acc), C.byref(caps[0]),
+                                        abi._ptr(blob), C.byref(caps[1]), abi._ptr(rep), C.byref(caps[2]),
+                                        abi._ptr(dec), C.byref(caps[3]))
+    rc = L.fn("wire_decode_batch")(*args(None, None, None, None))  # sizes first: an empty output is GPX_ERANGE
+    if rc not in (0, abi.GPX_ERANGE):
+        L.check(rc)
+    acc = np.zeros(max(caps[0].value, 1), abi.accept_dtype)
+    blob = np.zeros(max(caps[1].value, 16), np.uint8)
+    rep = np.zeros(max(caps[2].value, 1), abi.reply_dtype)
+    dec = np.zeros(max(caps[3].value, 1), abi.decision_dtype)
+    L.check(L.fn("wire_decode_batch")(*args(acc, blob, rep, dec)))
+    return (status[:n], acc[: caps[0].value], blob[: caps[1].value], rep[: caps[2].value], dec[: caps[3].value])
+
+
+def _encode(engine, name, recs, dtype):
+    L = engine.L
+    recs = np.ascontiguousarray(recs, dtype=dtype)
+    n = len(recs)
+    rstatus = np.zeros(max(n, 1), np.uint8)
+    nb, nr = C.c_uint64(0), C.c_uint32(0)
+    rc = L.fn(name)(engine.handle, C.c_uint32(n), abi._ptr(recs), abi._ptr(rstatus), None, C.byref(nb), None,
+                    C.byref(nr))
+    if rc not in (0, abi.GPX_ERANGE):
+        L.check(rc)
+    out = np.zeros(max(nb.value, 1), np.uint8)
+    refs = np.zeros(max(nr.value, 1), abi.wire_ref_dtype)
+    L.check(L.fn(name)(engine.handle, C.c_uint32(n), abi._ptr(recs), abi._ptr(rstatus), abi._ptr(out), C.byref(nb),
+                       abi._ptr(refs), C.byref(nr)))
+    return rstatus[:n], out[: nb.value], refs[: nr.value]
+
+
+def encode_replies(engine, replies: np.ndarray):
+    """gpx_wire_encode_replies over gpx_handle_accepts' output -> (rstatus[n], arena, refs)"""
+    return _encode(engine, "wire_encode_replies", replies, abi.reply_dtype)
+
+
+def encode_decisions(engine, decisions: np.ndarray):
+    """gpx_wire_encode_decisions over gpx_handle_accept_replies' output -> (rstatus[n], arena, refs)"""
+    return _encode(engine, "wire_encode_decisions", decisions, abi.decision_dtype)

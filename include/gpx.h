@@ -823,6 +823,88 @@ typedef struct gpx_kernel_times {
 int gpx_enable_kernel_timing(gpx_engine* e, int on);
 int gpx_get_kernel_times(gpx_engine* e, gpx_kernel_times* out, int reset);
 
+/* ---- phase-2 wire packets on the device: replicas of a group on other hosts ---------------------------------------
+ * A group's replicas on other machines exchange ACCEPT, ACCEPT_REPLY and DECISION as the reference's bytes:
+ * AcceptPacket, BatchedAcceptReply and BatchedCommit (layouts in gpx_wire.h).  These calls turn a batch of received
+ * packets into engine records and the engine's reply / decision records into packets, on the device; gpx_wire_* in
+ * gpx_wire.h is the host codec of one packet per call.
+ *
+ * Names.  A packet names its group by (paxosID, version) (PaxosPacket.java:459-476).  gpx_set_group_names gives gids
+ * their paxosID (names[name_off[k] .. + name_len[k]), ISO-8859-1 bytes, at most GPX_WIRE_MAX_ID) and stores the
+ * version the group was created or loaded with.  The first call allocates the name state: 128 B per gid, a 4-byte
+ * version and slot per gid, and an open-addressing table of 8-byte cells (at least 2 per gid); an engine that never
+ * calls it has none.  A name held by another live gid, the same name twice or the same gid twice in one call is
+ * GPX_EINVAL and changes nothing.  gpx_destroy_groups, gpx_pause_groups (for the groups that pause), gpx_create_groups
+ * and gpx_load_rows remove the names of the gids they touch: after a re-create or an unpause the caller sets the name
+ * again. */
+int gpx_set_group_names(gpx_engine* e, uint32_t n, const uint32_t* gids, const uint8_t* names, const uint32_t* name_off,
+                        const uint32_t* name_len);
+
+/* one packet in a byte arena: input of the decoder (gid and node ignored), output of the encoders, 16 B */
+typedef struct gpx_wire_ref {
+  uint32_t off;  /* byte offset in the arena */
+  uint32_t len;
+  uint32_t gid;  /* encoders: the packet's group */
+  int32_t node;  /* encoders: the destination node id */
+} gpx_wire_ref;
+
+/* per-packet status of gpx_wire_decode_batch (never fatal, gpx.h conventions) */
+enum {
+  GPX_WS_OK = 0,
+  GPX_WS_UNKNOWN_NAME = 1, /* no live gid has this paxosID: the host may unpause it (PaxosManager.getInstance), resubmit */
+  GPX_WS_VERSION = 2,      /* version differs from the group's: dropped (PISM :441-447) */
+  GPX_WS_MALFORMED = 3,    /* truncated, bad magic, idLen out of range, trailing bytes, negative length, a latched
+                            * request with latched requests of its own, an acceptor or coordinator outside the group */
+  GPX_WS_UNHANDLED = 4,    /* JSON packets and every type but ACCEPT / BATCHED_ACCEPT_REPLY / BATCHED_COMMIT: host */
+  GPX_WS_NOT_LOCAL = 5     /* no local lane is addressed (ACCEPT / commit: none is a member; reply: the ballot's
+                            * coordinator is not served by a local lane) */
+};
+
+/* Decode a batch of received packets.  bytes[0 .. n_bytes) is host memory, pkts[k] = {off, len} of packet k.
+ * Outputs, each grouped by gid and, within a group, in packet order and then in the packet's slot order -- the order
+ * gpx_handle_accepts, gpx_handle_accept_replies and gpx_handle_decisions require:
+ *   accepts[*n_accepts]    one gpx_accept_rec per ACCEPT, dst_mask = the group's local lanes; the request body goes to
+ *                          blob (payload_off into it, every body 16-byte aligned): the requestValue, or for a batched
+ *                          RequestPacket nreq x gpx_batch_ent then the values (gpx_propose's form).  Entry-lane bits of
+ *                          gpx_batch_ent.flags: the lane serving entryReplica, 0xf when it is not a local lane.
+ *   replies[*n_replies]    one gpx_accept_reply_rec per slot of a BATCHED_ACCEPT_REPLY: who = (member index of the
+ *                          acceptor, member index of the ballot's coordinator, 0); max_cp from the packet header.
+ *   decisions[*n_decisions] one gpx_decision_rec per slot of a BATCHED_COMMIT (flags GPX_F_DECISION, req_id 0: the
+ *                          value is the accept the acceptor holds).
+ *   status[n]              GPX_WS_* per packet; only GPX_WS_OK packets produce records.
+ * The four counts are in/out: capacities in, sizes out.  When an output is too small the call returns GPX_ERANGE,
+ * writes no record and reports the sizes needed.  Without gpx_set_group_names every packet is GPX_WS_UNKNOWN_NAME
+ * (or malformed / unhandled). */
+int gpx_wire_decode_batch(gpx_engine* e, uint32_t n, const uint8_t* bytes, uint64_t n_bytes, const gpx_wire_ref* pkts,
+                          int32_t* status, gpx_accept_rec* accepts, uint32_t* n_accepts, uint8_t* blob,
+                          uint64_t* blob_bytes, gpx_accept_reply_rec* replies, uint32_t* n_replies,
+                          gpx_decision_rec* decisions, uint32_t* n_decisions);
+
+/* per-record outcome of the encoders */
+enum {
+  GPX_WE_SENT = 0,    /* in a packet */
+  GPX_WE_VOID = 1,    /* a hole (GPX_F_VOID), or a group that is not live */
+  GPX_WE_LOCAL = 2,   /* loop-back: reply to a local lane / decision of a group with no remote member (SHORT_CIRCUIT_LOCAL) */
+  GPX_WE_NACK = 3,    /* not coalesced (PaxosPacketBatcher.allPositiveAcceptReplies :423-430): the host sends it alone */
+  GPX_WE_NO_NAME = 4  /* the group has no name (gpx_set_group_names) */
+};
+
+/* Encode accept replies, in the layout gpx_handle_accepts returns (record i * n_lanes + lane), the way one
+ * PaxosPacketBatcher per lane coalesces them: one BatchedAcceptReply per (lane, gid, ballot), its header taken from the
+ * first reply (BatchedAcceptReply(AcceptReplyPacket) :53-58), slot -> requestID of every reply added
+ * (addAcceptReply :179-184) and written in ascending slot order.  n = number of records (a multiple of n_lanes).
+ * out[0 .. *out_bytes) receives the packets, refs[*n_refs] one {off, len, gid, node = the coordinator} per packet, in
+ * (lane, gid) order; rstatus[n] GPX_WE_* per record.  *out_bytes and *n_refs are capacities in, sizes out;
+ * GPX_ERANGE as for the decoder. */
+int gpx_wire_encode_replies(gpx_engine* e, uint32_t n, const gpx_accept_reply_rec* replies, uint8_t* rstatus,
+                            uint8_t* out, uint64_t* out_bytes, gpx_wire_ref* refs, uint32_t* n_refs);
+/* Encode decisions, as gpx_handle_accept_replies returns them (any order): one BatchedCommit per (gid, ballot),
+ * medianCheckpointedSlot the wrap-aware maximum (gpx_wire_fuse_commits), slots ascending, the group's member node ids
+ * as its group list.  The packet is stored once and indexed once per member node that no local lane serves, in gid
+ * order. */
+int gpx_wire_encode_decisions(gpx_engine* e, uint32_t n, const gpx_decision_rec* decisions, uint8_t* rstatus,
+                              uint8_t* out, uint64_t* out_bytes, gpx_wire_ref* refs, uint32_t* n_refs);
+
 /* ---- helpers shared with the reference semantics ---------------------------------- */
 int32_t gpx_java_string_hash(const char* s, size_t len); /* String.hashCode() */
 /* PISM.roundRobinCoordinator :2251-2256 on sorted members */

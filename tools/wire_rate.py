@@ -1,0 +1,185 @@
+"""Packets/s and records/s of the phase-2 wire codec: the device calls (gpx_wire_decode_batch, gpx_wire_encode_*) at
+100 K and 1 M groups with one packet per group per round, and the host codec (gpx_wire_decode_accept /
+gpx_wire_encode_batched_commit, one packet per call) on one thread and on every host thread.
+
+Device numbers come two ways: the wall time of the C call, which includes the host->device and device->host copies
+and ends in a device synchronise; and the kernel time alone, the sum of the CUDA kernels torch.profiler records during
+a separate pass.  The host codec runs in a small C program built into a temporary directory and linked against
+libgpx.so, so no Python sits in its loop.  The card, its power limit and its SM clock are read in the same run.
+
+    python tools/wire_rate.py [--groups 100000 1000000] [--reps 5] [--out FILE.json]
+"""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+import tempfile
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+
+HOST_BENCH = r"""
+#include <pthread.h>
+#include <stdint.h>
+#include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
+#include <time.h>
+#include "gpx.h"
+#include "gpx_wire.h"
+static const uint8_t* g_bytes; static const gpx_wire_ref* g_refs; static uint32_t g_n; static int g_mode;
+static int32_t g_group[3] = {100, 101, 102};
+static void* run(void* arg) {
+  const uintptr_t t = (uintptr_t)arg; /* thread index << 8 | thread count */
+  uint32_t lo = (uint32_t)(((uint64_t)g_n * (t >> 8)) / (t & 0xff)), hi = (uint32_t)(((uint64_t)g_n * ((t >> 8) + 1)) / (t & 0xff));
+  gpx_wire_accept_view v; uint8_t out[512]; long sink = 0;
+  for (uint32_t i = lo; i < hi; i++) {
+    if (g_mode == 0) { if (gpx_wire_decode_accept(g_bytes + g_refs[i].off, g_refs[i].len, &v) == 0) sink += v.slot; }
+    else { int32_t s = (int32_t)i; sink += (long)gpx_wire_encode_batched_commit((const char*)g_bytes + g_refs[i].off + 13,
+             g_bytes[g_refs[i].off + 12], 0, 1, 100, 0, 1, &s, 3, g_group, out, sizeof out); }
+  }
+  return (void*)sink;
+}
+int main(int argc, char** argv) {
+  FILE* f = fopen(argv[1], "rb"); fseek(f, 0, SEEK_END); long sz = ftell(f); fseek(f, 0, SEEK_SET);
+  uint8_t* b = (uint8_t*)malloc(sz); if (fread(b, 1, sz, f) != (size_t)sz) return 1; fclose(f);
+  f = fopen(argv[2], "rb"); fseek(f, 0, SEEK_END); long rs = ftell(f); fseek(f, 0, SEEK_SET);
+  gpx_wire_ref* r = (gpx_wire_ref*)malloc(rs); if (fread(r, 1, rs, f) != (size_t)rs) return 1; fclose(f);
+  g_bytes = b; g_refs = r; g_n = (uint32_t)(rs / sizeof(gpx_wire_ref)); g_mode = atoi(argv[3]);
+  int T = atoi(argv[4]); pthread_t th[256]; struct timespec a, c;
+  clock_gettime(CLOCK_MONOTONIC, &a);
+  for (int t = 0; t < T; t++) pthread_create(&th[t], 0, run, (void*)(uintptr_t)(((uintptr_t)t << 8) | (uintptr_t)T));
+  for (int t = 0; t < T; t++) pthread_join(th[t], 0);
+  clock_gettime(CLOCK_MONOTONIC, &c);
+  printf("%.9f\n", (c.tv_sec - a.tv_sec) + 1e-9 * (c.tv_nsec - a.tv_nsec));
+  return 0;
+}
+"""
+
+
+def card_info():
+    q = "name,power.limit,clocks.sm,clocks.max.sm"
+    try:
+        out = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader", "-i", "0"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception as ex:  # pragma: no cover
+        out = f"unavailable: {ex}"
+    return dict(zip(q.split(","), [s.strip() for s in out.split(",")]))
+
+
+def kernel_ms(fn):
+    """sum of CUDA kernel time during one call of fn (torch.profiler, CUDA activities)"""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    tot = 0.0
+    for ev in prof.events():
+        if ev.device_type.name == "CUDA" and not ev.name.startswith("Memcpy") and not ev.name.startswith("Memset"):
+            tot += ev.device_time_total if hasattr(ev, "device_time_total") else ev.cuda_time_total
+    return tot / 1000.0
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--groups", type=int, nargs="+", default=[100_000, 1_000_000])
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--out", default=None)
+    args = ap.parse_args()
+    import gigapaxos_b200
+    from gigapaxos_b200 import abi, wire
+    from helpers import Engine, group_descs_fast, make_config
+
+    lib = gigapaxos_b200.load_library()
+    res = {"card": card_info(), "runs": []}
+    tmp = tempfile.mkdtemp(prefix="gpx_wire_rate_")
+    exe = os.path.join(tmp, "host_wire")
+    src = os.path.join(tmp, "host_wire.c")
+    open(src, "w").write(HOST_BENCH)
+    subprocess.check_call(["gcc", "-O2", "-o", exe, src, "-I", os.path.join(ROOT, "include"),
+                           os.path.join(ROOT, "gigapaxos_b200", "libgpx.so"), "-lpthread",
+                           "-Wl,-rpath," + os.path.join(ROOT, "gigapaxos_b200")])
+    for G in args.groups:
+        e = Engine(lib, make_config(lib, max_groups=G, n_lanes=1, lane_node=[101], window=8, max_batch_recs=G,
+                                    max_batch_payload=1 << 20, log_ring_bytes=1 << 20))
+        e.create_groups(group_descs_fast(G, members=(100, 101, 102)))
+        names = [f"NoopPaxosApp{i}" for i in range(G)]
+        gids = np.arange(G, dtype=np.uint32)
+        wire.set_group_names(e, gids, names)
+        # one ACCEPT per group (8-byte request value), as node 100 sends them to node 101
+        t0 = time.time()
+        pk = [wire.encode_accept(wire.Request(n, 0, i, b"12345678", entry_replica=100), 1, 0, 100, False, 0, 100)
+              for i, n in enumerate(names)]
+        arena, refs = wire.pack_packets(pk)
+        gen_s = time.time() - t0
+        status, acc, blob, _, _ = wire.decode_batch(e, pk)
+        assert (status == abi.WS_OK).all() and len(acc) == G
+        # replies in gpx_handle_accepts' layout, one per group, addressed to node 100; decisions one per group
+        rep = np.zeros(G, abi.reply_dtype)
+        rep["gid"], rep["slot"], rep["bnum"], rep["bcoord"], rep["who"] = gids, 1, 0, 100, abi.who(1, 0, 0)
+        dec = np.zeros(G, abi.decision_dtype)
+        dec["gid"], dec["slot"], dec["bnum"], dec["bcoord"], dec["flags"] = gids, 1, 0, 100, abi.F_DECISION
+        calls = {"decode_accepts": lambda: wire.decode_batch(e, pk),
+                 "encode_replies": lambda: wire.encode_replies(e, rep),
+                 "encode_decisions": lambda: wire.encode_decisions(e, dec)}
+        run = {"groups": G, "packet_gen_s": gen_s}
+        for k, fn in calls.items():
+            fn()  # warm-up
+            walls = []
+            for _ in range(args.reps):
+                t = time.perf_counter()
+                fn()  # ends in a device synchronise
+                walls.append(time.perf_counter() - t)
+            # the wall time includes the Python wrapper's own work; the bare C call is timed for decode below
+            kms = [kernel_ms(fn) for _ in range(args.reps)]
+            run[k] = {"packets": G, "wall_s_min": min(walls), "kernel_ms_min": min(kms),
+                      "packets_per_s_kernels": G / (min(kms) / 1000.0), "packets_per_s_wall": G / min(walls)}
+        # the bare C call (copies included, no Python record handling)
+        import ctypes as C
+        st = np.zeros(G, np.int32)
+        a_out = np.zeros(G, abi.accept_dtype)
+        b_out = np.zeros(len(blob) + 16, np.uint8)
+        z = np.zeros(1, np.uint8)
+        walls = []
+        for _ in range(args.reps + 1):
+            caps = [C.c_uint32(G), C.c_uint64(len(b_out)), C.c_uint32(0), C.c_uint32(0)]
+            t = time.perf_counter()
+            rc = lib.lib.gpx_wire_decode_batch(e.handle, C.c_uint32(G), abi._ptr(arena), C.c_uint64(len(arena)),
+                                                abi._ptr(refs), abi._ptr(st), abi._ptr(a_out), C.byref(caps[0]),
+                                                abi._ptr(b_out), C.byref(caps[1]), abi._ptr(z), C.byref(caps[2]),
+                                                abi._ptr(z), C.byref(caps[3]))
+            walls.append(time.perf_counter() - t)
+            assert rc == 0
+        run["decode_accepts"]["c_call_s_min"] = min(walls[1:])
+        run["decode_accepts"]["packets_per_s_c_call"] = G / min(walls[1:])
+        # host codec, one packet per call
+        arena.tofile(os.path.join(tmp, "bytes"))
+        refs.tofile(os.path.join(tmp, "refs"))
+        T = os.cpu_count() or 1
+        for mode, name in ((0, "host_decode_accept"), (1, "host_encode_batched_commit")):
+            for threads in (1, T):
+                s = min(float(subprocess.check_output([exe, os.path.join(tmp, "bytes"), os.path.join(tmp, "refs"),
+                                                       str(mode), str(threads)]).decode())
+                        for _ in range(args.reps))
+                run[f"{name}_{threads}t"] = {"packets": G, "s_min": s, "packets_per_s": G / s, "threads": threads}
+        res["runs"].append(run)
+        e.close()
+    res["card_after"] = card_info()
+    line = json.dumps(res)
+    print(line)
+    if args.out:
+        with open(args.out, "w") as f:
+            f.write(line + "\n")
+
+
+if __name__ == "__main__":
+    main()
