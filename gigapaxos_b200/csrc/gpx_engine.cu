@@ -121,8 +121,12 @@ struct gpx_engine {
   bool names_on = false;
   std::vector<uint8_t> h_named; /* [G] the gid has a table entry */
   uint64_t names_live = 0, names_used = 0; /* entries; cells taken since the last rebuild (live + removed) */
-  void* d_wire = nullptr;
+  void* d_wire = nullptr;    /* the kernels' scratch: counters, offsets, sort keys, CUB temporaries */
   size_t wire_bytes = 0;
+  void* d_wire_io = nullptr; /* the host-buffer forms' staged inputs and outputs */
+  size_t wire_io_bytes = 0;
+  cudaEvent_t ev_wire = nullptr; /* the last wire call's work on its stream: the next call, on any stream, waits for it */
+  bool wire_pending = false;
 
   template <typename T>
   int dalloc(T** p, size_t n) {
@@ -332,6 +336,8 @@ void gpx_engine_destroy(gpx_engine* e) {
   for (void* p : e->allocs) cudaFree(p);
   if (e->d_misc) cudaFree(e->d_misc);
   if (e->d_wire) cudaFree(e->d_wire);
+  if (e->d_wire_io) cudaFree(e->d_wire_io);
+  if (e->ev_wire) cudaEventDestroy(e->ev_wire);
   if (e->h_ctl) cudaFreeHost(e->h_ctl);
   for (auto& ps : e->pipe) {
     if (ps.h_ctl) cudaFreeHost(ps.h_ctl);

@@ -214,7 +214,7 @@ struct WireDecodeArgs {
   uint32_t* cnt;  /* [WD_NCNT][n]: pass 0 writes the packet's output sizes (blob bytes padded to 16) */
   uint32_t* off;  /* [WD_NCNT][n]: pass 1 reads their exclusive prefix sums */
   int32_t* status;
-  /* pass 1: staging in packet order, and the sort keys (gids) beside it */
+  /* pass 1: records staged in packet order, and the sort keys (gids) beside them; the blob is the output itself */
   gpx_accept_rec* acc;
   uint8_t* blob;
   gpx_accept_reply_rec* rep;
@@ -495,6 +495,7 @@ struct WireEncodeArgs {
   uint8_t* out;
   gpx_wire_ref* refs;
   int emit;
+  const uint32_t* n_ptr; /* decisions: records [*n_ptr, n) are not read and get no rstatus (device count); null = n */
 };
 
 /* one thread per record: what happens to it and its sort key */
@@ -518,6 +519,10 @@ __global__ void k_wire_enc_keys_decisions(const __grid_constant__ DevState S, co
                                           const __grid_constant__ WireEncodeArgs A) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= A.n) return;
+  if (A.n_ptr && i >= *A.n_ptr) { /* past the device count: sorts last, never encoded */
+    A.key[i] = GPX_WIRE_NOKEY;
+    return;
+  }
   const gpx_decision_rec d = reinterpret_cast<const gpx_decision_rec*>(A.recs)[i];
   uint8_t st = GPX_WE_SENT;
   const GroupCtx g = group_ctx(S, d.gid);

@@ -4,6 +4,7 @@ BatchedCommit.java:184-252, SQLPaxosLogger.java:1000-1003)."""
 from __future__ import annotations
 
 import ctypes as C
+from collections import namedtuple
 from dataclasses import dataclass, field
 from typing import Optional, Sequence
 
@@ -302,3 +303,107 @@ def encode_replies(engine, replies: np.ndarray):
 def encode_decisions(engine, decisions: np.ndarray):
     """gpx_wire_encode_decisions over gpx_handle_accept_replies' output -> (rstatus[n], arena, refs)"""
     return _encode(engine, "wire_encode_decisions", decisions, abi.decision_dtype)
+
+
+# ---- the device-buffer forms (gpx_wire_*_device) over torch CUDA tensors ---------------------------------------------
+# Records travel as uint8 tensors of shape [k, record bytes] (48 for accepts, 32 for replies and decisions, 16 for
+# gpx_wire_ref); to_records() reads one as a numpy structured array.
+DecodeOut = namedtuple("DecodeOut", "status accepts blob replies decisions sizes")
+EncodeOut = namedtuple("EncodeOut", "rstatus out refs sizes")
+
+
+def _dptr(t):
+    return C.c_void_p(t.data_ptr()) if t is not None and t.numel() else None
+
+
+def stream_handle(stream=None):
+    """the stream handle a device-form call runs on: `stream`, else torch's current stream.  torch's default stream is
+    CUDA's legacy stream; it is handed over as cudaStreamLegacy, because NULL would mean the engine's own stream."""
+    import torch
+    h = (stream if stream is not None else torch.cuda.current_stream()).cuda_stream
+    return C.c_void_p(h or 1)
+
+
+def _on(stream):
+    """allocate the outputs on the stream the call runs on"""
+    import contextlib
+    import torch
+    return torch.cuda.stream(stream) if stream is not None else contextlib.nullcontext()
+
+
+def device_packets(packets: Sequence[bytes], device="cuda"):
+    """the device-tensor form of a packet arena (pack_packets): (bytes uint8 [n_bytes], refs uint8 [n, 16])"""
+    import torch
+    arena, refs = pack_packets(packets)
+    return (torch.from_numpy(arena.copy()).to(device),
+            torch.from_numpy(refs.view(np.uint8).reshape(len(refs), 16)).to(device))
+
+
+def to_records(t, dtype) -> np.ndarray:
+    """a record tensor of the device forms as a numpy structured array (copied to the host)"""
+    return np.ascontiguousarray(t.detach().cpu().numpy()).reshape(-1).view(dtype)
+
+
+def decode_batch_device(engine, arena, refs, caps, stream=None) -> DecodeOut:
+    """gpx_wire_decode_batch_device: the packets refs[n] (gpx_wire_ref rows) of the byte arena `arena`, both CUDA tensors
+    (device_packets).  The outputs are allocated with caps = (accepts, blob bytes, replies, decisions); when one is too
+    small (GPX_ERANGE) they are allocated again at the sizes the call reports and the call is repeated.  Returns views:
+    status int32 [n], accepts [na, 48], blob [bytes], replies [nr, 32], decisions [nd, 32] -- grouped by gid, ready for
+    gpx_accepts_device (n_chunks = 0), gpx_replies_device and gpx_decisions_device -- and the four host sizes, which a
+    caller can hand to the next batch as its caps."""
+    import torch
+    n, dev = int(refs.shape[0]), refs.device
+    L, st = engine.L, stream_handle(stream)
+    caps = [int(c) for c in caps]
+    with _on(stream):
+        status = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+        for _ in range(2):
+            acc = torch.empty((max(caps[0], 1), 48), dtype=torch.uint8, device=dev)
+            blob = torch.empty(max(caps[1], 16), dtype=torch.uint8, device=dev)
+            rep = torch.empty((max(caps[2], 1), 32), dtype=torch.uint8, device=dev)
+            dec = torch.empty((max(caps[3], 1), 32), dtype=torch.uint8, device=dev)
+            sz = [C.c_uint32(caps[0]), C.c_uint64(caps[1]), C.c_uint32(caps[2]), C.c_uint32(caps[3])]
+            rc = L.fn("wire_decode_batch_device")(engine.handle, C.c_uint32(n), _dptr(arena), C.c_uint64(arena.numel()),
+                                                  _dptr(refs), _dptr(status), _dptr(acc), C.byref(sz[0]), _dptr(blob),
+                                                  C.byref(sz[1]), _dptr(rep), C.byref(sz[2]), _dptr(dec),
+                                                  C.byref(sz[3]), st)
+            caps = [s.value for s in sz]
+            if rc != abi.GPX_ERANGE:
+                break
+    L.check(rc)
+    return DecodeOut(status[:n], acc[: caps[0]], blob[: caps[1]], rep[: caps[2]], dec[: caps[3]], tuple(caps))
+
+
+def _encode_device(engine, name, lead, n, dev, caps, stream) -> EncodeOut:
+    import torch
+    L, st = engine.L, stream_handle(stream)
+    caps = [int(c) for c in caps]
+    with _on(stream):
+        rstatus = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+        for _ in range(2):
+            out = torch.empty(max(caps[0], 1), dtype=torch.uint8, device=dev)
+            refs = torch.empty((max(caps[1], 1), 16), dtype=torch.uint8, device=dev)
+            nb, nr = C.c_uint64(caps[0]), C.c_uint32(caps[1])
+            rc = L.fn(name)(engine.handle, *lead, _dptr(rstatus), _dptr(out), C.byref(nb), _dptr(refs), C.byref(nr), st)
+            caps = [nb.value, nr.value]
+            if rc != abi.GPX_ERANGE:
+                break
+    L.check(rc)
+    return EncodeOut(rstatus[:n], out[: caps[0]], refs[: caps[1]], tuple(caps))
+
+
+def encode_replies_device(engine, replies, n: int, caps, stream=None) -> EncodeOut:
+    """gpx_wire_encode_replies_device over the first n records of `replies` (a CUDA tensor in gpx_accepts_device's
+    layout, n = n_lanes x the ACCEPTs handled).  caps = (packet bytes, packets); GPX_ERANGE as in decode_batch_device.
+    Returns rstatus uint8 [n], the packet arena, refs [k, 16] and the two host sizes."""
+    return _encode_device(engine, "wire_encode_replies_device", (C.c_uint32(n), _dptr(replies)), n,
+                          replies.device, caps, stream)
+
+
+def encode_decisions_device(engine, decisions, n_ptr: Optional[int], n_max: int, caps, stream=None) -> EncodeOut:
+    """gpx_wire_encode_decisions_device: the record count is read on the device at address n_ptr (e.g. the
+    n_decisions word of the gpx_dev_ctl that gpx_replies_device counted into), at most n_max; None = n_max.
+    rstatus [n_max] is written only below that count."""
+    return _encode_device(engine, "wire_encode_decisions_device",
+                          (_dptr(decisions), C.c_void_p(n_ptr) if n_ptr else None, C.c_uint32(n_max)), n_max,
+                          decisions.device, caps, stream)

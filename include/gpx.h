@@ -905,6 +905,37 @@ int gpx_wire_encode_replies(gpx_engine* e, uint32_t n, const gpx_accept_reply_re
 int gpx_wire_encode_decisions(gpx_engine* e, uint32_t n, const gpx_decision_rec* decisions, uint8_t* rstatus,
                               uint8_t* out, uint64_t* out_bytes, gpx_wire_ref* refs, uint32_t* n_refs);
 
+/* Device-buffer forms of the three calls above: a remote replica's packets go from bytes to records, through the
+ * device phase calls (gpx_accepts_device, gpx_replies_device, gpx_decisions_device) and back to packets without
+ * leaving HBM.  They are the implementation: the host-buffer forms stage their inputs on the device, run them into
+ * engine-owned buffers and copy the outputs out.  The wire calls of one engine share its scratch, so a call on one
+ * stream waits for the previous call's work on another. */
+
+/* gpx_wire_decode_batch on device buffers.  bytes, pkts, status, accepts, blob, replies, decisions are device
+ * pointers; the four counts are HOST pointers, capacities in / sizes out, with GPX_ERANGE exactly as in the host form
+ * (sizes reported, no record written).  Stream-ordered on `stream` (NULL = the engine's stream); the call returns
+ * after the one synchronisation that reads the totals.  Outputs, order and statuses are byte-identical to
+ * gpx_wire_decode_batch, and feed gpx_accepts_device (n_chunks = 0), gpx_replies_device and gpx_decisions_device
+ * as they are. */
+int gpx_wire_decode_batch_device(gpx_engine* e, uint32_t n, const uint8_t* bytes, uint64_t n_bytes,
+                                 const gpx_wire_ref* pkts, int32_t* status, gpx_accept_rec* accepts,
+                                 uint32_t* n_accepts, uint8_t* blob, uint64_t* blob_bytes,
+                                 gpx_accept_reply_rec* replies, uint32_t* n_replies,
+                                 gpx_decision_rec* decisions, uint32_t* n_decisions, void* stream);
+
+/* gpx_wire_encode_replies on device buffers (replies, rstatus, out, refs device; out_bytes / n_refs host,
+ * capacities in / sizes out).  n = n_lanes x the ACCEPTs handled, which the caller always knows on the host. */
+int gpx_wire_encode_replies_device(gpx_engine* e, uint32_t n, const gpx_accept_reply_rec* replies, uint8_t* rstatus,
+                                   uint8_t* out, uint64_t* out_bytes, gpx_wire_ref* refs, uint32_t* n_refs,
+                                   void* stream);
+
+/* gpx_wire_encode_decisions on device buffers.  The number of records is read on the device from *n_ptr (device;
+ * e.g. &ctl->n_decisions after gpx_replies_device), at most n_max; NULL n_ptr = n_max.  Records at and beyond
+ * *n_ptr are neither read as input nor given an rstatus. */
+int gpx_wire_encode_decisions_device(gpx_engine* e, const gpx_decision_rec* decisions, const uint32_t* n_ptr,
+                                     uint32_t n_max, uint8_t* rstatus, uint8_t* out, uint64_t* out_bytes,
+                                     gpx_wire_ref* refs, uint32_t* n_refs, void* stream);
+
 /* ---- helpers shared with the reference semantics ---------------------------------- */
 int32_t gpx_java_string_hash(const char* s, size_t len); /* String.hashCode() */
 /* PISM.roundRobinCoordinator :2251-2256 on sorted members */

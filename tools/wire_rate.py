@@ -7,6 +7,10 @@ and ends in a device synchronise; and the kernel time alone, the sum of the CUDA
 a separate pass.  The host codec runs in a small C program built into a temporary directory and linked against
 libgpx.so, so no Python sits in its loop.  The card, its power limit and its SM clock are read in the same run.
 
+`acceptor_chain` times an acceptor's whole phase-2 path (decode the ACCEPTs, handle them, encode the replies) two ways:
+through the device-buffer forms with one upload of the packets and one download of the replies, and through the
+host-buffer calls (see acceptor_chain).
+
     python tools/wire_rate.py [--groups 100000 1000000] [--reps 5] [--out FILE.json]
 """
 from __future__ import annotations
@@ -87,6 +91,129 @@ def kernel_ms(fn):
         if ev.device_type.name == "CUDA" and not ev.name.startswith("Memcpy") and not ev.name.startswith("Memset"):
             tot += ev.device_time_total if hasattr(ev, "device_time_total") else ev.cuda_time_total
     return tot / 1000.0
+
+
+def with_round(arena, refs, slot, bnum):
+    """the ACCEPT packets of `arena` with their slot and ballot number rewritten (big-endian, in the 22-byte trailer
+    slot, bnum, bcoord, recovery, median, noCoalesce, sender of AcceptPacket)"""
+    a = arena.copy()
+    end = refs["off"].astype(np.int64) + refs["len"].astype(np.int64)
+    for at, v in ((end - 22, slot), (end - 18, bnum)):
+        for k in range(4):
+            a[at + k] = (v >> (24 - 8 * k)) & 0xFF
+    return a
+
+
+def acceptor_chain(lib, G, arena, refs, reps):
+    """An acceptor's whole phase-2 path for one ACCEPT per group, addressed to a node-101 engine: decode, handle, encode
+    the replies.  Every repetition is a fresh round (slot r, ballot (1, 100), above every group's initial ballot) made
+    before timing, so each does the same protocol work; `reps` + 2 rounds must fit the window of 8.
+
+    * device leg: pinned host arena -> one upload -> gpx_wire_decode_batch_device -> gpx_accepts_device ->
+      gpx_wire_encode_replies_device -> one download of the reply packets;
+    * host-buffer leg: gpx_wire_decode_batch -> gpx_handle_accepts -> gpx_wire_encode_replies as bare C calls, on a
+      second engine in the same state.
+    The legs alternate; wall time to a device synchronise, best of `reps`, then the kernel-only sum of one more round
+    of each leg under torch.profiler."""
+    import ctypes as C
+
+    import torch
+
+    from gigapaxos_b200 import abi, wire
+    from helpers import Engine, group_descs_fast, make_config
+
+    assert reps + 2 <= 8, "every round takes a slot of the window"
+    ring = 1 << 16
+    while ring < 2 * (96 + 64 * G):
+        ring <<= 1
+    engines = []
+    for _ in range(2):
+        e = Engine(lib, make_config(lib, max_groups=G, n_lanes=1, lane_node=[101], window=8, max_batch_recs=G,
+                                    max_batch_payload=16 * G, log_ring_bytes=ring))
+        e.create_groups(group_descs_fast(G, members=(100, 101, 102)))
+        wire.set_group_names(e, np.arange(G, dtype=np.uint32), [f"NoopPaxosApp{i}" for i in range(G)])
+        engines.append(e)
+    ed, eh = engines
+    rounds = [with_round(arena, refs, r, 1) for r in range(reps + 2)]
+    fn = lib.fn
+    st = wire.stream_handle()
+    ptr = lambda t: C.c_void_p(t.data_ptr())  # noqa: E731
+    # device leg: pinned staging and device buffers made once
+    h_refs = torch.from_numpy(refs.view(np.uint8).reshape(G, 16).copy()).pin_memory()
+    h_arenas = [torch.from_numpy(a).pin_memory() for a in rounds]
+    d_arena = torch.empty(len(arena), dtype=torch.uint8, device="cuda")
+    d_refs = torch.empty((G, 16), dtype=torch.uint8, device="cuda")
+    ctl = torch.zeros(8, dtype=torch.int32, device="cuda")
+    d_rep = torch.empty((G, 32), dtype=torch.uint8, device="cuda")
+    d_extra = torch.empty((4096, 24), dtype=torch.uint8, device="cuda")
+    h_out = torch.empty(128 * G, dtype=torch.uint8).pin_memory()
+    h_out_refs = torch.empty((G, 16), dtype=torch.uint8).pin_memory()
+    caps = {"dec": (G, 16 * G, 1, 1), "enc": (128 * G, G)}
+
+    def device_leg(r):
+        d_arena.copy_(h_arenas[r], non_blocking=True)
+        d_refs.copy_(h_refs, non_blocking=True)
+        d = wire.decode_batch_device(ed, d_arena, d_refs, caps["dec"])
+        ctl.zero_()
+        na = d.sizes[0]
+        lib.check(fn("accepts_device")(ed.handle, ptr(d.accepts), C.c_uint32(na), ptr(d.blob), C.c_uint64(d.sizes[1]),
+                                       C.c_uint32(0), None, None, ptr(d_rep), ptr(d_extra), C.c_uint32(4096), ptr(ctl),
+                                       st))
+        enc = wire.encode_replies_device(ed, d_rep, na, caps["enc"])
+        caps["dec"], caps["enc"] = d.sizes, enc.sizes
+        h_out[: enc.sizes[0]].copy_(enc.out, non_blocking=True)
+        h_out_refs[: enc.sizes[1]].copy_(enc.refs, non_blocking=True)
+        torch.cuda.synchronize()
+        return enc.sizes
+
+    # host-buffer leg: numpy buffers made once
+    status = np.zeros(G, np.int32)
+    acc = np.zeros(G, abi.accept_dtype)
+    blob = np.zeros(16 * G, np.uint8)
+    z = np.zeros(1, abi.reply_dtype)
+    rep = np.zeros(G, abi.reply_dtype)
+    extra = np.zeros(4096, abi.exec_dtype)
+    rst = np.zeros(G, np.uint8)
+    out = np.zeros(128 * G, np.uint8)
+    out_refs = np.zeros(G, abi.wire_ref_dtype)
+
+    def host_leg(r):
+        a = rounds[r]
+        sz = [C.c_uint32(G), C.c_uint64(len(blob)), C.c_uint32(0), C.c_uint32(0)]
+        lib.check(fn("wire_decode_batch")(eh.handle, C.c_uint32(G), abi._ptr(a), C.c_uint64(len(a)), abi._ptr(refs),
+                                          abi._ptr(status), abi._ptr(acc), C.byref(sz[0]), abi._ptr(blob),
+                                          C.byref(sz[1]), abi._ptr(z), C.byref(sz[2]), abi._ptr(z), C.byref(sz[3])))
+        nx = C.c_uint32(0)
+        lib.check(fn("handle_accepts")(eh.handle, sz[0], abi._ptr(acc), abi._ptr(blob), C.c_uint64(sz[1].value),
+                                       abi._ptr(rep), abi._ptr(extra), C.c_uint32(len(extra)), C.byref(nx)))
+        nb, nr = C.c_uint64(len(out)), C.c_uint32(G)
+        lib.check(fn("wire_encode_replies")(eh.handle, sz[0], abi._ptr(rep), abi._ptr(rst), abi._ptr(out),
+                                            C.byref(nb), abi._ptr(out_refs), C.byref(nr)))
+        return nb.value, nr.value
+
+    walls = {"device": [], "host_buffer": []}
+    sizes = {}
+    for r in range(reps + 1):  # round 0 warms both legs up
+        for leg, run in (("device", device_leg), ("host_buffer", host_leg)):
+            t = time.perf_counter()
+            sizes[leg] = run(r)
+            if r:
+                walls[leg].append(time.perf_counter() - t)
+    # both legs wrote the same reply packets
+    assert tuple(sizes["device"]) == tuple(sizes["host_buffer"])
+    nb, nr = sizes["device"]
+    assert nr == G, "every ACCEPT is accepted and its reply is encoded"
+    assert bytes(h_out[:nb].numpy()) == out[:nb].tobytes() and bytes(h_out_refs[:nr].numpy()) == out_refs[:nr].tobytes()
+    res = {"packets": G, "reply_packets": int(nr), "reply_bytes": int(nb), "upload_bytes": int(len(arena) + 16 * G),
+           "log_ring_bytes": ring}
+    for leg, run in (("device", device_leg), ("host_buffer", host_leg)):
+        w = min(walls[leg])
+        res[leg] = {"wall_s_min": w, "packets_per_s_wall": G / w,
+                    "kernel_ms": kernel_ms(lambda: run(reps + 1))}
+        res[leg]["packets_per_s_kernels"] = G / (res[leg]["kernel_ms"] / 1000.0)
+    for e in engines:
+        e.close()
+    return res
 
 
 def main():
@@ -171,8 +298,9 @@ def main():
                                                        str(mode), str(threads)]).decode())
                         for _ in range(args.reps))
                 run[f"{name}_{threads}t"] = {"packets": G, "s_min": s, "packets_per_s": G / s, "threads": threads}
-        res["runs"].append(run)
         e.close()
+        run["acceptor_chain"] = acceptor_chain(lib, G, arena, refs, args.reps)
+        res["runs"].append(run)
     res["card_after"] = card_info()
     line = json.dumps(res)
     print(line)
