@@ -50,6 +50,13 @@ wire_ref_dtype = np.dtype([("off", "<u4"), ("len", "<u4"), ("gid", "<u4"), ("nod
 # per-packet status of gpx_wire_decode_batch, per-record outcome of gpx_wire_encode_*
 WS_OK, WS_UNKNOWN_NAME, WS_VERSION, WS_MALFORMED, WS_UNHANDLED, WS_NOT_LOCAL = 0, 1, 2, 3, 4, 5
 WE_SENT, WE_VOID, WE_LOCAL, WE_NACK, WE_NO_NAME = 0, 1, 2, 3, 4
+WE_BAD_HEAD = 5  # gpx_wire_encode_accepts_device: the ACCEPT's head request is out of range or of another group
+# gpx_wire_req_meta: the RequestPacket wire fields a gpx_request_rec does not keep (gpx_wire_decode_requests_device)
+RM_RETURN_VALUE, RM_BROADCASTED = 1, 2
+req_meta_dtype = np.dtype([("client_ip", "u1", (4,)), ("client_port", "<u2"), ("listen_port", "<u2"),
+                           ("listen_ip", "u1", (4,)), ("forward_count", "<i4"), ("entry_time", "<i8"),
+                           ("flags", "<u4"), ("pad", "<u4")])
+assert req_meta_dtype.itemsize == 32
 accepted_pvalue_dtype = np.dtype([("slot", "<i4"), ("bnum", "<i4"), ("bcoord", "<i4"), ("frame_ref", "<u4"),
                                   ("req_id", "<i8"), ("payload_len", "<u4"), ("flags", "<u4")])
 prepare_reply_dtype = np.dtype([("gid", "<u4"), ("first_slot", "<i4"), ("bnum", "<i4"), ("bcoord", "<i4"), ("who", "<u4"),

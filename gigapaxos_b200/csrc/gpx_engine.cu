@@ -550,7 +550,8 @@ static inline void log_flip(gpx_engine* e) { e->S.lp ^= 1u; }
 
 /* ---- kernel launch helpers (device pointers) ------------------------------------- */
 static int launch_propose(gpx_engine* e, const gpx_request_rec* d_reqs, const uint8_t* d_payload,
-                          uint64_t payload_al, uint32_t n, int32_t* d_status, cudaStream_t st) {
+                          uint64_t payload_al, uint32_t n, int32_t* d_status, cudaStream_t st,
+                          uint32_t* d_head = nullptr) {
   ProposeArgs A;
   A.reqs = d_reqs;
   A.n = n;
@@ -560,7 +561,7 @@ static int launch_propose(gpx_engine* e, const gpx_request_rec* d_reqs, const ui
   A.copy_tab = e->d_copy_tab;
   A.copy_dst = e->d_copy_dst;
   A.ctl = e->d_ctl;
-  k_propose<<<cdiv(n, GPX_BLOCK), GPX_BLOCK, 0, st>>>(e->S, A, e->d_mark);
+  k_propose<<<cdiv(n, GPX_BLOCK), GPX_BLOCK, 0, st>>>(e->S, A, e->d_mark, d_head);
   k_build_blobs<<<cdiv(n, GPX_BLOCK), GPX_BLOCK, 0, st>>>(A, d_payload, e->d_blob1, e->d_mark);
   CK(cudaGetLastError());
   return GPX_OK;
@@ -1220,6 +1221,18 @@ int gpx_propose_device(gpx_engine* e, const gpx_request_rec* reqs, const uint8_t
   ScratchSwap sw(e, ctl, out_accepts, nullptr, 0);
   return launch_propose(e, reqs, payload, (payload_bytes + 15) & ~15ull, n, status,
                         stream ? (cudaStream_t)stream : e->stream);
+}
+int gpx_propose_device_heads(gpx_engine* e, const gpx_request_rec* reqs, const uint8_t* payload, uint64_t payload_bytes,
+                             uint32_t n, int32_t* status, gpx_accept_rec* out_accepts, uint32_t* out_head,
+                             gpx_dev_ctl* ctl, void* stream) {
+  if (!e || !ctl) return fail(GPX_EINVAL, "null argument");
+  if (n == 0) return GPX_OK;
+  if (!reqs || !status || !out_accepts || !out_head || (!payload && payload_bytes)) return fail(GPX_EINVAL, "null argument");
+  int rc = check_batch(e, n, payload_bytes);
+  if (rc) return rc;
+  ScratchSwap sw(e, ctl, out_accepts, nullptr, 0);
+  return launch_propose(e, reqs, payload, (payload_bytes + 15) & ~15ull, n, status,
+                        stream ? (cudaStream_t)stream : e->stream, out_head);
 }
 
 int gpx_route_device(gpx_engine* e, uint32_t kind, const void* recs, const uint32_t* n_ptr, uint32_t n_max,

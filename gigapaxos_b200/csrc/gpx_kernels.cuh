@@ -134,9 +134,10 @@ __device__ __forceinline__ uint32_t batch_end(const DevState& S, const gpx_reque
 
 /* `indexed`: the ACCEPT of the batch that starts at request k is written to A.accepts[k] (k_round) instead of
  * the compacted position base+emitted (k_propose).  Every request of the run gets its GPX_MK_* mark (GPX_MK_SLOW
- * kept when indexed). */
+ * kept when indexed).  head (k_propose, may be null): head[base + e] = the request that starts compacted ACCEPT e,
+ * 0xffffffff for a VOID filler. */
 __device__ __noinline__ void propose_run(const DevState& S, const ProposeArgs& A, uint32_t i, uint32_t run_end,
-                                         uint32_t nb, uint32_t base, unsigned int* s_ctr, uint8_t* mark,
+                                         uint32_t nb, uint32_t base, unsigned int* s_ctr, uint8_t* mark, uint32_t* head,
                                          bool indexed = false) {
   const uint8_t mk0 = indexed ? (uint8_t)GPX_MK_SLOW : (uint8_t)0;
   const gpx_request_rec* reqs = A.reqs;
@@ -270,6 +271,7 @@ __device__ __noinline__ void propose_run(const DevState& S, const ProposeArgs& A
       dst[0] = src[0];
       dst[1] = src[1];
       dst[2] = src[2];
+      if (head) head[base + emitted] = k;
       emitted++;
       A.status[k] = slot;
       mark[k] = mk0 | (uint8_t)GPX_MK_HEAD;
@@ -300,12 +302,15 @@ __device__ __noinline__ void propose_run(const DevState& S, const ProposeArgs& A
     dst[0] = src[0];
     dst[1] = src[1];
     dst[2] = src[2];
+    if (head) head[base + emitted] = 0xffffffffu;
   }
 }
 
-/* mark: the engine's [n] GPX_MK_* marks (the status buffer may be the caller's), read by k_build_blobs */
+/* mark: the engine's [n] GPX_MK_* marks (the status buffer may be the caller's), read by k_build_blobs.  heads (may be
+ * null): the request index that starts each compacted ACCEPT (propose_run) */
 __global__ void __launch_bounds__(GPX_BLOCK) k_propose(const __grid_constant__ DevState S,
-                                                       const __grid_constant__ ProposeArgs A, uint8_t* mark) {
+                                                       const __grid_constant__ ProposeArgs A, uint8_t* mark,
+                                                       uint32_t* heads) {
   __shared__ unsigned int s_ctr[C_NCTR];
   __shared__ uint32_t s_scan[GPX_BLOCK / 32 + 1];
   if (threadIdx.x < C_NCTR) s_ctr[threadIdx.x] = 0;
@@ -391,11 +396,12 @@ __global__ void __launch_bounds__(GPX_BLOCK) k_propose(const __grid_constant__ D
       dst[2] = src[2];
       A.status[i] = slot;
       mark[i] = (uint8_t)GPX_MK_HEAD;
+      if (heads) heads[base] = i;
       S.coord_row[ri] = Ce;
       atomicAdd(&s_ctr[C_PROPOSALS], 1u);
       atomicAdd(&s_ctr[C_REQS_BATCHED], 1u);
     } else
-      propose_run(S, A, i, run_end, nb, base, s_ctr, mark);
+      propose_run(S, A, i, run_end, nb, base, s_ctr, mark, heads);
   }
   if (i == 0) atomicAdd(&s_ctr[C_KERNEL_LAUNCHES], 1u);
   flush_counters(S, s_ctr);

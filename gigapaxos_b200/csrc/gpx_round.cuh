@@ -180,7 +180,7 @@ __device__ __forceinline__ uint32_t round_propose(const DevState& S, const Round
     k = batch_end(S, reqs, n, k, gid);
     nb++;
   }
-  propose_run(S, RA.P, i, k, nb, i, s_ctr, RA.mark, true);
+  propose_run(S, RA.P, i, k, nb, i, s_ctr, RA.mark, nullptr, true);
   return k;
 }
 

@@ -93,16 +93,45 @@ struct WireReq {
   uint32_t val_at, val_len;
   int32_t n_batched;
 };
-__device__ __forceinline__ void wr_request_body(WireRd& r, WireReq& q) {
+/* the fields the engine does not keep, for the REQUEST decoder (gpx_wire_req_meta) */
+struct WireReqMore {
+  gpx_wire_req_meta m;
+  uint32_t digest_len, resp_len;
+};
+__device__ __forceinline__ uint32_t wr_u16(WireRd& r) {
+  const uint32_t hi = wr_u8(r);
+  return (hi << 8) | wr_u8(r);
+}
+/* x == nullptr (k_wire_decode): the other fields are skipped */
+__device__ __forceinline__ void wr_request_body(WireRd& r, WireReq& q, WireReqMore* x = nullptr) {
   q.req_id = wr_i64(r);
   q.stop = wr_u8(r) == 1u;
-  wr_skip(r, 4 + 2 + 4 + 2); /* client and listen addresses */
+  if (x) {
+    for (int b = 0; b < 4; b++) x->m.client_ip[b] = (uint8_t)wr_u8(r);
+    x->m.client_port = (uint16_t)wr_u16(r);
+    for (int b = 0; b < 4; b++) x->m.listen_ip[b] = (uint8_t)wr_u8(r);
+    x->m.listen_port = (uint16_t)wr_u16(r);
+  } else {
+    wr_skip(r, 4 + 2 + 4 + 2); /* client and listen addresses */
+  }
   q.entry = wr_i32(r);
-  wr_skip(r, 8 + 1 + 4 + 1); /* entryTime, shouldReturnRequestValue, forwardCount, broadcasted */
+  if (x) {
+    x->m.entry_time = wr_i64(r);
+    x->m.flags = wr_u8(r) == 1u ? GPX_RM_RETURN_VALUE : 0u;
+    x->m.forward_count = wr_i32(r);
+    x->m.flags |= wr_u8(r) == 1u ? GPX_RM_BROADCASTED : 0u;
+    x->m.pad = 0;
+  } else {
+    wr_skip(r, 8 + 1 + 4 + 1); /* entryTime, shouldReturnRequestValue, forwardCount, broadcasted */
+  }
   uint32_t at;
-  wr_bytes(r, &at); /* digest */
+  const uint32_t dl = wr_bytes(r, &at); /* digest */
   q.val_len = wr_bytes(r, &q.val_at);
-  wr_bytes(r, &at); /* responseValue */
+  const uint32_t rl = wr_bytes(r, &at); /* responseValue */
+  if (x) {
+    x->digest_len = dl;
+    x->resp_len = rl;
+  }
   q.n_batched = wr_i32(r);
   if (q.n_batched < 0) r.ok = false;
 }
@@ -463,6 +492,157 @@ __global__ void k_wire_decode(const __grid_constant__ DevState S, const __grid_c
   }
 }
 
+/* ---- REQUEST packets -> proposals (gpx_wire_decode_requests_device) ------------------------------------------------ */
+enum { WQ_REQ = 0, WQ_PAY = 1, WQ_NCNT = 2 };
+
+struct WireReqDecodeArgs {
+  const uint8_t* bytes;
+  const gpx_wire_ref* pkts;
+  uint64_t n_bytes;
+  uint32_t n;
+  long long now_ms;
+  uint32_t* cnt;  /* [WQ_NCNT][n]: pass 0 writes the packet's requests and payload bytes (each value padded to 16) */
+  const uint32_t* off; /* [WQ_NCNT][n]: pass 1 reads their exclusive prefix sums */
+  int32_t* status;
+  /* pass 1: requests and meta staged in packet order, the sort keys (gids) beside them; the payload is the output */
+  gpx_request_rec* req;
+  gpx_wire_req_meta* meta;
+  uint32_t* key;
+  uint8_t* payload;
+  int emit;
+};
+
+/* one request of a REQUEST packet at staged position o, its value at payload offset *po (advanced) */
+__device__ __forceinline__ void wire_put_request(const WireReqDecodeArgs& A, uint32_t o, uint32_t* po, uint32_t gid,
+                                                 uint32_t k, int32_t node, uint32_t lane, const WireRd& r,
+                                                 const WireReq& q, const WireReqMore& x) {
+  gpx_request_rec rq;
+  rq.gid = gid;
+  rq.flags = (q.stop ? GPX_F_STOP : 0u) | (lane << 8);
+  rq.req_id = q.req_id;
+  rq.payload_off = *po;
+  rq.payload_len = q.val_len;
+  gpx_wire_req_meta m = x.m;
+  if (q.entry == -1) { /* IntegerMap.NULL_INT_NODE: setEntryReplica :393-403 with the call's clock */
+    rq.entry_node = node;
+    m.entry_time = A.now_ms;
+  } else {
+    rq.entry_node = q.entry;
+  }
+  rq.client = k;
+  A.req[o] = rq;
+  A.meta[o] = m;
+  A.key[o] = gid;
+  uint8_t* d = A.payload + *po;
+  wire_copy(d, r.p + q.val_at, q.val_len);
+  const uint32_t padded = (q.val_len + 15u) & ~15u;
+  for (uint32_t b = q.val_len; b < padded; b++) d[b] = 0;
+  *po += padded;
+}
+
+/* one thread per packet.  Pass 0 (emit == 0) parses and validates the packet (the request part of k_wire_decode's
+ * ACCEPT rules), looks its name and receiving node up and writes its status and output sizes; pass 1 parses it again
+ * and writes its requests, meta and values at the scanned offsets. */
+__global__ void k_wire_req_decode(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                                  const __grid_constant__ WireReqDecodeArgs A) {
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= A.n) return;
+  if (A.emit && A.status[k] != GPX_WS_OK) return;
+  const gpx_wire_ref ref = A.pkts[k];
+  int32_t st = GPX_WS_OK;
+  WireRd r;
+  r.p = A.bytes + ref.off;
+  r.len = ref.len;
+  r.n = 0;
+  r.ok = (uint64_t)ref.off + ref.len <= A.n_bytes;
+  WireHdr h;
+  if (r.ok && ref.len > 0 && r.p[0] == '{') {
+    st = GPX_WS_UNHANDLED; /* JSON packet */
+  } else if (!wr_header(r, h)) {
+    st = GPX_WS_MALFORMED;
+  } else if (h.type != GPX_PT_REQUEST) {
+    st = GPX_WS_UNHANDLED;
+  }
+  WireReq q;
+  WireReqMore x;
+  uint32_t sub_at = 0, n_sub = 0, pay = 0;
+  bool host_only = false;
+  if (st == GPX_WS_OK) {
+    wr_request_body(r, q, &x);
+    sub_at = r.n;
+    n_sub = r.ok ? (uint32_t)q.n_batched : 0u;
+    pay = (q.val_len + 15u) & ~15u;
+    host_only = x.digest_len != 0 || x.resp_len != 0;
+    for (uint32_t b = 0; b < n_sub && r.ok; b++) { /* {int length}{REQUEST packet} :929-936 */
+      const int32_t l = wr_i32(r);
+      if (l < 0 || !wr_need(r, (uint32_t)l)) {
+        r.ok = false;
+        break;
+      }
+      WireRd s;
+      s.p = r.p + r.n;
+      s.len = (uint32_t)l;
+      s.n = 0;
+      s.ok = true;
+      WireHdr sh;
+      WireReq sq;
+      WireReqMore sx;
+      const bool hok = wr_header(s, sh);
+      wr_request_body(s, sq, &sx);
+      /* a latched request carries no latched requests of its own (RequestBatcher latches one level) */
+      if (!hok || !s.ok || sq.n_batched != 0 || s.n != s.len) r.ok = false;
+      pay += (sq.val_len + 15u) & ~15u;
+      host_only = host_only || sx.digest_len != 0 || sx.resp_len != 0;
+      r.n += (uint32_t)l;
+    }
+    if (!r.ok || r.n != r.len) st = GPX_WS_MALFORMED;
+    else if (host_only) st = GPX_WS_UNHANDLED; /* digest mode / a response: the host's */
+  }
+  uint32_t gid = GPX_NAME_NONE, lane = 0;
+  if (st == GPX_WS_OK) {
+    gid = wire_name_find(W, r.p + h.id_at, h.id_len);
+    const GroupCtx g = group_ctx(S, gid);
+    if (gid == GPX_NAME_NONE || !g.live) {
+      st = GPX_WS_UNKNOWN_NAME;
+    } else if (W.version[gid] != h.version) {
+      st = GPX_WS_VERSION; /* PISM :441-447 */
+    } else {
+      lane = S.L;
+      for (uint32_t l = 0; l < S.L; l++)
+        if (S.lane_node[l] == ref.node) lane = l;
+      if (lane == S.L || wire_member_idx(g.ms, g.R, ref.node) == 0xffu) st = GPX_WS_NOT_LOCAL;
+    }
+  }
+  if (!A.emit) {
+    A.status[k] = st;
+    A.cnt[k] = st == GPX_WS_OK ? 1u + n_sub : 0u;
+    A.cnt[A.n + k] = st == GPX_WS_OK ? pay : 0u;
+    return;
+  }
+  uint32_t o = A.off[k], po = A.off[A.n + k];
+  wire_put_request(A, o++, &po, gid, k, ref.node, lane, r, q, x);
+  WireRd rr;
+  rr.p = r.p;
+  rr.len = r.len;
+  rr.n = sub_at;
+  rr.ok = true;
+  for (uint32_t b = 0; b < n_sub; b++) {
+    const int32_t l = wr_i32(rr);
+    WireRd s;
+    s.p = rr.p + rr.n;
+    s.len = (uint32_t)l;
+    s.n = 0;
+    s.ok = true;
+    WireHdr sh;
+    WireReq sq;
+    WireReqMore sx;
+    wr_header(s, sh);
+    wr_request_body(s, sq, &sx);
+    wire_put_request(A, o++, &po, gid, k, ref.node, lane, s, sq, sx);
+    rr.n += (uint32_t)l;
+  }
+}
+
 /* launch glue of the host side (gpx_wire_host.inc) */
 __global__ void k_wire_iota(uint32_t* p, uint32_t n) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -703,6 +883,131 @@ __global__ void k_wire_enc_decisions(const __grid_constant__ DevState S, const _
     r.off = A.off[p];
     r.len = b;
     r.gid = d.gid;
+    r.node = g.ms->nodes[m];
+    A.refs[ri++] = r;
+  }
+}
+
+/* ---- ACCEPTs -> AcceptPacket bytes (gpx_wire_encode_accepts_device) --------------------------------------------------- */
+struct WireAccArgs {
+  const uint32_t* head;          /* [n] request index that starts ACCEPT k (gpx_propose_device_heads) */
+  const gpx_request_rec* reqs;   /* [n_reqs] */
+  const gpx_wire_req_meta* meta; /* [n_reqs] */
+  uint32_t n_reqs;
+  const uint8_t* payload;        /* the request arena: bodies at reqs[q].payload_off */
+};
+
+/* one thread per ACCEPT: what happens to it and its sort key (the gid); past the device count: sorts last, unread */
+__global__ void k_wire_enc_keys_accepts(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                                        const __grid_constant__ WireEncodeArgs A, const __grid_constant__ WireAccArgs X) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= A.n) return;
+  if (A.n_ptr && i >= *A.n_ptr) {
+    A.key[i] = GPX_WIRE_NOKEY;
+    return;
+  }
+  const gpx_accept_rec a = reinterpret_cast<const gpx_accept_rec*>(A.recs)[i];
+  uint8_t st = GPX_WE_SENT;
+  const GroupCtx g = group_ctx(S, a.h.gid);
+  if ((a.h.flags & GPX_F_VOID) || !g.live) {
+    st = GPX_WE_VOID;
+  } else if (wire_popc(g.ms->lane_mask) >= g.R) {
+    st = GPX_WE_LOCAL; /* every member is a local lane */
+  } else if (W.slot == nullptr || W.slot[a.h.gid] == GPX_NAME_NONE) {
+    st = GPX_WE_NO_NAME;
+  } else {
+    const uint32_t q = X.head[i];
+    if (a.nreq == 0 || q >= X.n_reqs || a.nreq > X.n_reqs - q || X.reqs[q].gid != a.h.gid) st = GPX_WE_BAD_HEAD;
+  }
+  A.rstatus[i] = st;
+  A.key[i] = st == GPX_WE_SENT ? a.h.gid : GPX_WIRE_NOKEY;
+}
+
+/* RequestPacket.toBytes :819-949 of request q without batched requests (n_batched written by the caller's count) */
+__device__ __forceinline__ uint32_t ww_request(uint8_t* p, int32_t type, const WireNames& W, uint32_t gid,
+                                               const WireAccArgs& X, uint32_t q, uint32_t n_batched) {
+  const gpx_request_rec rq = X.reqs[q];
+  const gpx_wire_req_meta m = X.meta[q];
+  uint32_t b = ww_header(p, type, W, gid);
+  ww_i64(p + b, rq.req_id);
+  p[b + 8] = (rq.flags & GPX_F_STOP) ? 1u : 0u;
+  b += 9;
+  for (int j = 0; j < 4; j++) p[b + j] = m.client_port ? m.client_ip[j] : 0u;
+  p[b + 4] = (uint8_t)(m.client_port >> 8);
+  p[b + 5] = (uint8_t)m.client_port;
+  for (int j = 0; j < 4; j++) p[b + 6 + j] = m.listen_port ? m.listen_ip[j] : 0u;
+  p[b + 10] = (uint8_t)(m.listen_port >> 8);
+  p[b + 11] = (uint8_t)m.listen_port;
+  b += 12;
+  ww_i32(p + b, rq.entry_node);
+  ww_i64(p + b + 4, m.entry_time);
+  p[b + 12] = (m.flags & GPX_RM_RETURN_VALUE) ? 1u : 0u;
+  ww_i32(p + b + 13, m.forward_count);
+  p[b + 17] = (m.flags & GPX_RM_BROADCASTED) ? 1u : 0u;
+  ww_i32(p + b + 18, 0); /* digest */
+  ww_i32(p + b + 22, (int32_t)rq.payload_len);
+  b += 26;
+  wire_copy(p + b, X.payload + rq.payload_off, rq.payload_len);
+  b += rq.payload_len;
+  ww_i32(p + b, 0); /* responseValue */
+  ww_i32(p + b + 4, (int32_t)n_batched);
+  return b + 8;
+}
+/* bytes of one RequestPacket without batched requests: header, 55 fixed bytes, the value */
+__device__ __forceinline__ uint32_t wire_request_bytes(const WireNames& W, uint32_t gid, uint32_t val_len) {
+  return 13u + W.name[(size_t)gid * GPX_NAME_BYTES] + 55u + val_len;
+}
+
+/* one thread per sorted position; every encoded ACCEPT is one AcceptPacket (AcceptPacket.toBytes :95-138), stored once
+ * and indexed once per member node that no local lane serves */
+__global__ void k_wire_enc_accepts(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                                   const __grid_constant__ WireEncodeArgs A, const __grid_constant__ WireAccArgs X) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= A.n) return;
+  const bool sent = A.skey[p] != GPX_WIRE_NOKEY;
+  const gpx_accept_rec* recs = reinterpret_cast<const gpx_accept_rec*>(A.recs);
+  const uint32_t i = sent ? A.perm[p] : 0u;
+  if (!A.emit) {
+    uint32_t bytes = 0, n_remote = 0;
+    if (sent) {
+      const gpx_accept_rec a = recs[i];
+      const GroupCtx g = group_ctx(S, a.h.gid);
+      const uint32_t q0 = X.head[i];
+      bytes = 22u;
+      for (uint32_t q = q0; q < q0 + a.nreq; q++)
+        bytes += wire_request_bytes(W, a.h.gid, X.reqs[q].payload_len) + (q > q0 ? 4u : 0u);
+      n_remote = g.R - wire_popc(g.ms->lane_mask);
+    }
+    A.cnt[p] = bytes;
+    A.cnt[A.n + p] = n_remote;
+    return;
+  }
+  if (!sent) return;
+  const gpx_accept_rec a = recs[i];
+  const GroupCtx g = group_ctx(S, a.h.gid);
+  const uint32_t q0 = X.head[i];
+  uint8_t* o = A.out + A.off[p];
+  uint32_t b = ww_request(o, GPX_PT_ACCEPT, W, a.h.gid, X, q0, a.nreq - 1u);
+  for (uint32_t q = q0 + 1; q < q0 + a.nreq; q++) { /* {int length}{REQUEST packet} :929-936 */
+    const uint32_t l = ww_request(o + b + 4, GPX_PT_REQUEST, W, a.h.gid, X, q, 0u);
+    ww_i32(o + b, (int32_t)l);
+    b += 4u + l;
+  }
+  ww_i32(o + b, a.h.slot);
+  ww_i32(o + b + 4, a.h.bnum);
+  ww_i32(o + b + 8, a.h.bcoord);
+  o[b + 12] = 0; /* recovery */
+  ww_i32(o + b + 13, a.h.median_cp);
+  o[b + 17] = 0; /* noCoalesce */
+  ww_i32(o + b + 18, a.sender);
+  b += 22;
+  uint32_t ri = A.off[A.n + p];
+  for (uint32_t m = 0; m < g.R; m++) {
+    if (g.ms->lane_of_idx[m] != 0xffu) continue;
+    gpx_wire_ref r;
+    r.off = A.off[p];
+    r.len = b;
+    r.gid = a.h.gid;
     r.node = g.ms->nodes[m];
     A.refs[ri++] = r;
   }

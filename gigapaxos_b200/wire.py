@@ -407,3 +407,67 @@ def encode_decisions_device(engine, decisions, n_ptr: Optional[int], n_max: int,
     return _encode_device(engine, "wire_encode_decisions_device",
                           (_dptr(decisions), C.c_void_p(n_ptr) if n_ptr else None, C.c_uint32(n_max)), n_max,
                           decisions.device, caps, stream)
+
+
+# ---- the coordinator's side: REQUEST packets -> proposals -> ACCEPT packets, on the device ---------------------------
+RequestsOut = namedtuple("RequestsOut", "status reqs meta payload sizes")
+
+
+def req_meta(r: Request) -> np.ndarray:
+    """the gpx_wire_req_meta of a Request: the wire fields a gpx_request_rec does not keep"""
+    m = np.zeros(1, abi.req_meta_dtype)
+    for name, a in (("client", r.client), ("listen", r.listen)):
+        if a is not None and a[1]:
+            m[name + "_ip"][0] = [int(x) for x in a[0].split(".")]
+            m[name + "_port"] = a[1]
+    m["forward_count"], m["entry_time"] = r.forward_count, r.entry_time
+    m["flags"] = (abi.RM_RETURN_VALUE if r.should_return else 0) | (abi.RM_BROADCASTED if r.broadcasted else 0)
+    return m[0]
+
+
+def decode_requests_device(engine, arena, refs, now_ms: int, caps, stream=None) -> RequestsOut:
+    """gpx_wire_decode_requests_device: the REQUEST packets refs[n] of `arena` (device_packets; the refs' node column
+    names the node that received each packet).  caps = (requests, payload bytes); GPX_ERANGE as in decode_batch_device.
+    Returns status int32 [n], reqs [k, 32] and meta [k, 32] (grouped by gid, gpx_propose_device's input form), the
+    payload arena and the two host sizes."""
+    import torch
+    n, dev = int(refs.shape[0]), refs.device
+    L, st = engine.L, stream_handle(stream)
+    caps = [int(c) for c in caps]
+    with _on(stream):
+        status = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+        for _ in range(2):
+            reqs = torch.empty((max(caps[0], 1), 32), dtype=torch.uint8, device=dev)
+            meta = torch.empty((max(caps[0], 1), 32), dtype=torch.uint8, device=dev)
+            pay = torch.empty(max(caps[1], 16), dtype=torch.uint8, device=dev)
+            nq, nb = C.c_uint32(caps[0]), C.c_uint64(caps[1])
+            rc = L.fn("wire_decode_requests_device")(engine.handle, C.c_uint32(n), _dptr(arena),
+                                                     C.c_uint64(arena.numel()), _dptr(refs), C.c_int64(now_ms),
+                                                     _dptr(status), _dptr(reqs), _dptr(meta), C.byref(nq), _dptr(pay),
+                                                     C.byref(nb), st)
+            caps = [nq.value, nb.value]
+            if rc != abi.GPX_ERANGE:
+                break
+    L.check(rc)
+    return RequestsOut(status[:n], reqs[: caps[0]], meta[: caps[0]], pay[: caps[1]], tuple(caps))
+
+
+def propose_device_heads(engine, reqs, n: int, payload, payload_bytes: int, status, accepts, heads, ctl, stream=None):
+    """gpx_propose_device_heads over CUDA tensors: the ACCEPTs at `accepts` ([n, 48]), counted in ctl (gpx_dev_ctl,
+    zeroed by the caller), and heads [n] uint32: the request that starts each ACCEPT, 0xffffffff for a VOID filler"""
+    L = engine.L
+    L.check(L.fn("propose_device_heads")(engine.handle, _dptr(reqs), _dptr(payload), C.c_uint64(payload_bytes),
+                                         C.c_uint32(n), _dptr(status), _dptr(accepts), _dptr(heads), _dptr(ctl),
+                                         stream_handle(stream)))
+
+
+def encode_accepts_device(engine, accepts, n_ptr: Optional[int], n_max: int, heads, reqs, meta, n_reqs: int, payload,
+                          caps, stream=None) -> EncodeOut:
+    """gpx_wire_encode_accepts_device: AcceptPackets of the ACCEPTs (count read on the device at address n_ptr, e.g.
+    the n_accepts word of the gpx_dev_ctl propose_device_heads counted into, at most n_max; None = n_max), their
+    requests read at heads[k] of reqs / meta / payload.  caps = (packet bytes, packets); GPX_ERANGE as in
+    decode_batch_device."""
+    return _encode_device(engine, "wire_encode_accepts_device",
+                          (_dptr(accepts), C.c_void_p(n_ptr) if n_ptr else None, C.c_uint32(n_max), _dptr(heads),
+                           _dptr(reqs), _dptr(meta), C.c_uint32(n_reqs), _dptr(payload)), n_max, accepts.device, caps,
+                          stream)

@@ -845,7 +845,8 @@ int gpx_get_kernel_times(gpx_engine* e, gpx_kernel_times* out, int reset);
 int gpx_set_group_names(gpx_engine* e, uint32_t n, const uint32_t* gids, const uint8_t* names, const uint32_t* name_off,
                         const uint32_t* name_len);
 
-/* one packet in a byte arena: input of the decoder (gid and node ignored), output of the encoders, 16 B */
+/* one packet in a byte arena: input of the decoders (gid ignored; node ignored except by
+ * gpx_wire_decode_requests_device: the receiving node), output of the encoders, 16 B */
 typedef struct gpx_wire_ref {
   uint32_t off;  /* byte offset in the arena */
   uint32_t len;
@@ -940,6 +941,69 @@ int gpx_wire_encode_replies_device(gpx_engine* e, uint32_t n, const gpx_accept_r
 int gpx_wire_encode_decisions_device(gpx_engine* e, const gpx_decision_rec* decisions, const uint32_t* n_ptr,
                                      uint32_t n_max, uint8_t* rstatus, uint8_t* out, uint64_t* out_bytes,
                                      gpx_wire_ref* refs, uint32_t* n_refs, void* stream);
+
+/* ---- the coordinator's side: REQUEST packets in, ACCEPT packets out ---------------------------------------------
+ * A RequestPacket reaches the coordinator as REQUEST bytes (PaxosPacket type 1), from a client or forwarded by another
+ * replica (PISM.handleProposal :854-885), and leaves inside the coordinator's AcceptPacket, which carries the whole
+ * RequestPacket (AcceptPacket.java:95-138, RequestPacket.toBytes :819-949).  gpx_request_rec keeps what the engine
+ * needs; gpx_wire_req_meta keeps the rest of the wire fields, so that the ACCEPT can be written again byte for byte.
+ * Callers keep it parallel to the request array: meta[q] belongs to reqs[q].
+ *
+ * Requests that carry a digest (digest mode, PISM :842-843) or a non-empty responseValue stay on the host: the decoder
+ * reports their packets as GPX_WS_UNHANDLED and the encoder always writes both as empty. */
+#define GPX_RM_RETURN_VALUE 1u /* RequestPacket.shouldReturnRequestValue */
+#define GPX_RM_BROADCASTED 2u  /* RequestPacket.broadcasted */
+typedef struct gpx_wire_req_meta { /* 32 B */
+  uint8_t client_ip[4];   /* clientAddress (zeros when client_port is 0) */
+  uint16_t client_port;   /* 0 = no client address */
+  uint16_t listen_port;   /* 0 = no listen address */
+  uint8_t listen_ip[4];   /* listenAddress */
+  int32_t forward_count;  /* RequestPacket.forwardCount */
+  int64_t entry_time;     /* RequestPacket.entryTime (ms) */
+  uint32_t flags;         /* GPX_RM_* */
+  uint32_t pad;
+} gpx_wire_req_meta;
+
+/* Decode a batch of REQUEST packets into proposals.  bytes, pkts, status, reqs, meta and payload are device pointers;
+ * pkts[k].node names the node that received packet k (gid ignored).  Outputs:
+ *   reqs[*n_reqs], meta[*n_reqs]  grouped by gid, packet order within a group; a batched RequestPacket unrolls into
+ *                          its outer request and then its `batched` entries in order -- gpx_propose_device's input form.
+ *                          flags = STOP | the lane serving the receiving node << 8; client = packet index; an unset
+ *                          entryReplica (IntegerMap.NULL_INT_NODE, -1) becomes the receiving node with entry_time =
+ *                          now_ms (RequestPacket.setEntryReplica :393-403), otherwise both are the packet's.
+ *   payload[*payload_bytes] every requestValue at a 16-byte aligned offset (payload_off).
+ *   status[n]              GPX_WS_* per packet: GPX_WS_MALFORMED as gpx_wire_decode_batch judges an ACCEPT's request
+ *                          part; GPX_WS_UNHANDLED for JSON, every type but REQUEST, and a digest or a responseValue in
+ *                          any of its requests; GPX_WS_UNKNOWN_NAME / GPX_WS_VERSION from the name table;
+ *                          GPX_WS_NOT_LOCAL when no local lane serves the receiving node or it is not a member.
+ * *n_reqs and *payload_bytes are HOST pointers, capacities in / sizes out; GPX_ERANGE reports the sizes and writes
+ * nothing else.  Stream-ordered on `stream` (NULL = the engine's stream); one synchronisation reads the totals. */
+int gpx_wire_decode_requests_device(gpx_engine* e, uint32_t n, const uint8_t* bytes, uint64_t n_bytes,
+                                    const gpx_wire_ref* pkts, int64_t now_ms, int32_t* status, gpx_request_rec* reqs,
+                                    gpx_wire_req_meta* meta, uint32_t* n_reqs, uint8_t* payload,
+                                    uint64_t* payload_bytes, void* stream);
+
+/* gpx_propose_device, and out_head[n] (device): for each ACCEPT k below ctl->n_accepts, the index of the request that
+ * starts its slot -- its nreq requests are [out_head[k], out_head[k] + nreq) -- or 0xffffffff for a VOID filler.
+ * Every other output is byte-identical to gpx_propose_device's. */
+int gpx_propose_device_heads(gpx_engine* e, const gpx_request_rec* reqs, const uint8_t* payload, uint64_t payload_bytes,
+                             uint32_t n, int32_t* status, gpx_accept_rec* out_accepts, uint32_t* out_head,
+                             gpx_dev_ctl* ctl, void* stream);
+
+#define GPX_WE_BAD_HEAD 5 /* encode_accepts: head out of range, head + nreq > n_reqs, or reqs[head] of another gid */
+
+/* Encode ACCEPTs as AcceptPackets, byte-identical to gpx_wire_encode_accept: the outer RequestPacket is request
+ * heads[k] (header type ACCEPT), `batched` its next nreq - 1 requests as REQUEST packets, then slot, ballot,
+ * recovery 0, median_cp, noCoalesce 0 and sender.  Request bodies are read at reqs[q].payload_off of `payload` (the
+ * arena gpx_propose_device was given), never from the engine's constructed blobs.  The count of ACCEPTs is read on the
+ * device from *n_ptr (e.g. &ctl->n_accepts), at most n_max; NULL = n_max.  Each packet is stored once and indexed once
+ * per member node that no local lane serves, in gid order.  rstatus[k] (below the count): GPX_WE_SENT, GPX_WE_VOID,
+ * GPX_WE_LOCAL (no remote member), GPX_WE_NO_NAME or GPX_WE_BAD_HEAD.  All pointers but out_bytes / n_refs (host,
+ * capacities in / sizes out, GPX_ERANGE as above) are device pointers. */
+int gpx_wire_encode_accepts_device(gpx_engine* e, const gpx_accept_rec* accepts, const uint32_t* n_ptr, uint32_t n_max,
+                                   const uint32_t* heads, const gpx_request_rec* reqs, const gpx_wire_req_meta* meta,
+                                   uint32_t n_reqs, const uint8_t* payload, uint8_t* rstatus, uint8_t* out,
+                                   uint64_t* out_bytes, gpx_wire_ref* refs, uint32_t* n_refs, void* stream);
 
 /* ---- helpers shared with the reference semantics ---------------------------------- */
 int32_t gpx_java_string_hash(const char* s, size_t len); /* String.hashCode() */

@@ -216,11 +216,117 @@ def acceptor_chain(lib, G, arena, refs, reps):
     return res
 
 
+def coordinator_chain(lib, G, reps):
+    """node 100 as the coordinator of G groups {100, 101, 102}, one client REQUEST per group it coordinates per round.
+    Device leg: one upload of the request arena, decode_requests_device -> propose_device_heads ->
+    encode_accepts_device, one download of the ACCEPT arena.  Host leg: the same requests through gpx_propose (host
+    records) and the per-packet host encoder (wire.encode_accept, one call per ACCEPT).  The legs alternate on two
+    engines in the same state and must write the same ACCEPT packets."""
+    import ctypes as C
+
+    import torch
+
+    from gigapaxos_b200 import abi, wire
+    from gigapaxos_b200.spread import coordinator_of
+    from helpers import Engine, group_descs_fast, make_config
+
+    assert reps + 1 <= 8, "every round takes a slot of the window"
+    members = [100, 101, 102]
+    names = [f"NoopPaxosApp{i}" for i in range(G)]
+    gids = np.array([g for g in range(G) if coordinator_of(names[g], members) == 100], np.uint32)
+    engines = []
+    for _ in range(2):
+        e = Engine(lib, make_config(lib, max_groups=G, n_lanes=1, lane_node=[100], window=8, max_batch_recs=G,
+                                    max_batch_payload=16 * G, log_ring_bytes=1 << 20))
+        e.create_groups(group_descs_fast(G, members=tuple(members)))
+        wire.set_group_names(e, gids, [names[g] for g in gids])
+        engines.append(e)
+    ed, eh = engines
+    n = len(gids)
+
+    def round_requests(r):
+        return [wire.Request(names[g], 0, r * G + int(g), b"12345678", client=("10.0.0.1", 2000)) for g in gids]
+
+    rounds = []
+    for r in range(reps + 1):
+        arena, refs = wire.pack_packets([wire.encode_request(q) for q in round_requests(r)])
+        refs["node"] = 100
+        rounds.append((torch.from_numpy(arena.copy()).pin_memory(),
+                       torch.from_numpy(refs.view(np.uint8).reshape(n, 16).copy()).pin_memory(), round_requests(r)))
+    d_arena = torch.empty(rounds[0][0].numel(), dtype=torch.uint8, device="cuda")
+    d_refs = torch.empty((n, 16), dtype=torch.uint8, device="cuda")
+    status = torch.empty(n, dtype=torch.int32, device="cuda")
+    acc = torch.empty((n, 48), dtype=torch.uint8, device="cuda")
+    heads = torch.empty(n, dtype=torch.int32, device="cuda")
+    ctl = torch.zeros(8, dtype=torch.int32, device="cuda")
+    h_out = torch.empty(256 * n, dtype=torch.uint8).pin_memory()
+    h_refs = torch.empty((2 * n, 16), dtype=torch.uint8).pin_memory()
+    caps = {"req": (n, 16 * n), "enc": (256 * n, 2 * n)}
+    NOW = 1_700_000_000_000
+
+    def device_leg(r):
+        d_arena.copy_(rounds[r][0], non_blocking=True)
+        d_refs.copy_(rounds[r][1], non_blocking=True)
+        d = wire.decode_requests_device(ed, d_arena, d_refs, NOW, caps["req"])
+        ctl.zero_()
+        wire.propose_device_heads(ed, d.reqs, d.sizes[0], d.payload, d.sizes[1], status, acc, heads, ctl)
+        enc = wire.encode_accepts_device(ed, acc, ctl.data_ptr(), d.sizes[0], heads, d.reqs, d.meta, d.sizes[0],
+                                         d.payload, caps["enc"])
+        caps["req"], caps["enc"] = d.sizes, enc.sizes
+        h_out[: enc.sizes[0]].copy_(enc.out, non_blocking=True)
+        h_refs[: enc.sizes[1]].copy_(enc.refs, non_blocking=True)
+        torch.cuda.synchronize()
+        return enc.sizes
+
+    pay = np.zeros(16 * n, np.uint8)
+    pay.reshape(n, 16)[:, :8] = np.frombuffer(b"12345678", np.uint8)
+    host_reqs = np.zeros(n, abi.request_dtype)
+    host_reqs["gid"], host_reqs["payload_off"], host_reqs["payload_len"] = gids, 16 * np.arange(n), 8
+    host_reqs["entry_node"], host_reqs["client"] = 100, np.arange(n)
+    host_out = {}
+
+    def host_leg(r):
+        reqs = host_reqs.copy()
+        reqs["req_id"] = r * G + gids.astype(np.int64)
+        a, _, st = eh.propose(reqs, pay)
+        pk = []
+        for x in a[np.argsort(a["gid"], kind="stable")]:  # the device encoder writes in gid order
+            q = rounds[r][2][int(np.searchsorted(gids, x["gid"]))]
+            q.entry_replica, q.entry_time = 100, NOW
+            pk.append(wire.encode_accept(q, int(x["slot"]), int(x["bnum"]), int(x["bcoord"]), False,
+                                         int(x["median_cp"]), int(x["sender"])))
+        host_out[r] = pk
+        return sum(len(b) for b in pk), len(pk)
+
+    walls = {"device": [], "host": []}
+    for r in range(reps + 1):  # round 0 warms both legs up
+        for leg, run in (("device", device_leg), ("host", host_leg)):
+            t = time.perf_counter()
+            sizes = run(r)
+            if r:
+                walls[leg].append(time.perf_counter() - t)
+            if leg == "device":
+                dev_sizes = sizes
+        # the same ACCEPT packets: each stored once, indexed for nodes 101 and 102
+        refs = h_refs[: dev_sizes[1]].numpy().reshape(-1).view(abi.wire_ref_dtype)
+        got = [bytes(h_out[int(f["off"]): int(f["off"]) + int(f["len"])].numpy()) for f in refs[::2]]
+        assert got == host_out[r] and len(got) == n, "device and host ACCEPT packets differ"
+    res = {"groups": G, "requests": n, "accept_bytes": int(dev_sizes[0]), "upload_bytes": int(rounds[0][0].numel() + 16 * n)}
+    for leg in ("device", "host"):
+        w = min(walls[leg])
+        res[leg] = {"wall_s_min": w, "requests_per_s_wall": n / w}
+    for e in engines:
+        e.close()
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--groups", type=int, nargs="+", default=[100_000, 1_000_000])
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--only", choices=["coordinator_chain"], default=None,
+                    help="run only this entry (at each --groups size)")
     args = ap.parse_args()
     import gigapaxos_b200
     from gigapaxos_b200 import abi, wire
@@ -228,6 +334,16 @@ def main():
 
     lib = gigapaxos_b200.load_library()
     res = {"card": card_info(), "runs": []}
+    if args.only == "coordinator_chain":
+        for G in args.groups:
+            res["runs"].append({"groups": G, "coordinator_chain": coordinator_chain(lib, G, args.reps)})
+        res["card_after"] = card_info()
+        line = json.dumps(res)
+        print(line)
+        if args.out:
+            with open(args.out, "w") as f:
+                f.write(line + "\n")
+        return
     tmp = tempfile.mkdtemp(prefix="gpx_wire_rate_")
     exe = os.path.join(tmp, "host_wire")
     src = os.path.join(tmp, "host_wire.c")
@@ -300,6 +416,7 @@ def main():
                 run[f"{name}_{threads}t"] = {"packets": G, "s_min": s, "packets_per_s": G / s, "threads": threads}
         e.close()
         run["acceptor_chain"] = acceptor_chain(lib, G, arena, refs, args.reps)
+        run["coordinator_chain"] = coordinator_chain(lib, G, args.reps)
         res["runs"].append(run)
     res["card_after"] = card_info()
     line = json.dumps(res)
