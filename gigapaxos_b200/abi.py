@@ -57,6 +57,8 @@ req_meta_dtype = np.dtype([("client_ip", "u1", (4,)), ("client_port", "<u2"), ("
                            ("listen_ip", "u1", (4,)), ("forward_count", "<i4"), ("entry_time", "<i8"),
                            ("flags", "<u4"), ("pad", "<u4")])
 assert req_meta_dtype.itemsize == 32
+# gpx_wire_member: one member of a JSON packet (gpx_wire_decode_json_device)
+wire_member_dtype = np.dtype([("pkt", "<u4"), ("off", "<u4"), ("len", "<u4"), ("status", "<i4")])
 accepted_pvalue_dtype = np.dtype([("slot", "<i4"), ("bnum", "<i4"), ("bcoord", "<i4"), ("frame_ref", "<u4"),
                                   ("req_id", "<i8"), ("payload_len", "<u4"), ("flags", "<u4")])
 prepare_reply_dtype = np.dtype([("gid", "<u4"), ("first_slot", "<i4"), ("bnum", "<i4"), ("bcoord", "<i4"), ("who", "<u4"),

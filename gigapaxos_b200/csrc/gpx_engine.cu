@@ -27,6 +27,7 @@
 #include "gpx_pause.cuh"
 #include "gpx_logfind.cuh"
 #include "gpx_wire_dev.cuh"
+#include "gpx_wire_json.cuh"
 
 #include <cub/cub.cuh>
 

@@ -38,6 +38,7 @@ from typing import Dict, Iterable, List, Sequence, Tuple, Union
 
 PT_REQUEST, PT_PREPARE, PT_ACCEPT, PT_DECISION, PT_PREPARE_REPLY, PT_ACCEPT_REPLY = 1, 2, 3, 6, 7, 8
 PT_SYNC_DECISIONS, PT_BATCHED_ACCEPT, PT_BATCHED_PAXOS_PACKET, PT_PAXOS_PACKET = 32, 36, 37, 90  # PaxosPacketType :202-291
+PT_BATCHED_ACCEPT_REPLY, PT_BATCHED_COMMIT = 34, 35
 CHARSET = "iso-8859-1"  # PaxosPacket.CHARSET :439, BatchedAccept.CHARSET :36
 
 BATCH_ACROSS_GROUPS = True  # PaxosConfig.java:807
@@ -93,6 +94,32 @@ def accept_replies_to_packets(replies, names: Dict[int, Tuple[str, int]], node_o
         out.append(accept_reply_json(pid, ver, node_of_lane[who & 0xFF], int(r["bnum"]), int(r["bcoord"]),
                                      int(r["slot"]), int(r["max_cp"]), int(r["req_id"])))
     return out
+
+
+def batched_accept_reply_json(paxos_id: str, version: int, acceptor: int, bnum: int, bcoord: int, slot_number: int,
+                              max_checkpointed_slot: int, request_id: int, slots: Sequence[int],
+                              request_ids: Sequence[int]) -> bytes:
+    """BatchedAcceptReply.toJSONSmartImpl :86-96 on top of AcceptReplyPacket.toJSONSmartImpl :214-224: the header of the
+    first reply and SLOTS = [slot, requestID, ...] in ascending slot order (the TreeMap; a repeated slot keeps its last
+    requestID).  Wrapped by batched_paxos_packet_json, this is how a loaded Java peer's replies arrive."""
+    m = {}
+    for s, q in zip(slots, request_ids):
+        m[int(s)] = int(q)
+    d = _base(PT_BATCHED_ACCEPT_REPLY, paxos_id, version)
+    d.update({"SNDR": int(acceptor), "B": f"{int(bnum)}:{int(bcoord)}", "S": int(slot_number),
+              "CP_S": int(max_checkpointed_slot), "QID": int(request_id)})
+    d["SLOTS"] = [x for s in sorted(m) for x in (s, m[s])]
+    return _dumps(d)
+
+
+def batched_commit_json(paxos_id: str, version: int, bnum: int, bcoord: int, median_cp: int, slots: Sequence[int],
+                        group: Iterable[int]) -> bytes:
+    """BatchedCommit.toJSONSmartImpl :140-149: ballot, medianCheckpointedSlot, the group and the slots (a TreeSet:
+    ascending, distinct)"""
+    d = _base(PT_BATCHED_COMMIT, paxos_id, version)
+    d.update({"B": f"{int(bnum)}:{int(bcoord)}", "GC_S": int(median_cp), "GROUP": [int(g) for g in group],
+              "SLOTS": sorted(set(int(s) for s in slots))})
+    return _dumps(d)
 
 
 # ---- BATCHED_ACCEPT -------------------------------------------------------------------------------------------------
@@ -457,6 +484,18 @@ def parse_packet(pkt: bytes) -> dict:
         return {"kind": "ACCEPT_REPLY", "paxos_id": j["ID"], "version": j["V"], "acceptor": j["SNDR"], "bnum": bn,
                 "bcoord": bc, "slot_number": j["S"], "max_checkpointed_slot": j["CP_S"], "request_id": j["QID"],
                 "undigest_request": bool(j.get("NACK", False))}
+    if pt == PT_BATCHED_ACCEPT_REPLY:  # BatchedAcceptReply(JSONObject) :64-72
+        bn, bc = (int(x) for x in j["B"].split(":"))
+        pairs = [int(x) for x in j["SLOTS"]]
+        if len(pairs) % 2:
+            raise ValueError("SLOTS of odd length")
+        return {"kind": "BATCHED_ACCEPT_REPLY", "paxos_id": j["ID"], "version": j["V"], "acceptor": j["SNDR"],
+                "bnum": bn, "bcoord": bc, "slot_number": j["S"], "max_checkpointed_slot": j["CP_S"],
+                "request_id": j["QID"], "slots": pairs[0::2], "request_ids": pairs[1::2]}
+    if pt == PT_BATCHED_COMMIT:  # BatchedCommit(JSONObject) :75-92
+        bn, bc = (int(x) for x in j["B"].split(":"))
+        return {"kind": "BATCHED_COMMIT", "paxos_id": j["ID"], "version": j["V"], "bnum": bn, "bcoord": bc,
+                "median_cp": j["GC_S"], "group": [int(x) for x in j["GROUP"]], "slots": [int(x) for x in j["SLOTS"]]}
     if pt == PT_BATCHED_ACCEPT:
         b = BatchedAccept.from_json(j)
         return {"kind": "BATCHED_ACCEPT", "paxos_id": b.paxos_id, "version": b.version, "bnum": b.bnum, "bcoord": b.bcoord,

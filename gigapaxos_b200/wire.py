@@ -409,6 +409,36 @@ def encode_decisions_device(engine, decisions, n_ptr: Optional[int], n_max: int,
                           decisions.device, caps, stream)
 
 
+JsonOut = namedtuple("JsonOut", "status members replies decisions sizes")
+
+
+def decode_json_device(engine, arena, refs, caps, stream=None) -> JsonOut:
+    """gpx_wire_decode_json_device: the JSON packets refs[n] of `arena` (device_packets; the refs' node column names
+    the node that received each packet) -- BATCHED_PAXOS_PACKET wrappers and bare ACCEPT_REPLY / BATCHED_ACCEPT_REPLY /
+    BATCHED_COMMIT packets.  caps = (members, replies, decisions); GPX_ERANGE as in decode_batch_device.  Returns
+    status int32 [n], members [m, 16] (abi.wire_member_dtype), replies [nr, 32] and decisions [nd, 32] grouped by gid
+    (gpx_replies_device's and gpx_decisions_device's input form) and the three host sizes."""
+    import torch
+    n, dev = int(refs.shape[0]), refs.device
+    L, st = engine.L, stream_handle(stream)
+    caps = [int(c) for c in caps]
+    with _on(stream):
+        status = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+        for _ in range(2):
+            mem = torch.empty((max(caps[0], 1), 16), dtype=torch.uint8, device=dev)
+            rep = torch.empty((max(caps[1], 1), 32), dtype=torch.uint8, device=dev)
+            dec = torch.empty((max(caps[2], 1), 32), dtype=torch.uint8, device=dev)
+            sz = [C.c_uint32(caps[0]), C.c_uint32(caps[1]), C.c_uint32(caps[2])]
+            rc = L.fn("wire_decode_json_device")(engine.handle, C.c_uint32(n), _dptr(arena), C.c_uint64(arena.numel()),
+                                                 _dptr(refs), _dptr(status), _dptr(mem), C.byref(sz[0]), _dptr(rep),
+                                                 C.byref(sz[1]), _dptr(dec), C.byref(sz[2]), st)
+            caps = [s.value for s in sz]
+            if rc != abi.GPX_ERANGE:
+                break
+    L.check(rc)
+    return JsonOut(status[:n], mem[: caps[0]], rep[: caps[1]], dec[: caps[2]], tuple(caps))
+
+
 # ---- the coordinator's side: REQUEST packets -> proposals -> ACCEPT packets, on the device ---------------------------
 RequestsOut = namedtuple("RequestsOut", "status reqs meta payload sizes")
 

@@ -942,6 +942,84 @@ int gpx_wire_encode_decisions_device(gpx_engine* e, const gpx_decision_rec* deci
                                      uint32_t n_max, uint8_t* rstatus, uint8_t* out, uint64_t* out_bytes,
                                      gpx_wire_ref* refs, uint32_t* n_refs, void* stream);
 
+/* ---- the JSON form of replies and commits -------------------------------------------------------------------------
+ * A Java peer sends a BatchedAcceptReply or BatchedCommit as bytes only when it travels alone.  Under load its batcher
+ * wraps a sweep's packets in a BATCHED_PAXOS_PACKET (type 37, PaxosPacketBatcher.process :270-277), which is a JSON
+ * string {"type":90,"PT":37,"V":-1,"PP":[...]} whose members are the JSON objects of the BatchedAcceptReplies (34) and
+ * BatchedCommits (35) (BatchedPaxosPacket.toJSONSmartImpl :87-99); a wrapper is at most 4 MiB.  A NACK is a singleton
+ * ACCEPT_REPLY (8), always JSON.  gpx_wire_decode_json_device decodes these into the records gpx_wire_decode_batch
+ * makes from the byte forms.
+ *
+ * Schema (the keys of PaxosPacket.toJSONObject :478-494 and of the subclasses' toJSONSmartImpl):
+ *   every packet and member  "type" = 90 and "PT", both int; a member also "ID" (string; absent for PT 37) and "V" (int)
+ *   8  ACCEPT_REPLY          "SNDR", "B", "S", "CP_S", "QID", and optionally "NACK" (bool)
+ *   34 BATCHED_ACCEPT_REPLY  the keys of 8 and "SLOTS" = [slot, requestID, slot, requestID, ...] (an odd length is
+ *                            malformed)
+ *   35 BATCHED_COMMIT        "B", "GC_S", "GROUP" (int array), "SLOTS" (int array)
+ *   37 BATCHED_PAXOS_PACKET  "PP", an array of objects; no "ID", "V" = -1
+ * Strictness:
+ *   - Key order is free, unknown keys are skipped whatever their value, a duplicated key takes its last value (the
+ *     objects are hash maps), and any JSON whitespace may stand between tokens.
+ *   - Strings take every JSON escape (\uXXXX and \/ included); a raw byte 0x80-0xff is that ISO-8859-1 character (a
+ *     Java node writes String.getBytes("ISO-8859-1")); a raw control character is malformed.  "ID" is unescaped before
+ *     the lookup; one with a character above U+00FF or longer than GPX_WIRE_MAX_ID characters is GPX_WS_UNKNOWN_NAME
+ *     (no gid can have that name: the host decides).  "B" is "<int32>:<int32>", each part with an optional '-'.
+ *   - int fields are JSON integers within int32; "QID" and the requestIDs of SLOTS within int64.  A fraction, an
+ *     exponent, a leading zero or a leading '+' is malformed.  The reference would truncate some of these through
+ *     Number.intValue(); no Java sender writes them, and input from outside the process is rejected rather than
+ *     guessed at.
+ *   - A skipped value nested deeper than 64 levels is malformed.
+ *
+ * The one deliberate difference between the forms: a singleton ACCEPT_REPLY's "QID" is read as the reference reads it,
+ * with getInt (AcceptReplyPacket(JSONObject) :115), so req_id keeps its low 32 bits, sign-extended; the requestIDs of a
+ * BatchedAcceptReply's SLOTS are read with getLong (BatchedAcceptReply(JSONObject) :71), as the byte form carries
+ * them.  No state and no tally reads a reply's req_id (gpx_replies_device and gpx_handle_accept_replies use slot,
+ * ballot, max_cp and who), so the difference reaches no state; gpx_wire_encode_replies copies it into the bytes it
+ * writes.
+ *
+ * Scratch: the call sizes its working buffers from bounds known before its one synchronisation -- about 7 bytes of
+ * engine-owned HBM per arena byte (chunk summaries, the two event lists at half the covered bytes each, member slots
+ * at one per GPX_JSON_MIN_MEMBER bytes) plus about 1 KiB per packet -- and keeps them for the engine's next wire call,
+ * as the other wire calls keep theirs. */
+typedef struct gpx_wire_member { /* 16 B */
+  uint32_t pkt;   /* index of the packet it came from */
+  uint32_t off;   /* byte range of the member's JSON object in the arena (the whole packet for a bare one) */
+  uint32_t len;
+  int32_t status; /* GPX_WS_* */
+} gpx_wire_member;
+
+/* Decode JSON packets: BATCHED_PAXOS_PACKET wrappers and bare ACCEPT_REPLY / BATCHED_ACCEPT_REPLY / BATCHED_COMMIT
+ * packets.  bytes, pkts, status, members, replies, decisions are device pointers; the three counts are HOST pointers,
+ * capacities in / sizes out, and GPX_ERANGE reports the sizes and writes no output.  pkts[k].node is the node that
+ * received packet k (gid ignored).  The packets' lengths must add up to at most n_bytes (refs that do not overlap
+ * always do), else GPX_EINVAL and nothing is written.  Stream-ordered on `stream` (NULL = the engine's stream) with the
+ * other wire calls' scratch; one synchronisation reads the totals.
+ *   status[n]   GPX_WS_OK: well-formed JSON of type 37, or of type 8, 34 or 35 (one member, the whole packet); an
+ *               empty PP is OK without members.  GPX_WS_MALFORMED: invalid JSON anywhere in the packet, a schema
+ *               failure in it or in any member (no member of it is listed or gives records: the reference loses the
+ *               whole container when its constructor throws), or a ref past n_bytes.  GPX_WS_UNHANDLED: not JSON (the
+ *               first byte that is not whitespace is not '{': gpx_wire_decode_batch_device's), or JSON of another type.
+ *   members[*n_members]  the members of the OK packets, in packet order and in PP order within one.  Member status:
+ *               GPX_WS_UNKNOWN_NAME, GPX_WS_VERSION, GPX_WS_NOT_LOCAL, GPX_WS_OK as gpx_wire_decode_batch judges a
+ *               byte packet, and GPX_WS_MALFORMED for an acceptor or coordinator outside the group; GPX_WS_UNHANDLED
+ *               for other types (REQUEST, DECISION, BATCHED_ACCEPT, a nested 37) and an ACCEPT_REPLY with
+ *               "NACK":true (digest mode's undigestRequest): the host takes those from off / len.  An
+ *               GPX_WS_UNKNOWN_NAME member may be resubmitted alone, as a bare packet, once the host unpauses its group.
+ *   replies[*n_replies]  34: one per SLOTS pair, byte-identical to what gpx_wire_decode_batch makes of the byte form
+ *               (who = (member index of SNDR, member index of the ballot's coordinator, 0), max_cp = CP_S; S and QID
+ *               validated, not used).  8: one reply, slot = S, max_cp = CP_S, ballot = B, req_id = QID (see above);
+ *               its destination is the receiving node, not the ballot's coordinator -- a NACK carries the acceptor's
+ *               higher ballot, whose coordinator is another node -- and GPX_WS_NOT_LOCAL when that node is not a
+ *               member or no local lane serves it.
+ *   decisions[*n_decisions]  35: one per SLOTS entry, median_cp = GC_S, flags GPX_F_DECISION, dst_mask = the group's
+ *               local lanes, req_id 0; byte-identical to the byte form's.  GROUP is validated, not used.
+ * Records are grouped by gid and, within a group, in (packet, member, slot) order: gpx_replies_device's and
+ * gpx_decisions_device's input form. */
+int gpx_wire_decode_json_device(gpx_engine* e, uint32_t n, const uint8_t* bytes, uint64_t n_bytes,
+                                const gpx_wire_ref* pkts, int32_t* status, gpx_wire_member* members,
+                                uint32_t* n_members, gpx_accept_reply_rec* replies, uint32_t* n_replies,
+                                gpx_decision_rec* decisions, uint32_t* n_decisions, void* stream);
+
 /* ---- the coordinator's side: REQUEST packets in, ACCEPT packets out ---------------------------------------------
  * A RequestPacket reaches the coordinator as REQUEST bytes (PaxosPacket type 1), from a client or forwarded by another
  * replica (PISM.handleProposal :854-885), and leaves inside the coordinator's AcceptPacket, which carries the whole
