@@ -256,26 +256,35 @@ def set_group_names(engine, gids, names: Sequence[str]):
                                     abi._ptr(offs), abi._ptr(lens)))
 
 
+def _sized(engine, caps, size_types, alloc, call):
+    """outputs = alloc(caps), then rc = call(outputs, sizes) with the sizes passed by reference (capacities in, sizes
+    out); when an output is too small (GPX_ERANGE), both once more at the sizes the call reported -> (outputs, sizes)"""
+    caps = [int(c) for c in caps]
+    for _ in range(2):
+        outs = alloc(caps)
+        sz = [t(c) for t, c in zip(size_types, caps)]
+        rc = call(outs, [C.byref(s) for s in sz])
+        caps = [s.value for s in sz]
+        if rc != abi.GPX_ERANGE:
+            break
+    engine.L.check(rc)
+    return outs, tuple(caps)
+
+
 def decode_batch(engine, packets: Sequence[bytes]):
     """gpx_wire_decode_batch -> (status[n], accepts, blob, replies, decisions); outputs grouped by gid"""
     L = engine.L
     arena, refs = pack_packets(packets)
     n = len(packets)
     status = np.zeros(max(n, 1), np.int32)
-    caps = [C.c_uint32(0), C.c_uint64(0), C.c_uint32(0), C.c_uint32(0)]
-    args = lambda acc, blob, rep, dec: (engine.handle, C.c_uint32(n), abi._ptr(arena), C.c_uint64(len(arena)),
-                                        abi._ptr(refs), abi._ptr(status), abi._ptr(acc), C.byref(caps[0]),
-                                        abi._ptr(blob), C.byref(caps[1]), abi._ptr(rep), C.byref(caps[2]),
-                                        abi._ptr(dec), C.byref(caps[3]))
-    rc = L.fn("wire_decode_batch")(*args(None, None, None, None))  # sizes first: an empty output is GPX_ERANGE
-    if rc not in (0, abi.GPX_ERANGE):
-        L.check(rc)
-    acc = np.zeros(max(caps[0].value, 1), abi.accept_dtype)
-    blob = np.zeros(max(caps[1].value, 16), np.uint8)
-    rep = np.zeros(max(caps[2].value, 1), abi.reply_dtype)
-    dec = np.zeros(max(caps[3].value, 1), abi.decision_dtype)
-    L.check(L.fn("wire_decode_batch")(*args(acc, blob, rep, dec)))
-    return (status[:n], acc[: caps[0].value], blob[: caps[1].value], rep[: caps[2].value], dec[: caps[3].value])
+    (acc, blob, rep, dec), caps = _sized(  # sizes first: at capacity 0 any output is GPX_ERANGE
+        engine, (0, 0, 0, 0), (C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32),
+        lambda c: (np.zeros(max(c[0], 1), abi.accept_dtype), np.zeros(max(c[1], 16), np.uint8),
+                   np.zeros(max(c[2], 1), abi.reply_dtype), np.zeros(max(c[3], 1), abi.decision_dtype)),
+        lambda o, sz: L.fn("wire_decode_batch")(engine.handle, C.c_uint32(n), abi._ptr(arena), C.c_uint64(len(arena)),
+                                                abi._ptr(refs), abi._ptr(status), abi._ptr(o[0]), sz[0],
+                                                abi._ptr(o[1]), sz[1], abi._ptr(o[2]), sz[2], abi._ptr(o[3]), sz[3]))
+    return (status[:n], acc[: caps[0]], blob[: caps[1]], rep[: caps[2]], dec[: caps[3]])
 
 
 def _encode(engine, name, recs, dtype):
@@ -283,16 +292,12 @@ def _encode(engine, name, recs, dtype):
     recs = np.ascontiguousarray(recs, dtype=dtype)
     n = len(recs)
     rstatus = np.zeros(max(n, 1), np.uint8)
-    nb, nr = C.c_uint64(0), C.c_uint32(0)
-    rc = L.fn(name)(engine.handle, C.c_uint32(n), abi._ptr(recs), abi._ptr(rstatus), None, C.byref(nb), None,
-                    C.byref(nr))
-    if rc not in (0, abi.GPX_ERANGE):
-        L.check(rc)
-    out = np.zeros(max(nb.value, 1), np.uint8)
-    refs = np.zeros(max(nr.value, 1), abi.wire_ref_dtype)
-    L.check(L.fn(name)(engine.handle, C.c_uint32(n), abi._ptr(recs), abi._ptr(rstatus), abi._ptr(out), C.byref(nb),
-                       abi._ptr(refs), C.byref(nr)))
-    return rstatus[:n], out[: nb.value], refs[: nr.value]
+    (out, refs), caps = _sized(
+        engine, (0, 0), (C.c_uint64, C.c_uint32),
+        lambda c: (np.zeros(max(c[0], 1), np.uint8), np.zeros(max(c[1], 1), abi.wire_ref_dtype)),
+        lambda o, sz: L.fn(name)(engine.handle, C.c_uint32(n), abi._ptr(recs), abi._ptr(rstatus), abi._ptr(o[0]),
+                                 sz[0], abi._ptr(o[1]), sz[1]))
+    return rstatus[:n], out[: caps[0]], refs[: caps[1]]
 
 
 def encode_replies(engine, replies: np.ndarray):
@@ -354,42 +359,32 @@ def decode_batch_device(engine, arena, refs, caps, stream=None) -> DecodeOut:
     import torch
     n, dev = int(refs.shape[0]), refs.device
     L, st = engine.L, stream_handle(stream)
-    caps = [int(c) for c in caps]
     with _on(stream):
         status = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
-        for _ in range(2):
-            acc = torch.empty((max(caps[0], 1), 48), dtype=torch.uint8, device=dev)
-            blob = torch.empty(max(caps[1], 16), dtype=torch.uint8, device=dev)
-            rep = torch.empty((max(caps[2], 1), 32), dtype=torch.uint8, device=dev)
-            dec = torch.empty((max(caps[3], 1), 32), dtype=torch.uint8, device=dev)
-            sz = [C.c_uint32(caps[0]), C.c_uint64(caps[1]), C.c_uint32(caps[2]), C.c_uint32(caps[3])]
-            rc = L.fn("wire_decode_batch_device")(engine.handle, C.c_uint32(n), _dptr(arena), C.c_uint64(arena.numel()),
-                                                  _dptr(refs), _dptr(status), _dptr(acc), C.byref(sz[0]), _dptr(blob),
-                                                  C.byref(sz[1]), _dptr(rep), C.byref(sz[2]), _dptr(dec),
-                                                  C.byref(sz[3]), st)
-            caps = [s.value for s in sz]
-            if rc != abi.GPX_ERANGE:
-                break
-    L.check(rc)
-    return DecodeOut(status[:n], acc[: caps[0]], blob[: caps[1]], rep[: caps[2]], dec[: caps[3]], tuple(caps))
+        (acc, blob, rep, dec), caps = _sized(
+            engine, caps, (C.c_uint32, C.c_uint64, C.c_uint32, C.c_uint32),
+            lambda c: (torch.empty((max(c[0], 1), 48), dtype=torch.uint8, device=dev),
+                       torch.empty(max(c[1], 16), dtype=torch.uint8, device=dev),
+                       torch.empty((max(c[2], 1), 32), dtype=torch.uint8, device=dev),
+                       torch.empty((max(c[3], 1), 32), dtype=torch.uint8, device=dev)),
+            lambda o, sz: L.fn("wire_decode_batch_device")(engine.handle, C.c_uint32(n), _dptr(arena),
+                                                           C.c_uint64(arena.numel()), _dptr(refs), _dptr(status),
+                                                           _dptr(o[0]), sz[0], _dptr(o[1]), sz[1], _dptr(o[2]), sz[2],
+                                                           _dptr(o[3]), sz[3], st))
+    return DecodeOut(status[:n], acc[: caps[0]], blob[: caps[1]], rep[: caps[2]], dec[: caps[3]], caps)
 
 
 def _encode_device(engine, name, lead, n, dev, caps, stream) -> EncodeOut:
     import torch
     L, st = engine.L, stream_handle(stream)
-    caps = [int(c) for c in caps]
     with _on(stream):
         rstatus = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
-        for _ in range(2):
-            out = torch.empty(max(caps[0], 1), dtype=torch.uint8, device=dev)
-            refs = torch.empty((max(caps[1], 1), 16), dtype=torch.uint8, device=dev)
-            nb, nr = C.c_uint64(caps[0]), C.c_uint32(caps[1])
-            rc = L.fn(name)(engine.handle, *lead, _dptr(rstatus), _dptr(out), C.byref(nb), _dptr(refs), C.byref(nr), st)
-            caps = [nb.value, nr.value]
-            if rc != abi.GPX_ERANGE:
-                break
-    L.check(rc)
-    return EncodeOut(rstatus[:n], out[: caps[0]], refs[: caps[1]], tuple(caps))
+        (out, refs), caps = _sized(
+            engine, caps, (C.c_uint64, C.c_uint32),
+            lambda c: (torch.empty(max(c[0], 1), dtype=torch.uint8, device=dev),
+                       torch.empty((max(c[1], 1), 16), dtype=torch.uint8, device=dev)),
+            lambda o, sz: L.fn(name)(engine.handle, *lead, _dptr(rstatus), _dptr(o[0]), sz[0], _dptr(o[1]), sz[1], st))
+    return EncodeOut(rstatus[:n], out[: caps[0]], refs[: caps[1]], caps)
 
 
 def encode_replies_device(engine, replies, n: int, caps, stream=None) -> EncodeOut:
@@ -421,22 +416,18 @@ def decode_json_device(engine, arena, refs, caps, stream=None) -> JsonOut:
     import torch
     n, dev = int(refs.shape[0]), refs.device
     L, st = engine.L, stream_handle(stream)
-    caps = [int(c) for c in caps]
     with _on(stream):
         status = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
-        for _ in range(2):
-            mem = torch.empty((max(caps[0], 1), 16), dtype=torch.uint8, device=dev)
-            rep = torch.empty((max(caps[1], 1), 32), dtype=torch.uint8, device=dev)
-            dec = torch.empty((max(caps[2], 1), 32), dtype=torch.uint8, device=dev)
-            sz = [C.c_uint32(caps[0]), C.c_uint32(caps[1]), C.c_uint32(caps[2])]
-            rc = L.fn("wire_decode_json_device")(engine.handle, C.c_uint32(n), _dptr(arena), C.c_uint64(arena.numel()),
-                                                 _dptr(refs), _dptr(status), _dptr(mem), C.byref(sz[0]), _dptr(rep),
-                                                 C.byref(sz[1]), _dptr(dec), C.byref(sz[2]), st)
-            caps = [s.value for s in sz]
-            if rc != abi.GPX_ERANGE:
-                break
-    L.check(rc)
-    return JsonOut(status[:n], mem[: caps[0]], rep[: caps[1]], dec[: caps[2]], tuple(caps))
+        (mem, rep, dec), caps = _sized(
+            engine, caps, (C.c_uint32, C.c_uint32, C.c_uint32),
+            lambda c: (torch.empty((max(c[0], 1), 16), dtype=torch.uint8, device=dev),
+                       torch.empty((max(c[1], 1), 32), dtype=torch.uint8, device=dev),
+                       torch.empty((max(c[2], 1), 32), dtype=torch.uint8, device=dev)),
+            lambda o, sz: L.fn("wire_decode_json_device")(engine.handle, C.c_uint32(n), _dptr(arena),
+                                                          C.c_uint64(arena.numel()), _dptr(refs), _dptr(status),
+                                                          _dptr(o[0]), sz[0], _dptr(o[1]), sz[1], _dptr(o[2]), sz[2],
+                                                          st))
+    return JsonOut(status[:n], mem[: caps[0]], rep[: caps[1]], dec[: caps[2]], caps)
 
 
 # ---- the coordinator's side: REQUEST packets -> proposals -> ACCEPT packets, on the device ---------------------------
@@ -463,23 +454,18 @@ def decode_requests_device(engine, arena, refs, now_ms: int, caps, stream=None) 
     import torch
     n, dev = int(refs.shape[0]), refs.device
     L, st = engine.L, stream_handle(stream)
-    caps = [int(c) for c in caps]
     with _on(stream):
         status = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
-        for _ in range(2):
-            reqs = torch.empty((max(caps[0], 1), 32), dtype=torch.uint8, device=dev)
-            meta = torch.empty((max(caps[0], 1), 32), dtype=torch.uint8, device=dev)
-            pay = torch.empty(max(caps[1], 16), dtype=torch.uint8, device=dev)
-            nq, nb = C.c_uint32(caps[0]), C.c_uint64(caps[1])
-            rc = L.fn("wire_decode_requests_device")(engine.handle, C.c_uint32(n), _dptr(arena),
-                                                     C.c_uint64(arena.numel()), _dptr(refs), C.c_int64(now_ms),
-                                                     _dptr(status), _dptr(reqs), _dptr(meta), C.byref(nq), _dptr(pay),
-                                                     C.byref(nb), st)
-            caps = [nq.value, nb.value]
-            if rc != abi.GPX_ERANGE:
-                break
-    L.check(rc)
-    return RequestsOut(status[:n], reqs[: caps[0]], meta[: caps[0]], pay[: caps[1]], tuple(caps))
+        (reqs, meta, pay), caps = _sized(
+            engine, caps, (C.c_uint32, C.c_uint64),
+            lambda c: (torch.empty((max(c[0], 1), 32), dtype=torch.uint8, device=dev),
+                       torch.empty((max(c[0], 1), 32), dtype=torch.uint8, device=dev),
+                       torch.empty(max(c[1], 16), dtype=torch.uint8, device=dev)),
+            lambda o, sz: L.fn("wire_decode_requests_device")(engine.handle, C.c_uint32(n), _dptr(arena),
+                                                              C.c_uint64(arena.numel()), _dptr(refs), C.c_int64(now_ms),
+                                                              _dptr(status), _dptr(o[0]), _dptr(o[1]), sz[0],
+                                                              _dptr(o[2]), sz[1], st))
+    return RequestsOut(status[:n], reqs[: caps[0]], meta[: caps[0]], pay[: caps[1]], caps)
 
 
 def propose_device_heads(engine, reqs, n: int, payload, payload_bytes: int, status, accepts, heads, ctl, stream=None):

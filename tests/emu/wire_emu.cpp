@@ -1,7 +1,8 @@
 /*
- * wire_emu.cpp -- k_names_*, k_wire_decode and the k_wire_enc_* kernels (gigapaxos_b200/csrc/gpx_wire_dev.cuh, the
- * source the GPU runs) compiled for the host over cuda_emu.h; see p1b_emu.cpp.  The scans and the stable sorts by gid
- * that gpx_wire_host.inc does with CUB are done here with the standard library.  Test infrastructure only.
+ * wire_emu.cpp -- k_names_*, k_wire_decode, k_wire_req_decode and the k_wire_enc_* kernels
+ * (gigapaxos_b200/csrc/gpx_wire_dev.cuh, the source the GPU runs) compiled for the host over cuda_emu.h; see
+ * p1b_emu.cpp.  The scans and the stable sorts by gid that gpx_wire_host.inc does with CUB are done here with the
+ * standard library.  Test infrastructure only.
  */
 #include "cuda_emu.h"
 
@@ -115,6 +116,11 @@ static std::vector<uint32_t> stable_order(const std::vector<uint32_t>& key) {
   std::stable_sort(perm.begin(), perm.end(), [&](uint32_t a, uint32_t b) { return key[a] < key[b]; });
   return perm;
 }
+/* records into a stable order: dst[i] = src[perm[i]] */
+template <class T>
+static void gather(const std::vector<uint32_t>& perm, const std::vector<T>& src, T* dst) {
+  for (size_t i = 0; i < perm.size(); i++) dst[i] = src[perm[i]];
+}
 static void exclusive_rows(const std::vector<uint32_t>& cnt, std::vector<uint32_t>& off, uint32_t n, uint32_t rows,
                            uint64_t* tot) {
   for (uint32_t j = 0; j < rows; j++) {
@@ -165,16 +171,62 @@ extern "C" int emu_wire_decode(void* p, uint32_t n, const uint8_t* bytes, uint64
   A.dec_key = kd.data();
   A.emit = 1;
   emu_launch(k_wire_decode, (n + block - 1) / block, block, x->S, x->W, A);
-  std::vector<uint32_t> pa = stable_order(ka), pr = stable_order(kr), pd = stable_order(kd);
-  for (size_t i = 0; i < pa.size(); i++) acc[i] = sa[pa[i]];
-  for (size_t i = 0; i < pr.size(); i++) rep[i] = sr[pr[i]];
-  for (size_t i = 0; i < pd.size(); i++) dec[i] = sd[pd[i]];
+  gather(stable_order(ka), sa, acc);
+  gather(stable_order(kr), sr, rep);
+  gather(stable_order(kd), sd, dec);
   return 0;
 }
 
-/* gpx_wire_encode_replies (is_replies = 1, n records of n_lanes) / _decisions without the copies; sizes[2] = {bytes,
- * refs} in / out */
-extern "C" int emu_wire_encode(void* p, int is_replies, uint32_t n, const void* recs, uint8_t* rstatus, uint8_t* out,
+/* gpx_wire_decode_requests_device without the copies; sizes[2] = {requests, payload bytes} in / out; GPX_ERANGE when
+ * an output is too small (nothing but status written then) */
+extern "C" int emu_wire_decode_requests(void* p, uint32_t n, const uint8_t* bytes, uint64_t n_bytes,
+                                        const gpx_wire_ref* pkts, int64_t now_ms, int32_t* status,
+                                        gpx_request_rec* reqs, gpx_wire_req_meta* meta, uint8_t* payload,
+                                        uint64_t* sizes, uint32_t block) {
+  EmuWire* x = static_cast<EmuWire*>(p);
+  std::vector<uint32_t> cnt((size_t)WQ_NCNT * n + 1), off((size_t)WQ_NCNT * n + 1);
+  WireReqDecodeArgs A;
+  memset(&A, 0, sizeof A);
+  A.bytes = bytes;
+  A.pkts = pkts;
+  A.n_bytes = n_bytes;
+  A.n = n;
+  A.now_ms = now_ms;
+  A.cnt = cnt.data();
+  A.off = off.data();
+  A.status = status;
+  emu_launch(k_wire_req_decode, (n + block - 1) / block, block, x->S, x->W, A);
+  uint64_t tot[WQ_NCNT];
+  exclusive_rows(cnt, off, n, WQ_NCNT, tot);
+  const bool small = tot[WQ_REQ] > sizes[0] || tot[WQ_PAY] > sizes[1];
+  sizes[0] = tot[WQ_REQ];
+  sizes[1] = tot[WQ_PAY];
+  if (small) return GPX_ERANGE;
+  const size_t nq = tot[WQ_REQ];
+  std::vector<gpx_request_rec> sq(nq + 1);
+  std::vector<gpx_wire_req_meta> sm(nq + 1);
+  std::vector<uint32_t> key(nq);
+  A.req = sq.data();
+  A.meta = sm.data();
+  A.key = key.data();
+  A.payload = payload;
+  A.emit = 1;
+  emu_launch(k_wire_req_decode, (n + block - 1) / block, block, x->S, x->W, A);
+  const std::vector<uint32_t> perm = stable_order(key);
+  gather(perm, sq, reqs);
+  gather(perm, sm, meta);
+  return 0;
+}
+
+enum { EMU_ENC_REPLIES = 0, EMU_ENC_DECISIONS = 1, EMU_ENC_ACCEPTS = 2 };
+
+/* gpx_wire_encode_replies (kind 0: n records of n_lanes), gpx_wire_encode_decisions (1) or
+ * gpx_wire_encode_accepts_device (2, the ACCEPTs' requests at heads .. payload) without the copies.  The keys, the sort
+ * and the passes run over n records; n_ptr, when not null, is the record count as the device reads it.  sizes[2] =
+ * {bytes, refs} in / out. */
+extern "C" int emu_wire_encode(void* p, int kind, const uint32_t* n_ptr, uint32_t n, const void* recs,
+                               const uint32_t* heads, const gpx_request_rec* reqs, const gpx_wire_req_meta* meta,
+                               uint32_t n_reqs, const uint8_t* payload, uint8_t* rstatus, uint8_t* out,
                                gpx_wire_ref* refs, uint64_t* sizes, uint32_t block) {
   EmuWire* x = static_cast<EmuWire*>(p);
   std::vector<uint32_t> key(n + 1), perm, skey(n + 1), cnt(2 * (size_t)n + 1), off(2 * (size_t)n + 1);
@@ -185,10 +237,26 @@ extern "C" int emu_wire_encode(void* p, int is_replies, uint32_t n, const void* 
   A.n_lanes = x->S.L;
   A.rstatus = rstatus;
   A.key = key.data();
-  if (is_replies)
-    emu_launch(k_wire_enc_keys_replies, (n + block - 1) / block, block, x->S, x->W, A);
-  else
-    emu_launch(k_wire_enc_keys_decisions, (n + block - 1) / block, block, x->S, x->W, A);
+  A.n_ptr = n_ptr;
+  WireAccArgs X;
+  X.head = heads;
+  X.reqs = reqs;
+  X.meta = meta;
+  X.n_reqs = n_reqs;
+  X.payload = payload;
+  const uint32_t grid = (n + block - 1) / block;
+  const auto launch = [&](bool keys) {
+    if (kind == EMU_ENC_REPLIES)
+      keys ? emu_launch(k_wire_enc_keys_replies, grid, block, x->S, x->W, A)
+           : emu_launch(k_wire_enc_replies, grid, block, x->S, x->W, A);
+    else if (kind == EMU_ENC_DECISIONS)
+      keys ? emu_launch(k_wire_enc_keys_decisions, grid, block, x->S, x->W, A)
+           : emu_launch(k_wire_enc_decisions, grid, block, x->S, x->W, A);
+    else
+      keys ? emu_launch(k_wire_enc_keys_accepts, grid, block, x->S, x->W, A, X)
+           : emu_launch(k_wire_enc_accepts, grid, block, x->S, x->W, A, X);
+  };
+  launch(true);
   key.resize(n);
   perm = stable_order(key);
   for (uint32_t i = 0; i < n; i++) skey[i] = key[perm[i]];
@@ -196,10 +264,7 @@ extern "C" int emu_wire_encode(void* p, int is_replies, uint32_t n, const void* 
   A.skey = skey.data();
   A.cnt = cnt.data();
   A.off = off.data();
-  if (is_replies)
-    emu_launch(k_wire_enc_replies, (n + block - 1) / block, block, x->S, x->W, A);
-  else
-    emu_launch(k_wire_enc_decisions, (n + block - 1) / block, block, x->S, x->W, A);
+  launch(false);
   uint64_t tot[2];
   exclusive_rows(cnt, off, n, 2, tot);
   const bool small = tot[0] > sizes[0] || tot[1] > sizes[1];
@@ -209,9 +274,6 @@ extern "C" int emu_wire_encode(void* p, int is_replies, uint32_t n, const void* 
   A.out = out;
   A.refs = refs;
   A.emit = 1;
-  if (is_replies)
-    emu_launch(k_wire_enc_replies, (n + block - 1) / block, block, x->S, x->W, A);
-  else
-    emu_launch(k_wire_enc_decisions, (n + block - 1) / block, block, x->S, x->W, A);
+  launch(false);
   return 0;
 }

@@ -103,8 +103,7 @@ extern "C" int emu_wire_decode_json(void* p, uint32_t n, const uint8_t* bytes, u
   A.emit = 1;
   const uint32_t nm_all = poff[2 * n - 1] + pcnt[2 * n - 1];
   emu_launch(k_json_member, grid(nm_all), block, x->S, x->W, A);
-  std::vector<uint32_t> pr = stable_order(kr), pd = stable_order(kd);
-  for (size_t i = 0; i < pr.size(); i++) rep[i] = sr[pr[i]];
-  for (size_t i = 0; i < pd.size(); i++) dec[i] = sd[pd[i]];
+  gather(stable_order(kr), sr, rep);
+  gather(stable_order(kd), sd, dec);
   return 0;
 }

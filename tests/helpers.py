@@ -16,6 +16,7 @@ from gigapaxos_b200.abi import GpxError as GpxErrorT  # noqa: E402
 
 ORACLE_PATH = os.path.join(ROOT, "oracle", "libgpx_oracle.so")
 _oracle = None
+_wire_emu = None
 
 
 def oracle_library() -> Library:
@@ -27,6 +28,31 @@ def oracle_library() -> Library:
             build.build_oracle()
         _oracle = Library(ORACLE_PATH, "gpxo_")
     return _oracle
+
+
+def wire_emu_library(tmp_path_factory):
+    """tests/emu/wire_emu.cpp, the wire kernels' source compiled for the host (under AddressSanitizer + UBSan when
+    GPX_EMU_SANITIZE is set), built once per process; skips the test without the CUDA headers"""
+    global _wire_emu
+    if _wire_emu is None:
+        import ctypes as C
+        import subprocess
+
+        import pytest
+        cuda_inc = "/usr/local/cuda/include"
+        if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
+            pytest.skip("no CUDA headers")
+        sanitize = (["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"]
+                    if os.environ.get("GPX_EMU_SANITIZE") else [])
+        out = str(tmp_path_factory.mktemp("emu") / "libwire_emu.so")
+        subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *sanitize, "-I", cuda_inc,
+                               "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
+                               "-x", "c++", os.path.join(ROOT, "tests", "emu", "wire_emu.cpp"), "-o", out])
+        lib = C.CDLL(out)
+        lib.emu_wire_new.restype = C.c_void_p
+        lib.emu_wire_new.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p]
+        _wire_emu = lib
+    return _wire_emu
 
 
 def make_config(lib: Library, **kw) -> abi.Config:

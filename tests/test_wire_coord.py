@@ -1,5 +1,5 @@
 """CPU: the coordinator's wire kernels (gigapaxos_b200/csrc/gpx_wire_dev.cuh: k_wire_req_decode, k_wire_enc_keys_accepts,
-k_wire_enc_accepts) compiled for the host (tests/emu/wire_coord_emu.cpp).
+k_wire_enc_accepts) compiled for the host (tests/emu/wire_emu.cpp).
 
 * Decode: seeded REQUEST packets (singles, batched with 1-20 latched requests, empty values, every address and flag
   combination, entryReplica set and unset) give the requests and meta that the host codec's fields and
@@ -18,8 +18,8 @@ import sys
 import numpy as np
 import pytest
 
-from helpers import ROOT, abi
-from test_wire_dev import SANITIZE, Emu
+from helpers import ROOT, abi, wire_emu_library
+from test_wire_dev import ENC_ACCEPTS, Emu
 from wire_coord_cases import (NOW_MS, check_requests, expected_accepts, malformed_request_packets, propose_blob,
                               random_accepts, random_request_packets)
 from wire_dev_cases import random_world
@@ -33,20 +33,7 @@ def ptr(a):
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    cuda_inc = "/usr/local/cuda/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("no CUDA headers")
-    out = str(tmp_path_factory.mktemp("emu") / "libwire_coord_emu.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *SANITIZE, "-I", cuda_inc,
-                           "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
-                           "-x", "c++", os.path.join(ROOT, "tests", "emu", "wire_coord_emu.cpp"), "-o", out])
-    lib = C.CDLL(out)
-    lib.emu_wire_new.restype = C.c_void_p
-    lib.emu_wire_new.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p]
-    for f in ("emu_wire_free", "emu_wire_group", "emu_wire_names", "emu_wire_names_remove", "emu_wire_names_rehash",
-              "emu_wire_decode", "emu_wire_encode", "emu_wire_decode_requests", "emu_wire_encode_accepts"):
-        getattr(lib, f).argtypes = None
-    return lib
+    return wire_emu_library(tmp_path_factory)
 
 
 def decode_requests(e: Emu, pkts, block=64):
@@ -72,22 +59,8 @@ def decode_requests(e: Emu, pkts, block=64):
 
 def encode_accepts(e: Emu, acc, heads, reqs, meta, payload, count=None, block=64):
     """(rstatus[n_max], [(gid, node, bytes)]); count = the device count (None: all)"""
-    n_max = len(acc)
-    n_ptr = np.array([n_max if count is None else count], np.uint32)
-    rst = np.full(max(n_max, 1), 0xAB, np.uint8)
-    sizes = np.zeros(2, np.uint64)
-    z = np.zeros(16, np.uint8)
-    acc, heads = np.ascontiguousarray(acc), np.ascontiguousarray(heads)
-    a_p, h_p = (ptr(acc), ptr(heads)) if len(acc) else (None, None)
-    args = lambda out, refs: (e.h, ptr(n_ptr), C.c_uint32(n_max), a_p, h_p, ptr(reqs), ptr(meta), C.c_uint32(len(reqs)),
-                              ptr(payload), ptr(rst), ptr(out), ptr(refs), ptr(sizes), C.c_uint32(block))
-    rc = e.lib.emu_wire_encode_accepts(*args(z, z))
-    assert rc in (0, abi.GPX_ERANGE)
-    out = np.zeros(max(int(sizes[0]), 1), np.uint8)
-    refs = np.zeros(max(int(sizes[1]), 1), abi.wire_ref_dtype)
-    rst[:] = 0xAB
-    assert e.lib.emu_wire_encode_accepts(*args(out, refs)) == 0
-    return rst[:n_max], wire.unpack_packets(out, refs[: int(sizes[1])])
+    return e.encode_kind(ENC_ACCEPTS, acc, len(acc), count=len(acc) if count is None else count,
+                         accepts=(heads, reqs, meta, payload), block=block)
 
 
 @pytest.mark.parametrize("seed", [1, 2, 3])
@@ -162,9 +135,10 @@ def test_local_groups_and_no_memory_past_the_count(emu):
         sizes = np.array([1 << 24, 1 << 16], np.uint64)
         out = np.zeros(1 << 24, np.uint8)
         refs = np.zeros(1 << 16, abi.wire_ref_dtype)
-        assert e.lib.emu_wire_encode_accepts(e.h, ptr(n_ptr), C.c_uint32(len(acc) + 50), ptr(a) if k else None,
-                                             ptr(h) if k else None, ptr(reqs), ptr(meta), C.c_uint32(len(reqs)),
-                                             ptr(pay), ptr(rst), ptr(out), ptr(refs), ptr(sizes), C.c_uint32(64)) == 0
+        assert e.lib.emu_wire_encode(e.h, C.c_int(ENC_ACCEPTS), ptr(n_ptr), C.c_uint32(len(acc) + 50),
+                                     ptr(a) if k else None, ptr(h) if k else None, ptr(reqs), ptr(meta),
+                                     C.c_uint32(len(reqs)), ptr(pay), ptr(rst), ptr(out), ptr(refs), ptr(sizes),
+                                     C.c_uint32(64)) == 0
         assert np.array_equal(rst[:k], want_rst) and (rst[k:] == 0xAB).all()
         assert wire.unpack_packets(out, refs[: int(sizes[1])]) == want
     e.lib.emu_wire_free(e.h)

@@ -12,14 +12,14 @@ import sys
 import numpy as np
 import pytest
 
-from helpers import ROOT, abi
+from helpers import ROOT, abi, wire_emu_library
 from wire_dev_cases import (World, check_decode, expected_encode_decisions, expected_encode_replies, malformed_packets,
                             random_decisions, random_packets, random_replies, random_world)
 
 from gigapaxos_b200 import wire
 
-SANITIZE = ["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"] if os.environ.get("GPX_EMU_SANITIZE") else []
 GOLD = json.load(open(os.path.join(ROOT, "tests", "golden", "wire_vectors.json")))
+ENC_REPLIES, ENC_DECISIONS, ENC_ACCEPTS = 0, 1, 2  # the encoders of emu_wire_encode
 
 
 def ptr(a):
@@ -28,20 +28,7 @@ def ptr(a):
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    cuda_inc = "/usr/local/cuda/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("no CUDA headers")
-    out = str(tmp_path_factory.mktemp("emu") / "libwire_emu.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *SANITIZE, "-I", cuda_inc,
-                           "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
-                           "-x", "c++", os.path.join(ROOT, "tests", "emu", "wire_emu.cpp"), "-o", out])
-    lib = C.CDLL(out)
-    lib.emu_wire_new.restype = C.c_void_p
-    lib.emu_wire_new.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p]
-    for f in ("emu_wire_free", "emu_wire_group", "emu_wire_names", "emu_wire_names_remove", "emu_wire_names_rehash",
-              "emu_wire_decode", "emu_wire_encode"):
-        getattr(lib, f).argtypes = None
-    return lib
+    return wire_emu_library(tmp_path_factory)
 
 
 class Emu:
@@ -95,19 +82,31 @@ class Emu:
         return status[:n], acc[: int(sizes[0])], blob[: int(sizes[1])], rep[: int(sizes[2])], dec[: int(sizes[3])]
 
     def encode(self, recs, is_replies, block=64):
-        n = len(recs)
-        rst = np.zeros(max(n, 1), np.uint8)
+        return self.encode_kind(ENC_REPLIES if is_replies else ENC_DECISIONS, recs, len(recs), block=block)
+
+    def encode_kind(self, kind, recs, n_max, count=None, accepts=None, block=64):
+        """emu_wire_encode over n_max records of recs, the sizes first; count = the record count the device reads (None:
+        no device count), accepts = the ACCEPTs' (heads, reqs, meta, payload) -> (rstatus[n_max], packets), rstatus
+        0xAB where the encoder wrote none"""
+        cnt = None if count is None else np.array([count], np.uint32)
+        recs = np.ascontiguousarray(recs)
+        heads, reqs, meta, pay = accepts if accepts is not None else (None, None, None, None)
+        heads = None if heads is None else np.ascontiguousarray(heads)
+        rst = np.full(max(n_max, 1), 0xAB, np.uint8)
         sizes = np.zeros(2, np.uint64)
         z = np.zeros(16, np.uint8)
-        recs = np.ascontiguousarray(recs)
-        rc = self.lib.emu_wire_encode(self.h, C.c_int(is_replies), C.c_uint32(n), ptr(recs), ptr(rst), ptr(z), ptr(z),
-                                      ptr(sizes), C.c_uint32(block))
+        opt = lambda a: None if a is None else ptr(a)
+        r_p, h_p = (ptr(recs), opt(heads)) if len(recs) else (None, None)
+        args = lambda out, refs: (self.h, C.c_int(kind), opt(cnt), C.c_uint32(n_max), r_p, h_p, opt(reqs), opt(meta),
+                                  C.c_uint32(0 if reqs is None else len(reqs)), opt(pay), ptr(rst), ptr(out), ptr(refs),
+                                  ptr(sizes), C.c_uint32(block))
+        rc = self.lib.emu_wire_encode(*args(z, z))
         assert rc in (0, abi.GPX_ERANGE)
         out = np.zeros(max(int(sizes[0]), 1), np.uint8)
         refs = np.zeros(max(int(sizes[1]), 1), abi.wire_ref_dtype)
-        assert self.lib.emu_wire_encode(self.h, C.c_int(is_replies), C.c_uint32(n), ptr(recs), ptr(rst), ptr(out),
-                                        ptr(refs), ptr(sizes), C.c_uint32(block)) == 0
-        return rst[:n], wire.unpack_packets(out, refs[: int(sizes[1])])
+        rst[:] = 0xAB
+        assert self.lib.emu_wire_encode(*args(out, refs)) == 0
+        return rst[:n_max], wire.unpack_packets(out, refs[: int(sizes[1])])
 
     def close(self):
         self.lib.emu_wire_free(self.h)

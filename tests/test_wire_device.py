@@ -1,8 +1,7 @@
 """CPU: the decisions encoder of gpx_wire_encode_decisions_device, whose record count is read on the device from
-*n_ptr, as kernel source compiled for the host (tests/emu/wire_device_emu.cpp).  Records past the count -- valid-looking
+*n_ptr, as kernel source compiled for the host (tests/emu/wire_emu.cpp).  Records past the count -- valid-looking
 ones in the buffer, or no memory at all -- are never encoded, never read and get no rstatus: the packets, refs and
 rstatus[0:*n_ptr] equal encoding only the counted records.  Also once more under AddressSanitizer + UBSan."""
-import ctypes as C
 import os
 import subprocess
 import sys
@@ -10,52 +9,19 @@ import sys
 import numpy as np
 import pytest
 
-from helpers import ROOT, abi
-from test_wire_dev import SANITIZE, Emu
+from helpers import ROOT, wire_emu_library
+from test_wire_dev import ENC_DECISIONS, Emu
 from wire_dev_cases import expected_encode_decisions, random_decisions, random_world
-
-from gigapaxos_b200 import wire
-
-
-def ptr(a):
-    return a.ctypes.data_as(C.c_void_p)
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    cuda_inc = "/usr/local/cuda/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("no CUDA headers")
-    out = str(tmp_path_factory.mktemp("emu") / "libwire_device_emu.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *SANITIZE, "-I", cuda_inc,
-                           "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
-                           "-x", "c++", os.path.join(ROOT, "tests", "emu", "wire_device_emu.cpp"), "-o", out])
-    lib = C.CDLL(out)
-    lib.emu_wire_new.restype = C.c_void_p
-    lib.emu_wire_new.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p]
-    for f in ("emu_wire_free", "emu_wire_group", "emu_wire_names", "emu_wire_names_remove", "emu_wire_names_rehash",
-              "emu_wire_decode", "emu_wire_encode", "emu_wire_encode_decisions_n"):
-        getattr(lib, f).argtypes = None
-    return lib
+    return wire_emu_library(tmp_path_factory)
 
 
 def encode_counted(e: Emu, recs, count, n_max, block):
     """the device-count encoder over recs (n_max records, or only `count` of them in memory) -> (rstatus, packets)"""
-    n_ptr = np.array([count], np.uint32)
-    rst = np.full(max(n_max, 1), 0xAB, np.uint8)
-    sizes = np.zeros(2, np.uint64)
-    z = np.zeros(16, np.uint8)
-    recs = np.ascontiguousarray(recs)
-    rp = ptr(recs) if len(recs) else None
-    rc = e.lib.emu_wire_encode_decisions_n(e.h, ptr(n_ptr), C.c_uint32(n_max), rp, ptr(rst), ptr(z), ptr(z),
-                                           ptr(sizes), C.c_uint32(block))
-    assert rc in (0, abi.GPX_ERANGE)
-    out = np.zeros(max(int(sizes[0]), 1), np.uint8)
-    refs = np.zeros(max(int(sizes[1]), 1), abi.wire_ref_dtype)
-    rst[:] = 0xAB
-    assert e.lib.emu_wire_encode_decisions_n(e.h, ptr(n_ptr), C.c_uint32(n_max), rp, ptr(rst), ptr(out), ptr(refs),
-                                             ptr(sizes), C.c_uint32(block)) == 0
-    return rst[:n_max], wire.unpack_packets(out, refs[: int(sizes[1])])
+    return e.encode_kind(ENC_DECISIONS, recs, n_max, count=count, block=block)
 
 
 @pytest.mark.parametrize("seed", [4, 5, 6])

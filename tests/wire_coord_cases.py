@@ -1,5 +1,5 @@
 """Cases and expectations shared by tests/test_wire_coord.py (the coordinator's wire kernels on the host,
-tests/emu/wire_coord_emu.cpp) and tests/test_wire_coord_gpu.py (the same kernels through the C ABI): REQUEST packets
+tests/emu/wire_emu.cpp) and tests/test_wire_coord_gpu.py (the same kernels through the C ABI): REQUEST packets
 made by the host codec and what decoding them must give, and ACCEPT records with their requests and the AcceptPacket
 bytes gpx_wire_encode_accept writes for them."""
 from __future__ import annotations
