@@ -78,7 +78,8 @@ struct gpx_engine {
   RoundCtl* d_rctl = nullptr; /* [2] the round kernels' own control blocks: they alternate as the working block, each
                                * round zeroes the one the next round counts into */
   const RoundCtl* last_ctl = nullptr; /* where the last round left its counters */
-  int round_mode = 0;         /* gpx_set_round_mode: 0 / 1 device tail launch of k_round_slow, 2 host-launched pair */
+  int round_mode = 0;         /* gpx_set_round_mode: 0 / 1 device tail launch of k_round_slow, 2 host-launched pair;
+                               * 3 / 4 the same two with the team kernel k_round in place of k_round_g */
   uint32_t rparity = 0;
   RoundCtl* h_ctl = nullptr; /* pinned */
   void* d_misc = nullptr;    /* group-management staging */
@@ -319,7 +320,7 @@ int gpx_engine_create(const gpx_config* cfg, gpx_engine** out) {
   }
   cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking);
   for (int i = 0; i < 5; i++) cudaEventCreate(&e->ev[i]);
-  if (const char* rm = getenv("GPX_ROUND_MODE")) e->round_mode = atoi(rm) >= 0 && atoi(rm) <= 2 ? atoi(rm) : 0; /* tuning / tests */
+  if (const char* rm = getenv("GPX_ROUND_MODE")) e->round_mode = atoi(rm) >= 0 && atoi(rm) <= 4 ? atoi(rm) : 0; /* tuning / tests */
   e->h_version.assign(G, 0);
   e->h_name_hash.assign(G, 0);
   cudaError_t err = cudaDeviceSynchronize();
@@ -652,14 +653,30 @@ static int launch_commit(gpx_engine* e, const gpx_decision_rec* d_dec, const uin
   return GPX_OK;
 }
 
-/* k_round<L, LP, DEF>: LP = L (team width); DEF = the reference's default configuration folded at compile time */
+/* k_round_g<L, DEF> (one thread per group) where it is built, k_round<L, LP, DEF> (a team of LP = L threads per group)
+ * otherwise or when `team` forces it; DEF = the reference's default configuration folded at compile time */
 extern "C++" {
 template <int L, int LP>
-static void launch_round_t(uint32_t grid, cudaStream_t st, const DevState& S, const RoundArgs& RA) {
-  if (S.journaling && S.gc_majority_executed && S.log_meta && !S.cpi_per_group)
-    k_round<L, LP, true><<<grid, GPX_RBLOCK, 0, st>>>(S, RA);
-  else
-    k_round<L, LP, false><<<grid, GPX_RBLOCK, 0, st>>>(S, RA);
+static void launch_round_t(uint32_t n, bool team, cudaStream_t st, const DevState& S, const RoundArgs& RA) {
+  const bool def = S.journaling && S.gc_majority_executed && S.log_meta && !S.cpi_per_group;
+  bool done = false;
+  if constexpr (L <= GPX_GROUND_MAXL) {
+    if (!team) {
+      const uint32_t grid = cdiv((uint64_t)n, GPX_GBLOCK);
+      if (def)
+        k_round_g<L, true><<<grid, GPX_GBLOCK, 0, st>>>(S, RA);
+      else
+        k_round_g<L, false><<<grid, GPX_GBLOCK, 0, st>>>(S, RA);
+      done = true;
+    }
+  }
+  if (!done) {
+    const uint32_t grid = cdiv((uint64_t)n, (GPX_RBLOCK / 32u) * (32u / LP)); /* teams of L adjacent lanes */
+    if (def)
+      k_round<L, LP, true><<<grid, GPX_RBLOCK, 0, st>>>(S, RA);
+    else
+      k_round<L, LP, false><<<grid, GPX_RBLOCK, 0, st>>>(S, RA);
+  }
   if (!RA.tail_launch) { /* host-launched pair; programmatic dependent launch hides k_round_slow's launch latency */
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof cfg);
@@ -731,17 +748,18 @@ static int launch_round(gpx_engine* e, const gpx_request_rec* d_reqs, const uint
   const uint32_t teams_per_block = (GPX_RBLOCK / 32u) * (32u / L); /* teams of L adjacent lanes */
   const uint32_t grid = cdiv((uint64_t)n, teams_per_block);
   RA.slow_grid = std::min<uint32_t>(grid, 2u * (uint32_t)e->n_sms);
-  RA.tail_launch = e->round_mode == 2 ? 0u : 1u; /* grid-stride over the todo list; all
+  RA.tail_launch = (e->round_mode == 2 || e->round_mode == 4) ? 0u : 1u; /* grid-stride over the todo list; all
                                                                             * blocks resident (grid barriers) */
+  const bool team = e->round_mode >= 3;
   switch (L) {
-    case 1: launch_round_t<1, 1>(grid, st, e->S, RA); break;
-    case 2: launch_round_t<2, 2>(grid, st, e->S, RA); break;
-    case 3: launch_round_t<3, 3>(grid, st, e->S, RA); break;
-    case 4: launch_round_t<4, 4>(grid, st, e->S, RA); break;
-    case 5: launch_round_t<5, 5>(grid, st, e->S, RA); break;
-    case 6: launch_round_t<6, 6>(grid, st, e->S, RA); break;
-    case 7: launch_round_t<7, 7>(grid, st, e->S, RA); break;
-    default: launch_round_t<8, 8>(grid, st, e->S, RA); break;
+    case 1: launch_round_t<1, 1>(n, team, st, e->S, RA); break;
+    case 2: launch_round_t<2, 2>(n, team, st, e->S, RA); break;
+    case 3: launch_round_t<3, 3>(n, team, st, e->S, RA); break;
+    case 4: launch_round_t<4, 4>(n, team, st, e->S, RA); break;
+    case 5: launch_round_t<5, 5>(n, team, st, e->S, RA); break;
+    case 6: launch_round_t<6, 6>(n, team, st, e->S, RA); break;
+    case 7: launch_round_t<7, 7>(n, team, st, e->S, RA); break;
+    default: launch_round_t<8, 8>(n, team, st, e->S, RA); break;
   }
   log_flip(e);
   CK(cudaGetLastError());
@@ -1098,7 +1116,8 @@ static int round_on_stream(gpx_engine* e, bool fused, const gpx_request_rec* d_r
 
 int gpx_set_round_mode(gpx_engine* e, int mode) {
   if (!e) return fail(GPX_EINVAL, "null argument");
-  if (mode < 0 || mode > 2) return fail(GPX_EINVAL, "round mode: 0 / 1 device tail launch, 2 host-launched pair");
+  if (mode < 0 || mode > 4)
+    return fail(GPX_EINVAL, "round mode: 0 / 1 device tail launch, 2 host-launched pair, 3 / 4 the same with k_round");
   e->round_mode = mode;
   return GPX_OK;
 }

@@ -3,8 +3,10 @@
  * round (RequestBatcher -> propose -> accept x R -> tally -> commit x R) for co-located replicas.
  *
  * Work mapping: a TEAM of L threads (adjacent lanes of one warp, 32/L teams per warp) owns one request index;
- * team thread `sub` is replica lane `sub` of the group.  Two kernels:
+ * team thread `sub` is replica lane `sub` of the group.  Three kernels:
  *
+ *   k_round_g     (below k_round) the same in-order case with ONE thread per group, owning all L lanes: the default
+ *                 for L <= GPX_GROUND_MAXL; k_round serves larger L and gpx_set_round_mode 3 / 4.
  *   k_round       the in-order case, straight-line predicated code.  Every thread loads ITS lane's acceptor row,
  *                 aux word and coordinator row (+ the group's meta word and the first payload chunk); the entry
  *                 lane's and the coordinator lane's rows reach the team by full-warp __shfl_sync
@@ -638,6 +640,350 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
     const uint32_t nc = __reduce_add_sync(FULL, c_ckpt);
     if (lane_id == 0 && (nl | nt)) { /* aggregates, expanded by gpx_get_counters */
       atomicAdd(&s_ctr[C_FAST_LANES], nl);
+      atomicAdd(&s_ctr[C_FAST_TEAMS], nt);
+      if (nc) atomicAdd(&s_ctr[C_FAST_CKPT], nc);
+    }
+  }
+  flush_counters(S, s_ctr);
+}
+
+#ifndef GPX_GBLOCK
+#define GPX_GBLOCK 128 /* threads (= groups) per block of k_round_g */
+#endif
+#ifndef GPX_GROUND_MINB
+#define GPX_GROUND_MINB 6 /* at most 80 registers per thread, no spills at L <= 3: 6 blocks = 768 groups in flight per \
+                           * SM, so 100 K groups (782 blocks) run in ONE wave on a 132-SM H100.  At 96 registers (5 \
+                           * blocks, 1.2 waves) k_round_g took 28.2 us at 100 K groups, at 80 registers 24.1-24.9 us; \
+                           * 72 registers (7 blocks) was no faster at 100 K and 2 % slower at 1 M groups */
+#endif
+#ifndef GPX_GROUND_MAXL
+#define GPX_GROUND_MAXL 3 /* k_round_g is built for L <= this; larger L keeps k_round (at L = 4, 5 k_round_g is \
+                           * spill-free but made the R = 5 workload slower on an H100) */
+#endif
+
+/*
+ * The fast kernel with one THREAD per group: the thread owns request i and all L lanes of its group.  Same inputs,
+ * load levels, in-order predicate and durable outputs as k_round; the team vote is an AND over the lanes held in
+ * registers, the entry lane's and the coordinator lane's rows are register selects, and nothing is shuffled.  A warp
+ * serves 32 adjacent groups, so every per-lane plane access (acc_row, acc_aux, coord_row, node_slots, the frame
+ * records) is 32 x 4..16 B contiguous: whole lines per instruction.  The log images are staged per warp as in
+ * k_round; a warp whose 32 groups all took the fast path stages its EXEC rows too and stores them as 16-byte pieces.
+ */
+template <int L, bool DEF>
+__global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const __grid_constant__ DevState S,
+                                                                       const __grid_constant__ RoundArgs RA) {
+  const bool cf_journaling = DEF ? true : (S.journaling != 0);
+  const bool cf_gcme = DEF ? true : (S.gc_majority_executed != 0);
+  const bool cf_logmeta = DEF ? true : (S.log_meta != 0);
+  const bool cf_cpi_pg = DEF ? false : (S.cpi_per_group != 0);
+  constexpr uint32_t FULL = 0xffffffffu;
+  constexpr uint32_t TPB = GPX_GBLOCK; /* groups (= requests) per block */
+  __shared__ unsigned int s_ctr[C_NCTR];
+  __shared__ __align__(128) gpx_request_rec s_req[TPB + 2];
+  __shared__ __align__(8) unsigned long long s_bar;
+  /* per warp: the ACCEPT and DECISION images, [kind x lane][group][half] x 16 B; afterwards the warp's EXEC rows,
+   * [group][lane] x 24 B, when they are stored as 16-byte pieces */
+  __shared__ __align__(16) int4 s_img[GPX_GBLOCK / 32u][4 * L * 32];
+  static_assert(32 * L * sizeof(gpx_exec_rec) <= sizeof(s_img[0]), "EXEC staging fits the image buffer");
+  if (threadIdx.x < C_NCTR) s_ctr[threadIdx.x] = 0;
+  if (threadIdx.x == 0) mbar_init(&s_bar, 1);
+  __syncthreads();
+  const AcceptArgs& A = RA.A;
+  const gpx_request_rec* reqs = RA.P.reqs;
+  const uint32_t n = RA.P.n;
+  const uint32_t r0 = blockIdx.x * TPB; /* first request of the block; records [t0, t1) are staged */
+  const uint32_t t0 = r0 ? r0 - 1u : 0u, t1 = min(n, r0 + TPB + 1u);
+  const uint32_t tile_bytes = t1 > t0 ? (t1 - t0) * (uint32_t)sizeof(gpx_request_rec) : 0u;
+  if (threadIdx.x == 0 && tile_bytes) tma_load_1d(s_req, &reqs[t0], tile_bytes, &s_bar);
+  const uint32_t lane_id = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+  const uint32_t i = r0 + threadIdx.x;
+  const uint32_t G = S.G, Wm = S.W - 1;
+  const unsigned long long pay_bytes = RA.pay_bytes, res_a = RA.res_a, res_d = RA.res_d;
+  const uint32_t pay_rel = RA.pay_rel;
+  unsigned long long seg[L]; /* every lane's segment base (DevState.lp's copy of log_pos) */
+#pragma unroll
+  for (int l = 0; l < L; l++) seg[l] = seg_base(S, l, res_a + res_d);
+  if (blockIdx.x == 0 && threadIdx.x < (uint32_t)L) { /* thread l writes lane l's two segment headers */
+    const uint32_t t = threadIdx.x;
+    const unsigned long long sg = seg_base(S, t, res_a + res_d), sq = seg_seq_of(S, t);
+    write_seg_hdr(S, t, sg, GPX_F_ACCEPT, n, n, pay_bytes, 48, sq);
+    write_seg_hdr(S, t, sg + res_a, GPX_F_DECISION, n, n, 0, 32, sq + 1ull);
+    log_publish(S, t, sg + res_a + res_d, sq + 2ull);
+    S.cur_seg[t] = sg;
+    if (t == 0) {
+      atomicAdd(&s_ctr[C_KERNEL_LAUNCHES], 1u);
+      if (RA.ctl_zero) {
+        int4* z = reinterpret_cast<int4*>(RA.ctl_zero);
+        z[0] = make_int4(0, 0, 0, 0);
+        z[1] = make_int4(0, 0, 0, 0);
+      }
+    }
+  }
+
+  /* ---- level A: the request record and the neighbours' gids ---- */
+  const bool valid = i < n;
+  int4 rq0 = make_int4(0, 0, 0, 0), rq1 = rq0;
+  uint32_t gprev = 0xffffffffu, gnext = 0xffffffffu;
+  if (tile_bytes) mbar_wait(&s_bar, 0);
+  if (valid) {
+    const int4* rp = reinterpret_cast<const int4*>(&s_req[i - t0]);
+    rq0 = rp[0];
+    rq1 = rp[1];
+    if (i > 0) gprev = s_req[i - t0 - 1].gid;
+    if (i + 1 < n) gnext = s_req[i - t0 + 1].gid;
+  }
+  const uint32_t gid = (uint32_t)rq0.x, rflags = (uint32_t)rq0.y, entry = (rflags >> 8) & 0xfu;
+  const uint32_t poff = (uint32_t)rq1.x, plen = (uint32_t)rq1.y;
+  const bool head = valid && (i == 0 || gprev != gid);
+  const bool cand = head && gnext != gid && gid < G && entry < (uint32_t)L && !(rflags & GPX_F_STOP);
+
+  /* ---- level B: group meta and, for every lane, its acceptor row, aux word, coordinator row and the
+   * nodeSlotNumbers it holds for every lane that may coordinate; the first payload chunk ---- */
+  uint32_t meta = 0, aux[L], dirty[L];
+  int4 arow[L], crw[L];
+  int ns_all[L][L]; /* [coordinator lane c][lane l] */
+#pragma unroll
+  for (int l = 0; l < L; l++) {
+    aux[l] = 0;
+    dirty[l] = 1;
+    arow[l] = crw[l] = make_int4(0, 0, 0, 0);
+#pragma unroll
+    for (int c = 0; c < L; c++) ns_all[c][l] = 0;
+  }
+  int4 pv = make_int4(0, 0, 0, 0);
+  const uint8_t* const psrc = A.blob0 + poff;
+  const bool pal = ((poff | (uint32_t)(uintptr_t)A.blob0) & 15u) == 0;
+  if (cand) {
+    meta = S.grp_meta[gid];
+#pragma unroll
+    for (int l = 0; l < L; l++) {
+      const uint32_t ri = (uint32_t)l * G + gid;
+      aux[l] = S.acc_aux[ri];
+      arow[l] = S.acc_row[ri];
+      crw[l] = S.coord_row[ri];
+      if (cf_journaling) dirty[l] = S.acc_dirty[ri];
+#pragma unroll
+      for (int c = 0; c < L; c++) ns_all[c][l] = S.node_slots[((uint32_t)c * S.Rcap + l) * G + gid];
+    }
+    if (plen) {
+      if (pal)
+        pv = ld_stream4(psrc);
+      else
+        pv.x = psrc[0];
+    }
+  }
+  bool sf = cand && ((meta & (GPX_META_LIVE | GPX_META_IDENT)) == (GPX_META_LIVE | GPX_META_IDENT)) &&
+            ((meta >> 16) & 0xffu) == (uint32_t)L;
+  /* PISM.handleProposal :818-888: who coordinates?  (the entry lane's rows) */
+  int4 ae = arow[0], ce = crw[0];
+#pragma unroll
+  for (int c = 1; c < L; c++)
+    if (entry == (uint32_t)c) {
+      ae = arow[c];
+      ce = crw[c];
+    }
+  uint32_t cl = entry;
+  if (!(((unsigned)ce.w & GPX_CF_EXISTS) && bcmp(ce.x, ce.y, ae.y, ae.z) >= 0)) {
+    int fl = -1;
+#pragma unroll
+    for (int l = 0; l < L; l++)
+      if (S.lane_node[l] == ae.z) fl = l;
+    sf = sf && fl >= 0 && fl != (int)entry;
+    cl = fl >= 0 ? (uint32_t)fl : 0u;
+  }
+  int4 crow = crw[0];
+  int af_y = arow[0].y, af_z = arow[0].z;
+  int ns[L];
+#pragma unroll
+  for (int l = 0; l < L; l++) ns[l] = ns_all[0][l];
+#pragma unroll
+  for (int c = 1; c < L; c++)
+    if (cl == (uint32_t)c) {
+      crow = crw[c];
+      af_y = arow[c].y;
+      af_z = arow[c].z;
+#pragma unroll
+      for (int l = 0; l < L; l++) ns[l] = ns_all[c][l];
+    }
+  /* an ACTIVE coordinator whose ballot is not behind its acceptor, no proposal outstanding; every lane the plain
+   * in-order case */
+  const int slot = crow.z;
+  sf = sf && ((unsigned)crow.w == (GPX_CF_EXISTS | GPX_CF_ACTIVE)) && bcmp(crow.x, crow.y, af_y, af_z) >= 0;
+#pragma unroll
+  for (int l = 0; l < L; l++)
+    sf = sf && st_usable(aux[l]) && arow[l].y == crow.x && arow[l].z == crow.y && arow[l].x == slot &&
+         GPX_AUX_PRESENT(aux[l]) == 0u && jsub(slot, arow[l].w) > 0;
+
+  /* ---- level C (depends on the slot): every lane's window entry ---- */
+  uint32_t evalid = 0; /* bit l: lane l's window entry holds a VALID occupant */
+  if (sf) {
+#pragma unroll
+    for (int l = 0; l < L; l++) {
+      int4 e0 = make_int4(0, 0, 0, 0), e1 = e0;
+      if (dirty[l]) ld256(&S.acc_win[2u * (((uint32_t)l * S.W + ((uint32_t)slot & Wm)) * G + gid)], e0, e1);
+      if ((unsigned)e1.w & GPX_ENT_VALID) {
+        evalid |= 1u << l;
+        if (jsub(e0.x, arow[l].w) > 0 && e0.x == slot) sf = false; /* an accept already sits at this slot */
+      }
+    }
+  }
+  const int median = median_regs<L>(ns, (uint32_t)L); /* AcceptPacket.medianCheckpointedSlot (initCommander) */
+  const int cpi = cf_cpi_pg ? (sf ? S.grp_cpi[gid] : 1) : S.cpi_const;
+  int max_cp = (int)((unsigned)slot - 1u); /* every lane's maxCheckpointedSlot :1139-1143 (acc_slot == slot) */
+  if (!cf_gcme) {
+    int lcp = max_cp - max_cp % cpi;
+    if (lcp < 0) {
+      lcp = jsub(lcp, cpi);
+      if (lcp > 0) lcp = 2147483647 - 2147483647 % cpi;
+    }
+    max_cp = lcp;
+  }
+  /* tally: replies in lane order, the decision made by reply L/2 (recordSlotNumber :809-825, plain <) */
+  int nsd[L], mine[L];
+#pragma unroll
+  for (int k = 0; k < L; k++) {
+    nsd[k] = mine[k] = ns[k];
+    if (ns[k] < max_cp) {
+      if (k <= L / 2) nsd[k] = max_cp;
+      mine[k] = max_cp;
+    }
+  }
+  const int dmed = median_regs<L>(nsd, (uint32_t)L); /* makeDecision(getMajorityCommittedSlot()) :630 */
+
+  const bool ckpt = sf && (slot % cpi) == 0;
+  if (sf) {
+    /* ================= in-order fast path ================= */
+    const int4 q0 = make_int4((int)gid, slot, crow.x, crow.y);
+    const bool metaf = cf_logmeta;
+    int4* const img = &s_img[warp][lane_id * 2];
+#pragma unroll
+    for (int l = 0; l < L; l++) {
+      uint8_t* const seg_p = ring_ptr(S, l, seg[l]);
+      const unsigned frame_ref = (unsigned)(((seg[l] + pay_rel + poff) & (S.ring_cap - 1)) >> 4);
+      img[l * 64] = q0; /* ACCEPT image */
+      img[l * 64 + 1] = make_int4(median, (int)(GPX_F_ACCEPT | ((1u << l) << 16)), rq0.z, rq0.w);
+      img[(L + l) * 64] = q0; /* DECISION image */
+      img[(L + l) * 64 + 1] =
+          make_int4(metaf ? -1 : dmed, (int)((GPX_F_DECISION | (metaf ? GPX_F_META : 0u)) | ((1u << l) << 16)),
+                    rq0.z, rq0.w);
+      st_stream4(seg_p + 64 + (size_t)n * 32 + (size_t)i * 16, make_int4((int)poff, (int)plen, 1, crow.y));
+      if (plen) {
+        uint8_t* dst = seg_p + pay_rel + poff;
+        if (pal)
+          st_stream4(dst, pv);
+        else
+          dst[0] = (uint8_t)pv.x;
+      }
+      int4 row = arow[l];
+      gc_step(row, median);
+      gc_step(row, dmed);
+      row.x = (int)((unsigned)row.x + 1u); /* executed(): _slot++ */
+      gc_step(row, dmed);                  /* second EEC iteration; nothing is queued (checked above) */
+      S.acc_row[(uint32_t)l * G + gid] = row;
+      const uint32_t wi = 2u * (((uint32_t)l * S.W + ((uint32_t)slot & Wm)) * G + gid);
+      if (cf_journaling) {
+        if ((evalid >> l) & 1u)
+          st256(&S.acc_win[wi], make_int4(slot, crow.x, crow.y, (int)frame_ref),
+                make_int4(rq0.z, rq0.w, (int)plen, (int)(1u << 16)));
+      } else
+        st256(&S.acc_win[wi], make_int4(slot, crow.x, crow.y, (int)frame_ref),
+              make_int4(rq0.z, rq0.w, (int)plen, (int)(GPX_ENT_VALID | (1u << 16))));
+      if (mine[l] != ns[l]) S.node_slots[(cl * S.Rcap + l) * G + gid] = mine[l]; /* nodeSlotNumbers[cl][l] */
+    }
+    if (plen > 1 && !pal) { /* unaligned body: byte by byte, every lane */
+#pragma unroll 1
+      for (uint32_t b = 1; b < plen; b++) {
+        const uint8_t v = psrc[b];
+#pragma unroll
+        for (int l = 0; l < L; l++) ring_ptr(S, l, seg[l])[pay_rel + poff + b] = v;
+      }
+    }
+    if (RA.sum)
+      store_sum(&RA.sum[i], slot, (1u << L) - 1u, ckpt ? GPX_F_CKPT : 0u, 1u);
+    else
+      RA.P.status[i] = slot;
+    crow.z = (int)((unsigned)crow.z + 1u); /* PCS.propose: nextProposalSlotNumber++ */
+    S.coord_row[cl * G + gid] = crow;
+  } else if (head) {
+    const uint32_t k = atomicAdd(RA.n_todo, 1u);
+    RA.todo[k] = i; /* the run goes to k_round_slow */
+    if (k == 0 && RA.tail_launch)
+      k_round_slow<L, L><<<RA.slow_grid, GPX_BLOCK, 0, cudaStreamTailLaunch>>>(S, RA);
+  }
+  const uint32_t sfm = __ballot_sync(FULL, sf); /* bit g: group g of the warp took the fast path */
+  const uint32_t i0 = r0 + warp * 32u;         /* request of the warp's group 0 */
+  __syncwarp();
+  { /* the staged log images as contiguous 16 B pieces: piece k is half k & 1 of the image of group (k >> 1) & 31,
+     * kind x lane k >> 6 -- constant over one iteration */
+#pragma unroll
+    for (uint32_t k0 = 0; k0 < 4u * L * 32u; k0 += 32u) {
+      const uint32_t kl = k0 >> 6, l = kl % L, k = k0 + lane_id, g = (k >> 1) & 31u;
+      if ((sfm >> g) & 1u)
+        st_stream4(ring_ptr(S, l, seg[l] + (kl >= (uint32_t)L ? res_a : 0ull) + 64ull +
+                                     (unsigned long long)(i0 + g) * 32ull + (k & 1u) * 16u),
+                   s_img[warp][k]);
+    }
+  }
+  if (!RA.sum) { /* EXEC records (PISM.execute hands the request to the app); shouldCheckpoint :2037-2041 */
+    gpx_exec_rec er[L];
+#pragma unroll
+    for (int l = 0; l < L; l++) {
+      er[l].gid = gid;
+      er[l].slot = slot;
+      er[l].req_id = ((long long)rq0.w << 32) | (unsigned)rq0.z;
+      er[l].payload_off = (unsigned)(((seg[l] + pay_rel + poff) & (S.ring_cap - 1)) >> 4);
+      er[l].flags = (ckpt ? GPX_F_CKPT : 0u) | ((uint32_t)l << 12) | (1u << 16);
+    }
+    if (sfm == FULL && (((uint32_t)(uintptr_t)A.exec & 15u) == 0)) {
+      /* the warp's 32 x L rows are one contiguous, 16-byte aligned run: staged, then stored as whole pieces */
+      __syncwarp(); /* the images above have been read */
+      long long* const sx = reinterpret_cast<long long*>(s_img[warp]);
+#pragma unroll
+      for (int l = 0; l < L; l++) {
+        const long long* s = reinterpret_cast<const long long*>(&er[l]);
+        long long* d = sx + (lane_id * L + l) * 3u;
+        d[0] = s[0];
+        d[1] = s[1];
+        d[2] = s[2];
+      }
+      __syncwarp();
+      uint8_t* const dst = reinterpret_cast<uint8_t*>(A.exec + (size_t)i0 * L);
+      constexpr uint32_t NP = 32u * L * (uint32_t)sizeof(gpx_exec_rec) / 16u;
+#pragma unroll
+      for (uint32_t k0 = 0; k0 < NP; k0 += 32u)
+        if (k0 + lane_id < NP) st_stream4(dst + (size_t)(k0 + lane_id) * 16, s_img[warp][k0 + lane_id]);
+    } else if (sf) {
+#pragma unroll
+      for (int l = 0; l < L; l++) store_exec(&A.exec[(size_t)i * L + l], er[l]);
+    }
+  }
+  if (valid) RA.mark[i] = sf ? 0 : 1;
+  if (sf && pal && plen > 16u) { /* bodies longer than one chunk: four independent 128-bit loads in flight */
+    uint32_t b = 16;
+#pragma unroll 1
+    for (; b + 64 <= plen; b += 64) {
+      const int4 a0 = ld_stream4(psrc + b), a1 = ld_stream4(psrc + b + 16), a2 = ld_stream4(psrc + b + 32),
+                 a3 = ld_stream4(psrc + b + 48);
+#pragma unroll
+      for (int l = 0; l < L; l++) {
+        uint8_t* const dst = ring_ptr(S, l, seg[l]) + pay_rel + poff;
+        st_stream4(dst + b, a0);
+        st_stream4(dst + b + 16, a1);
+        st_stream4(dst + b + 32, a2);
+        st_stream4(dst + b + 48, a3);
+      }
+    }
+#pragma unroll 1
+    for (; b < plen; b += 16) {
+      const int4 a = ld_stream4(psrc + b);
+#pragma unroll
+      for (int l = 0; l < L; l++) st_stream4(ring_ptr(S, l, seg[l]) + pay_rel + poff + b, a);
+    }
+  }
+  { /* fast-path events, counted per lane as k_round does: one shared-memory update per warp */
+    const uint32_t nt = __popc(sfm), nc = __reduce_add_sync(FULL, ckpt ? (uint32_t)L : 0u);
+    if (lane_id == 0 && nt) {
+      atomicAdd(&s_ctr[C_FAST_LANES], nt * (uint32_t)L);
       atomicAdd(&s_ctr[C_FAST_TEAMS], nt);
       if (nc) atomicAdd(&s_ctr[C_FAST_CKPT], nc);
     }

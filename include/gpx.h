@@ -691,7 +691,10 @@ typedef struct gpx_dev_round_bufs {
 int gpx_round_device(gpx_engine* e, const gpx_dev_round_bufs* b, void* stream);        /* fused */
 /* Form of the fused round.  0 / 1 (default): k_round_slow -- the general code for runs that are not the plain in-order
  * case -- is launched from the device, as a tail launch, by the first team that leaves a run over: a round without
- * such runs is ONE kernel on the stream.  2: the host launches k_round_slow behind every k_round (tuning / fallback). */
+ * such runs is ONE kernel on the stream.  2: the host launches k_round_slow behind every k_round (tuning / fallback).
+ * The in-order kernel is k_round_g (one thread per group) for n_lanes <= 3 and k_round (a team of n_lanes threads per
+ * group) above that; 3 and 4 are 0 and 2 with k_round at every n_lanes, to time the two against each other and to test
+ * that they compute the same round. */
 int gpx_set_round_mode(gpx_engine* e, int mode);
 int gpx_round_device_phases(gpx_engine* e, const gpx_dev_round_bufs* b, void* stream); /* phase by phase */
 /* gpx_propose + gpx_handle_accepts_fused on device buffers: ACCEPTs compacted at the front (exec[k * n_lanes + lane]
