@@ -51,6 +51,7 @@ wire_ref_dtype = np.dtype([("off", "<u4"), ("len", "<u4"), ("gid", "<u4"), ("nod
 WS_OK, WS_UNKNOWN_NAME, WS_VERSION, WS_MALFORMED, WS_UNHANDLED, WS_NOT_LOCAL = 0, 1, 2, 3, 4, 5
 WE_SENT, WE_VOID, WE_LOCAL, WE_NACK, WE_NO_NAME = 0, 1, 2, 3, 4
 WE_BAD_HEAD = 5  # gpx_wire_encode_accepts_device: the ACCEPT's head request is out of range or of another group
+WE_ELECT = 6  # gpx_wire_encode_forwards_device: the host runs for coordinator instead of forwarding
 # gpx_wire_req_meta: the RequestPacket wire fields a gpx_request_rec does not keep (gpx_wire_decode_requests_device)
 RM_RETURN_VALUE, RM_BROADCASTED = 1, 2
 req_meta_dtype = np.dtype([("client_ip", "u1", (4,)), ("client_port", "<u2"), ("listen_port", "<u2"),

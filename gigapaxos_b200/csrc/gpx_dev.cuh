@@ -162,6 +162,58 @@ __device__ __forceinline__ GroupCtx group_ctx(const DevState& S, uint32_t gid) {
   return g;
 }
 
+/* RequestBatcher.dequeueImpl's cut (RequestBatcher.java:198-219): the end of the batch that starts at request k of a
+ * run of gid's requests (BATCHING_ENABLED, MAX_BATCH_SIZE, the byte bound with the size estimate) */
+__device__ __forceinline__ uint32_t batch_end(const DevState& S, const gpx_request_rec* reqs, uint32_t n, uint32_t k,
+                                              uint32_t gid) {
+  long long bytes = (long long)reqs[k].payload_len + S.size_est;
+  int cnt = 1;
+  uint32_t b = k + 1;
+  if (S.batching)
+    while (b < n && reqs[b].gid == gid) {
+      bytes += (long long)reqs[b].payload_len + S.size_est;
+      if (bytes > S.max_batch_bytes) break;
+      cnt += 1;
+      if (cnt > S.max_batch_size) break;
+      b++;
+    }
+  return b;
+}
+
+/* PISM.handleProposal's routing (:854-885) of a request of gid entering at lane `entry`, on the current rows: 0 with
+ * *clane = the lane whose coordinator proposes; GPX_RS_DROPPED (no such group or lane, or an acceptor that is not
+ * ACTIVE); GPX_RS_FORWARD (the entry lane has no usable coordinator and no local lane serves the ballot's coordinator
+ * *bcoord, which is then remote); GPX_RS_NOCOORD.  *meta = the group's grp_meta once it is known to be live.  Proposing
+ * changes neither the acceptor rows nor whether a coordinator exists, so after k_propose, and before any call that
+ * changes state, this gives the answer k_propose gave: propose_run and the forward encoder (k_wire_fwd) both call it. */
+__device__ __forceinline__ int propose_route(const DevState& S, uint32_t gid, uint32_t entry, uint32_t* meta, int* clane,
+                                             int32_t* bcoord) {
+  if (gid >= S.G || entry >= S.L) return GPX_RS_DROPPED;
+  const uint32_t m = S.grp_meta[gid];
+  if (!(m & GPX_META_LIVE) || !st_usable(S.acc_aux[row_idx(S, entry, gid)])) return GPX_RS_DROPPED;
+  *meta = m;
+  const int4 Ae = S.acc_row[row_idx(S, entry, gid)];
+  const int4 Ce = S.coord_row[row_idx(S, entry, gid)];
+  *bcoord = Ae.z;
+  if (((unsigned)Ce.w & GPX_CF_EXISTS) && bcmp(Ce.x, Ce.y, Ae.y, Ae.z) >= 0) { /* PaxosCoordinator.exists(c, ballot) */
+    *clane = (int)entry;
+    return 0;
+  }
+  int fl = -1;
+  for (uint32_t l = 0; l < S.L; l++)
+    if (S.lane_node[l] == Ae.z) fl = (int)l;
+  if (fl < 0) return GPX_RS_FORWARD;
+  if (fl == (int)entry) return GPX_RS_NOCOORD;
+  if (!st_usable(S.acc_aux[row_idx(S, (uint32_t)fl, gid)])) return GPX_RS_DROPPED;
+  const int4 Af = S.acc_row[row_idx(S, fl, gid)];
+  const int4 Cf = S.coord_row[row_idx(S, fl, gid)];
+  if (((unsigned)Cf.w & GPX_CF_EXISTS) && bcmp(Cf.x, Cf.y, Af.y, Af.z) >= 0) {
+    *clane = fl;
+    return 0;
+  }
+  return GPX_RS_NOCOORD;
+}
+
 /* ---- per-group helpers shared by the management kernels (gpx_kernels.cuh) and k_pause_groups (gpx_pause.cuh) ---- */
 /* the HotRestoreInfo field set of (gid, lane) (paxosutil/HotRestoreInfo.java:40-58, PISM.tryPause :2004-2025) */
 __device__ __forceinline__ void dump_row(const DevState& S, uint32_t lane, uint32_t gid, gpx_row& r) {

@@ -28,6 +28,7 @@
 #include "gpx_logfind.cuh"
 #include "gpx_wire_dev.cuh"
 #include "gpx_wire_json.cuh"
+#include "gpx_wire_fwd.cuh"
 
 #include <cub/cub.cuh>
 

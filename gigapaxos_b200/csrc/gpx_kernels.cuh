@@ -116,22 +116,6 @@ __device__ __forceinline__ bool mk_batched(const uint8_t* mark, uint32_t n, uint
   return (mk & GPX_MK_BATCHED) || ((mk & GPX_MK_HEAD) && q + 1 < n && (mark[q + 1] & GPX_MK_BATCHED));
 }
 
-__device__ __forceinline__ uint32_t batch_end(const DevState& S, const gpx_request_rec* reqs, uint32_t n, uint32_t k,
-                                              uint32_t gid) {
-  long long bytes = (long long)reqs[k].payload_len + S.size_est;
-  int cnt = 1;
-  uint32_t b = k + 1;
-  if (S.batching)
-    while (b < n && reqs[b].gid == gid) {
-      bytes += (long long)reqs[b].payload_len + S.size_est;
-      if (bytes > S.max_batch_bytes) break;
-      cnt += 1;
-      if (cnt > S.max_batch_size) break;
-      b++;
-    }
-  return b;
-}
-
 /* `indexed`: the ACCEPT of the batch that starts at request k is written to A.accepts[k] (k_round) instead of
  * the compacted position base+emitted (k_propose).  Every request of the run gets its GPX_MK_* mark (GPX_MK_SLOW
  * kept when indexed).  head (k_propose, may be null): head[base + e] = the request that starts compacted ACCEPT e,
@@ -149,50 +133,13 @@ __device__ __noinline__ void propose_run(const DevState& S, const ProposeArgs& A
   int clane = -1;
   const MsetInfo* ms = nullptr;
   uint32_t R = 0;
-  do {
-    uint32_t entry = (reqs[i].flags >> 8) & 0xfu;
-    if (gid >= S.G || entry >= S.L) {
-      code = GPX_RS_DROPPED;
-      break;
-    }
-    uint32_t meta = S.grp_meta[gid];
-    uint32_t aux;
-    if (!(meta & GPX_META_LIVE) || !usable(S, gid, entry, &aux)) {
-      code = GPX_RS_DROPPED;
-      break;
-    }
+  {
+    uint32_t meta = 0;
+    int32_t bcoord;
+    code = propose_route(S, gid, (reqs[i].flags >> 8) & 0xfu, &meta, &clane, &bcoord);
     ms = &S.msets[meta & 0xffffu];
     R = (meta >> 16) & 0xffu;
-    int4 Ae = S.acc_row[row_idx(S, entry, gid)];
-    int4 Ce = S.coord_row[row_idx(S, entry, gid)];
-    if (((unsigned)Ce.w & GPX_CF_EXISTS) && bcmp(Ce.x, Ce.y, Ae.y, Ae.z) >= 0) { /* PaxosCoordinator.exists(c, ballot) */
-      clane = (int)entry;
-    } else {
-      int fl = -1;
-      for (uint32_t l = 0; l < S.L; l++)
-        if (S.lane_node[l] == Ae.z) fl = (int)l;
-      if (fl < 0) {
-        code = GPX_RS_FORWARD;
-        break;
-      }
-      if (fl == (int)entry) {
-        code = GPX_RS_NOCOORD;
-        break;
-      }
-      if (!usable(S, gid, (uint32_t)fl, &aux)) {
-        code = GPX_RS_DROPPED;
-        break;
-      }
-      int4 Af = S.acc_row[row_idx(S, fl, gid)];
-      int4 Cf = S.coord_row[row_idx(S, fl, gid)];
-      if (((unsigned)Cf.w & GPX_CF_EXISTS) && bcmp(Cf.x, Cf.y, Af.y, Af.z) >= 0)
-        clane = fl;
-      else {
-        code = GPX_RS_NOCOORD;
-        break;
-      }
-    }
-  } while (false);
+  }
 
   if (code == 0) {
     int4 crow = S.coord_row[row_idx(S, clane, gid)];

@@ -1,0 +1,445 @@
+/*
+ * gpx_wire_fwd.cuh -- client requests forwarded between nodes, on the device.  With the coordinators spread over the
+ * members (PISM.roundRobinCoordinator :2251-2256), most requests enter at a node that does not coordinate their group,
+ * and that node forwards them to the coordinator (PISM.handleProposal :854-885):
+ *   k_wire_fwd    the sending side (gpx_wire_encode_forwards_device): the requests gpx_propose_device gave
+ *                 GPX_RS_FORWARD become REQUEST packets addressed to the ballot's coordinator, cut as the RequestBatcher
+ *                 cuts them.  One thread per run of a gid's requests, as in k_propose.
+ *   k_json_req    the receiving side for a Java peer (gpx_wire_decode_json_requests_device): under load a Java node
+ *                 sends its forwards as JSON members of BATCHED_PAXOS_PACKETs (PaxosPacketBatcher.process :270-277),
+ *                 which gpx_wire_decode_json_device lists as GPX_WS_UNHANDLED; the REQUEST members among them become
+ *                 proposals, as k_wire_req_decode makes them of the byte form.  One thread per member.
+ * Both are scalar, like the kernels they sit beside, so tests/emu compiles this file for the host.
+ */
+#pragma once
+#include "gpx_wire_json.cuh"
+
+/* ---- forwarded REQUEST packets (gpx_wire_encode_forwards_device) -------------------------------------------------- */
+struct WireFwdArgs {
+  const gpx_request_rec* reqs;   /* [n] grouped by gid, as gpx_propose_device took them */
+  const gpx_wire_req_meta* meta; /* [n] */
+  const int32_t* status;         /* [n] gpx_propose_device's */
+  const uint8_t* payload;        /* the request arena: bodies at reqs[q].payload_off */
+  const int32_t* down;           /* [n_down] the nodes the host takes for down (PaxosManager.isNodeUp) */
+  uint32_t n, n_down;
+  uint8_t* rstatus;              /* [n] GPX_WE_* */
+  uint32_t* cnt;                 /* [2][n] pass 0, per request that starts a packet: packet bytes, 1 */
+  const uint32_t* off;           /* [2][n] their exclusive prefix sums */
+  uint8_t* out;
+  gpx_wire_ref* refs;
+  int emit;
+};
+
+/* request q is forwarded: propose_run gave it GPX_RS_FORWARD (a wrapped slot may equal that code: the caller's route
+ * says which), and it is not broadcasted (a broadcasted request reached every replica already, :854) */
+__device__ __forceinline__ bool fwd_request(const WireFwdArgs& A, uint32_t q) {
+  return A.status[q] == GPX_RS_FORWARD && !(A.meta[q].flags & GPX_RM_BROADCASTED);
+}
+
+/* one thread per request; the first request of a gid's run handles the run.  The run is routed as propose_run routes
+ * it, from its first request's entry lane; its forwarded requests are cut with batch_end, each cut one REQUEST packet:
+ * the outer request is the cut's first with forwardCount + 1 (setForwarderID :437-441), the others its `batched`.
+ * Pass 0 writes rstatus and the packet sizes, pass 1 the packets and their refs at the scanned offsets. */
+__global__ void k_wire_fwd(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                           const __grid_constant__ WireFwdArgs A) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= A.n) return;
+  const uint32_t gid = A.reqs[i].gid;
+  if (i > 0 && A.reqs[i - 1].gid == gid) return;
+  uint32_t run_end = i + 1;
+  while (run_end < A.n && A.reqs[run_end].gid == gid) run_end++;
+  uint32_t meta = 0;
+  int clane = -1;
+  int32_t bcoord = 0;
+  const bool routed = propose_route(S, gid, (A.reqs[i].flags >> 8) & 0xfu, &meta, &clane, &bcoord) == GPX_RS_FORWARD;
+  /* the destination: the ballot's coordinator, or the member after it when the host takes it for down
+   * (getNextCoordinator :2232-2241); the host runs for coordinator instead when that is a local node (:869) or the
+   * coordinator is not a member */
+  uint8_t run_st = GPX_WE_SENT;
+  int32_t dst = bcoord;
+  if (routed) {
+    const MsetInfo* ms = &S.msets[meta & 0xffffu];
+    const uint32_t R = (meta >> 16) & 0xffu;
+    uint32_t di = wire_member_idx(ms, R, bcoord);
+    if (di == 0xffu) {
+      run_st = GPX_WE_ELECT;
+    } else {
+      for (uint32_t d = 0; d < A.n_down; d++)
+        if (A.down[d] == bcoord) {
+          di = (di + 1u) % R;
+          break;
+        }
+      dst = ms->nodes[di];
+      if (ms->lane_of_idx[di] != 0xffu) run_st = GPX_WE_ELECT;
+    }
+  }
+  const bool named = routed && W.slot != nullptr && W.slot[gid] != GPX_NAME_NONE;
+  WireAccArgs X;
+  X.head = nullptr;
+  X.reqs = A.reqs;
+  X.meta = A.meta;
+  X.n_reqs = A.n;
+  X.payload = A.payload;
+  uint32_t k = i;
+  while (k < run_end) {
+    if (!routed || !fwd_request(A, k)) {
+      if (!A.emit) {
+        A.rstatus[k] = GPX_WE_VOID;
+        A.cnt[k] = A.cnt[A.n + k] = 0;
+      }
+      k++;
+      continue;
+    }
+    uint32_t b = batch_end(S, A.reqs, A.n, k, gid), e = k + 1; /* the cut of the consecutive forwarded requests */
+    while (e < b && fwd_request(A, e)) e++;
+    b = e;
+    uint8_t st = run_st;
+    const int32_t fc = (int32_t)((uint32_t)A.meta[k].forward_count + 1u); /* forwardCount++ (Java int) */
+    if (st == GPX_WE_SENT && fc > 3) st = GPX_WE_ELECT; /* isPingPonging :508 */
+    if (st == GPX_WE_SENT && !named) st = GPX_WE_NO_NAME;
+    if (!A.emit) {
+      uint32_t bytes = 0;
+      for (uint32_t q = k; q < b; q++) {
+        A.rstatus[q] = st;
+        A.cnt[q] = A.cnt[A.n + q] = 0;
+        bytes += wire_request_bytes(W, gid, A.reqs[q].payload_len) + (q > k ? 4u : 0u);
+      }
+      if (st == GPX_WE_SENT) {
+        A.cnt[k] = bytes;
+        A.cnt[A.n + k] = 1;
+      }
+    } else if (st == GPX_WE_SENT) {
+      uint8_t* o = A.out + A.off[k];
+      uint32_t len = ww_request(o, GPX_PT_REQUEST, W, gid, X, k, b - k - 1u);
+      ww_i32(o + 13u + W.name[(size_t)gid * GPX_NAME_BYTES] + 34u, fc); /* the outer request's forwardCount */
+      for (uint32_t q = k + 1; q < b; q++) { /* {int length}{REQUEST packet} :929-936 */
+        const uint32_t l = ww_request(o + len + 4, GPX_PT_REQUEST, W, gid, X, q, 0u);
+        ww_i32(o + len, (int32_t)l);
+        len += 4u + l;
+      }
+      gpx_wire_ref r;
+      r.off = A.off[k];
+      r.len = len;
+      r.gid = gid;
+      r.node = dst;
+      A.refs[A.off[A.n + k]] = r;
+    }
+    k = b;
+  }
+}
+
+/* ---- REQUEST members of a Java peer's BATCHED_PAXOS_PACKETs (gpx_wire_decode_json_requests_device) ---------------- */
+/* the keys of RequestPacket(net.minidev.json.JSONObject) :584-649 / toJSONSmartImpl :697-742 and PaxosPacket's */
+enum { JQ_TYPE, JQ_PT, JQ_ID, JQ_V, JQ_QID, JQ_QV, JQ_ET, JQ_E, JQ_NFWDS, JQ_STOP, JQ_QF, JQ_BC, JQ_CA, JQ_LA, JQ_BATCH,
+       JQ_RV, JQ_DIG, JQ_N };
+__device__ __forceinline__ int json_req_key(const JStr& s) {
+  if (s.wide) return -1;
+  switch (s.len) {
+    case 1:
+      if (s.head == 'V') return JQ_V;
+      if (s.head == 'E') return JQ_E;
+      return -1;
+    case 2:
+      if (s.head == JK('P', 'T', 0, 0, 0)) return JQ_PT;
+      if (s.head == JK('I', 'D', 0, 0, 0)) return JQ_ID;
+      if (s.head == JK('Q', 'V', 0, 0, 0)) return JQ_QV;
+      if (s.head == JK('E', 'T', 0, 0, 0)) return JQ_ET;
+      if (s.head == JK('Q', 'F', 0, 0, 0)) return JQ_QF;
+      if (s.head == JK('B', 'C', 0, 0, 0)) return JQ_BC;
+      if (s.head == JK('C', 'A', 0, 0, 0)) return JQ_CA;
+      if (s.head == JK('L', 'A', 0, 0, 0)) return JQ_LA;
+      if (s.head == JK('R', 'V', 0, 0, 0)) return JQ_RV;
+      return -1;
+    case 3:
+      if (s.head == JK('Q', 'I', 'D', 0, 0)) return JQ_QID;
+      if (s.head == JK('D', 'I', 'G', 0, 0)) return JQ_DIG;
+      return -1;
+    case 4:
+      if (s.head == JK('t', 'y', 'p', 'e', 0)) return JQ_TYPE;
+      if (s.head == JK('S', 'T', 'O', 'P', 0)) return JQ_STOP;
+      return -1;
+    case 5:
+      if (s.head == JK('N', 'F', 'W', 'D', 'S')) return JQ_NFWDS;
+      if (s.head == JK('B', 'A', 'T', 'C', 'H')) return JQ_BATCH;
+      return -1;
+    default: return -1;
+  }
+}
+struct JsonReqKeys {
+  enum { N = JQ_N, PP = -2 };
+  __device__ __forceinline__ static int id(const JStr& s) { return json_req_key(s); }
+};
+
+/* the fields of one request object */
+struct JsonReq {
+  int64_t qid, et;
+  int32_t e, nfwds;
+  uint32_t qv_at, qv_len; /* QV's opening quote, its characters */
+  bool stop, qf, bc;
+  uint8_t ca_ip[4], la_ip[4];
+  uint16_t ca_port, la_port;
+};
+
+/* an optional bool at `at`: false when present and not true / false */
+__device__ __forceinline__ bool json_get_bool(const JRd& J0, uint32_t at, bool* v) {
+  JRd J = J0;
+  *v = false;
+  if (!json_at(J, at)) return true;
+  if (jr_peek(J) == 't') return *v = jr_word(J, "true", 4);
+  return jr_word(J, "false", 5);
+}
+/* an optional address string at `at` (false: not a string).  *lit: it is [anything/]a.b.c.d:port with a port of
+ * 1-65535 -- Util.getInetSocketAddressFromString :278-287 (everything up to the last '/' dropped) for a literal IPv4
+ * address.  Anything else (a hostname wants a lookup; leading zeros, a line terminator, which the reference's ".*"
+ * does not cross, or extra ':' parts) is left to the host. */
+__device__ __forceinline__ bool json_get_addr(const JRd& J0, uint32_t at, bool* lit, uint8_t* ip, uint16_t* port) {
+  JRd J = J0;
+  *lit = true;
+  if (!json_at(J, at)) return true;
+  if (!jr_eat(J, '"')) return false;
+  uint32_t part = 0, val = 0, nd = 0;
+  bool bad = false, host = false;
+  for (;;) {
+    uint32_t u = 0;
+    const int r = jr_unit(J, &u);
+    if (r < 0) return false;
+    if (r == 1) break;
+    if (u == '\n' || u == '\r' || u == 0x85u || u > 0xffu) host = true;
+    if (u == '/') {
+      part = val = nd = 0;
+      bad = false;
+    } else if (bad) {
+    } else if (u >= '0' && u <= '9') {
+      if (part < 4 && nd == 1 && val == 0) bad = true; /* a leading zero in an octet */
+      val = val * 10u + (u - '0');
+      if (++nd > 5 || (part < 4 && val > 255u)) bad = true;
+    } else if (u == '.' && part < 3 && nd > 0) {
+      ip[part++] = (uint8_t)val;
+      val = nd = 0;
+    } else if (u == ':' && part == 3 && nd > 0) {
+      ip[3] = (uint8_t)val;
+      part = 4;
+      val = nd = 0;
+    } else {
+      bad = true;
+    }
+  }
+  *lit = !host && !bad && part == 4 && nd > 0 && val >= 1u && val <= 65535u;
+  *port = *lit ? (uint16_t)val : (uint16_t)0;
+  if (!*lit) ip[0] = ip[1] = ip[2] = ip[3] = 0;
+  return true;
+}
+/* the request fields of an object whose keys are at pos: GPX_WS_OK, GPX_WS_MALFORMED (a schema failure) or
+ * GPX_WS_UNHANDLED (RV or DIG present, a QV character above U+00FF, an address the host decides) */
+__device__ __forceinline__ int32_t json_req_fields(const JRd& J0, const uint32_t* pos, JsonReq& f) {
+  memset(&f, 0, sizeof f);
+  JRd J = J0;
+  bool ok = json_at(J, pos[JQ_QID]);
+  if (ok) {
+    f.qid = jr_i64(J);
+    ok = J.ok;
+  }
+  J = J0;
+  if (ok && (ok = json_at(J, pos[JQ_ET]))) {
+    f.et = jr_i64(J);
+    ok = J.ok;
+  }
+  ok = ok && json_get_i32(J0, pos[JQ_E], &f.e);
+  ok = ok && (!pos[JQ_NFWDS] || json_get_i32(J0, pos[JQ_NFWDS], &f.nfwds));
+  ok = ok && json_get_bool(J0, pos[JQ_STOP], &f.stop) && json_get_bool(J0, pos[JQ_QF], &f.qf) &&
+       json_get_bool(J0, pos[JQ_BC], &f.bc);
+  bool wide = false, ca = true, la = true;
+  J = J0;
+  if (ok && (ok = json_at(J, pos[JQ_QV]) && jr_peek(J) == '"')) {
+    f.qv_at = J.n;
+    const JStr s = jr_string(J);
+    ok = J.ok;
+    f.qv_len = s.len;
+    wide = s.wide;
+  }
+  ok = ok && json_get_addr(J0, pos[JQ_CA], &ca, f.ca_ip, &f.ca_port) &&
+       json_get_addr(J0, pos[JQ_LA], &la, f.la_ip, &f.la_port);
+  if (!ok) return GPX_WS_MALFORMED;
+  if (pos[JQ_RV] || pos[JQ_DIG] || wide || !ca || !la) return GPX_WS_UNHANDLED;
+  return GPX_WS_OK;
+}
+
+struct WireJsonReqArgs {
+  const uint8_t* bytes;
+  const gpx_wire_ref* pkts;
+  const gpx_wire_member* mem;
+  uint64_t n_bytes;
+  uint32_t n_pkts;
+  uint32_t n;          /* members */
+  long long now_ms;
+  int32_t* status;     /* [n] */
+  uint32_t* cnt;       /* [WQ_NCNT][n]: pass 0 writes the member's requests and payload bytes (each value padded to 16) */
+  const uint32_t* off; /* [WQ_NCNT][n]: pass 1 reads their exclusive prefix sums */
+  /* pass 1: requests and meta staged in member order, the sort keys (gids) beside them; the payload is the output */
+  gpx_request_rec* req;
+  gpx_wire_req_meta* meta;
+  uint32_t* key;
+  uint8_t* payload;
+  int emit;
+};
+
+/* one request at staged position o, its value unescaped at payload offset *po (advanced): k_wire_req_decode's record
+ * (wire_put_request) for the same RequestPacket */
+__device__ __forceinline__ void json_put_request(const WireJsonReqArgs& A, uint32_t o, uint32_t* po, uint32_t gid,
+                                                 uint32_t i, int32_t node, uint32_t lane, const JRd& J0,
+                                                 const JsonReq& f) {
+  gpx_request_rec rq;
+  rq.gid = gid;
+  rq.flags = (f.stop ? GPX_F_STOP : 0u) | (lane << 8);
+  rq.req_id = f.qid;
+  rq.payload_off = *po;
+  rq.payload_len = f.qv_len;
+  gpx_wire_req_meta m;
+  memset(&m, 0, sizeof m);
+  for (int b = 0; b < 4; b++) {
+    m.client_ip[b] = f.ca_ip[b];
+    m.listen_ip[b] = f.la_ip[b];
+  }
+  m.client_port = f.ca_port;
+  m.listen_port = f.la_port;
+  m.forward_count = f.nfwds;
+  m.entry_time = f.et;
+  m.flags = (f.qf ? GPX_RM_RETURN_VALUE : 0u) | (f.bc ? GPX_RM_BROADCASTED : 0u);
+  if (f.e == -1) { /* IntegerMap.NULL_INT_NODE: setEntryReplica :393-403 with the call's clock */
+    rq.entry_node = node;
+    m.entry_time = A.now_ms;
+  } else {
+    rq.entry_node = f.e;
+  }
+  rq.client = i;
+  A.req[o] = rq;
+  A.meta[o] = m;
+  A.key[o] = gid;
+  uint8_t* d = A.payload + *po;
+  JRd Q = J0;
+  Q.n = f.qv_at + 1u;
+  for (uint32_t b = 0; b < f.qv_len; b++) { /* one thread copies the whole value, however long */
+    uint32_t u = 0;
+    jr_unit(Q, &u);
+    d[b] = (uint8_t)u;
+  }
+  const uint32_t padded = (f.qv_len + 15u) & ~15u;
+  for (uint32_t b = f.qv_len; b < padded; b++) d[b] = 0;
+  *po += padded;
+}
+
+/* one thread per member.  Pass 0 (emit == 0): a member listed GPX_WS_UNHANDLED that is a REQUEST object (PT 1) is
+ * parsed and validated with its BATCH, its name, version and receiving node looked up: its status and output sizes;
+ * every other member's status is copied.  Pass 1 parses the OK members again and writes their requests, meta and
+ * values at the scanned offsets. */
+__global__ void k_json_req(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                           const __grid_constant__ WireJsonReqArgs A) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= A.n) return;
+  const gpx_wire_member mb = A.mem[i];
+  if (A.emit && (A.status[i] != GPX_WS_OK || mb.status != GPX_WS_UNHANDLED)) return; /* a copied OK has no request */
+  int32_t st = mb.status;
+  uint32_t nreq = 0, pay = 0, gid = GPX_NAME_NONE, lane = 0;
+  int32_t node = 0;
+  JRd J;
+  J.b = A.bytes;
+  J.n = mb.off;
+  J.end = mb.off + mb.len;
+  J.ok = true;
+  uint32_t pos[JQ_N], ppc = GPX_JSON_NONE;
+  JsonReq f;
+  if (st == GPX_WS_UNHANDLED) {
+    int32_t type = 0, pt = 0, ver = 0;
+    if ((uint64_t)mb.off + mb.len > A.n_bytes || mb.pkt >= A.n_pkts) {
+      st = GPX_WS_MALFORMED;
+    } else {
+      json_keys_t<JsonReqKeys>(J, pos, nullptr, &ppc);
+      jr_ws(J);
+      if (!J.ok || J.n != J.end || !json_get_i32(J, pos[JQ_TYPE], &type) || type != GPX_PT_PAXOS_PACKET ||
+          !json_get_i32(J, pos[JQ_PT], &pt))
+        st = GPX_WS_MALFORMED;
+      else if (pt != GPX_PT_REQUEST)
+        st = GPX_WS_UNHANDLED;
+      else
+        st = pos[JQ_ID] && J.b[pos[JQ_ID]] == '"' && json_get_i32(J, pos[JQ_V], &ver) ? GPX_WS_OK : GPX_WS_MALFORMED;
+    }
+    if (st == GPX_WS_OK) {
+      st = json_req_fields(J, pos, f);
+      nreq = 1;
+      pay = (f.qv_len + 15u) & ~15u;
+      if (st != GPX_WS_MALFORMED && pos[JQ_BATCH]) { /* one level of latched requests (RequestBatcher) */
+        JRd B = J;
+        B.n = pos[JQ_BATCH];
+        bool ok = jr_eat(B, '[');
+        jr_ws(B);
+        if (ok && jr_peek(B) == ']') {
+        } else {
+          while (ok) {
+            uint32_t sp[JQ_N];
+            json_keys_t<JsonReqKeys>(B, sp, nullptr, &ppc);
+            ok = B.ok && !sp[JQ_BATCH];
+            if (!ok) break;
+            JsonReq g;
+            const int32_t s = json_req_fields(B, sp, g);
+            if (s == GPX_WS_MALFORMED) {
+              ok = false;
+              break;
+            }
+            if (s == GPX_WS_UNHANDLED) st = GPX_WS_UNHANDLED; /* the request goes to the host whole */
+            nreq++;
+            pay += (g.qv_len + 15u) & ~15u;
+            jr_ws(B);
+            if (jr_peek(B) == ',') {
+              B.n++;
+              continue;
+            }
+            ok = jr_eat(B, ']');
+            break;
+          }
+        }
+        if (!ok) st = GPX_WS_MALFORMED;
+      }
+    }
+    if (st == GPX_WS_OK) {
+      JRd I = J;
+      I.n = pos[JQ_ID];
+      const JStr id = jr_string(I);
+      gid = json_id_gid(W, J, pos[JQ_ID], id);
+      const GroupCtx g = group_ctx(S, gid);
+      if (gid == GPX_NAME_NONE || !g.live) {
+        st = GPX_WS_UNKNOWN_NAME;
+      } else if (W.version[gid] != ver) {
+        st = GPX_WS_VERSION; /* PISM :441-447 */
+      } else {
+        node = A.pkts[mb.pkt].node;
+        lane = S.L;
+        for (uint32_t l = 0; l < S.L; l++)
+          if (S.lane_node[l] == node) lane = l;
+        if (lane == S.L || wire_member_idx(g.ms, g.R, node) == 0xffu) st = GPX_WS_NOT_LOCAL;
+      }
+    }
+  }
+  if (!A.emit) {
+    A.status[i] = st;
+    A.cnt[i] = st == GPX_WS_OK ? nreq : 0u;
+    A.cnt[A.n + i] = st == GPX_WS_OK ? pay : 0u;
+    return;
+  }
+  uint32_t o = A.off[i], po = A.off[A.n + i];
+  json_put_request(A, o++, &po, gid, i, node, lane, J, f);
+  if (!pos[JQ_BATCH]) return;
+  JRd B = J;
+  B.n = pos[JQ_BATCH] + 1u;
+  jr_ws(B);
+  if (jr_peek(B) == ']') return;
+  for (;;) {
+    uint32_t sp[JQ_N];
+    json_keys_t<JsonReqKeys>(B, sp, nullptr, &ppc);
+    JsonReq g;
+    json_req_fields(B, sp, g);
+    json_put_request(A, o++, &po, gid, i, node, lane, B, g);
+    jr_ws(B);
+    if (jr_peek(B) != ',') return;
+    B.n++;
+  }
+}

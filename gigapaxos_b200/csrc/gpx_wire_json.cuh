@@ -501,6 +501,12 @@ __device__ __forceinline__ int json_key(const JStr& s) {
   }
 }
 
+/* the key table of the packets and members above: json_key, JK_N of them, JK_PP the array a top level jumps over */
+struct JsonPktKeys {
+  enum { N = JK_N, PP = JK_PP };
+  __device__ __forceinline__ static int id(const JStr& s) { return json_key(s); }
+};
+
 /* the PP jump of a packet's top level: PP's '[' at p closes at the first depth-1 close after p */
 struct JsonJump {
   const uint32_t* close;
@@ -508,8 +514,11 @@ struct JsonJump {
 };
 /* phase 1 of an object at J.n: every key's value is validated (the PP array of a top level only by its members'
  * threads: jumped over) and the last position of each known key's value kept (0 = absent: a value is never at
- * arena offset 0).  pp_close: the ']' of the jumped PP. */
-__device__ __forceinline__ void json_keys(JRd& J, uint32_t* pos, const JsonJump* jump, uint32_t* pp_close) {
+ * arena offset 0).  pp_close: the ']' of the jumped PP.  Keys: the key table (JsonPktKeys, or a table without a PP
+ * whose PP is -2, which no key has). */
+template <typename Keys>
+__device__ __forceinline__ void json_keys_t(JRd& J, uint32_t* pos, const JsonJump* jump, uint32_t* pp_close) {
+  constexpr int JK_N = Keys::N, JK_PP = Keys::PP;
   for (int q = 0; q < JK_N; q++) pos[q] = 0;
   jr_ws(J);
   jr_eat(J, '{');
@@ -525,7 +534,7 @@ __device__ __forceinline__ void json_keys(JRd& J, uint32_t* pos, const JsonJump*
     jr_eat(J, ':');
     jr_ws(J);
     if (!J.ok) return;
-    const int kid = json_key(key);
+    const int kid = Keys::id(key);
     if (kid == JK_PP && *pp_close != GPX_JSON_NONE) { /* a duplicated PP: validate the jumped one, the last counts */
       JRd V = J;
       V.n = pos[JK_PP];
@@ -556,6 +565,9 @@ __device__ __forceinline__ void json_keys(JRd& J, uint32_t* pos, const JsonJump*
     jr_eat(J, '}');
     return;
   }
+}
+__device__ __forceinline__ void json_keys(JRd& J, uint32_t* pos, const JsonJump* jump, uint32_t* pp_close) {
+  json_keys_t<JsonPktKeys>(J, pos, jump, pp_close);
 }
 __device__ __forceinline__ bool json_at(JRd& J, uint32_t at) {
   if (!at) return false;
@@ -730,6 +742,26 @@ struct JsonDecSink { /* BatchedCommit SLOTS */
     key[j] = d.gid;
   }
 };
+
+/* the gid named by the "ID" string at `at` (id: what jr_string read of it), unescaped before the lookup, or
+ * GPX_NAME_NONE; a name with a character above U+00FF or longer than GPX_WIRE_MAX_ID names no gid.  k_json_req calls
+ * it; k_json_member below keeps the same steps inline, which leaves its instructions as they were. */
+__device__ __forceinline__ uint32_t json_id_gid(const WireNames& W, const JRd& J, uint32_t at, const JStr& id) {
+  if (id.wide || id.len > GPX_WIRE_MAX_ID) return GPX_NAME_NONE;
+  uint8_t buf[GPX_WIRE_MAX_ID];
+  const uint8_t* name = J.b + at + 1u;
+  if (id.esc) {
+    JRd I = J;
+    I.n = at + 1u;
+    uint32_t u = 0;
+    for (uint32_t q = 0; q < id.len; q++) {
+      jr_unit(I, &u);
+      buf[q] = (uint8_t)u;
+    }
+    name = buf;
+  }
+  return wire_name_find(W, name, id.len);
+}
 
 /* one thread per member (the device count of them; cap_mem slots).  Pass 0: parse and validate the member, the
  * separators after it, its name, version and locality: status and record counts, the packet's bad flag on a schema

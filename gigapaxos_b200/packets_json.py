@@ -222,6 +222,39 @@ def _request_obj(paxos_id, version, pt, req_id, value: bytes, entry_replica, ent
     return d
 
 
+def _request_smart(r, pt: int) -> dict:
+    d = _base(pt, r.paxos_id, r.version)
+    d.update({"QID": int(r.request_id), "QV": bytes(r.value).decode(CHARSET)})
+    if r.response:
+        d["RV"] = bytes(r.response).decode(CHARSET)
+    d["ET"] = int(r.entry_time)
+    if r.forward_count > 0:
+        d["NFWDS"] = int(r.forward_count)
+    if r.stop:
+        d["STOP"] = True
+    d["E"] = int(r.entry_replica)
+    for key, a in (("CA", r.client), ("LA", r.listen)):
+        if a is not None:
+            d[key] = f"/{a[0]}:{int(a[1])}"  # InetSocketAddress.toString() of a literal address
+    if r.should_return:
+        d["QF"] = True
+    if r.batched:
+        d["BATCH"] = [_request_smart(b, PT_REQUEST) for b in r.batched]
+    if r.broadcasted:
+        d["BC"] = True
+    if r.digest:
+        d["DIG"] = bytes(r.digest).decode(CHARSET)
+    return d
+
+
+def request_json(r, pt: int = PT_REQUEST) -> bytes:
+    """RequestPacket.toJSONSmartImpl :697-742 of a wire.Request: QID, QV, RV (a response), ET, NFWDS (forwardCount > 0),
+    STOP, E, CA and LA (InetSocketAddress.toString(): "/1.2.3.4:5678"), QF, BATCH (the batched requests' own objects),
+    BC and DIG, over PaxosPacket's type / PT / ID / V.  A Java peer's forwarded requests arrive in this form, as members
+    of a batched_paxos_packet_json wrapper."""
+    return _dumps(_request_smart(r, pt))
+
+
 def accepted_pvalue_obj(paxos_id: str, version: int, pv, blob: bytes, entry_replica: int = -1, entry_time: int = 0,
                         pt: int = PT_ACCEPT) -> dict:
     """One entry of ACC_MAP: the PValuePacket JSON (PaxosPacket.toJSONObject :478-494 + PValuePacket.toJSONObjectImpl

@@ -487,3 +487,41 @@ def encode_accepts_device(engine, accepts, n_ptr: Optional[int], n_max: int, hea
                           (_dptr(accepts), C.c_void_p(n_ptr) if n_ptr else None, C.c_uint32(n_max), _dptr(heads),
                            _dptr(reqs), _dptr(meta), C.c_uint32(n_reqs), _dptr(payload)), n_max, accepts.device, caps,
                           stream)
+
+
+# ---- forwarding: a non-coordinator's REQUEST packets, and a Java peer's forwards in JSON wrappers ---------------------
+def encode_forwards_device(engine, reqs, meta, n: int, status, payload, down_nodes: Sequence[int], caps,
+                           stream=None) -> EncodeOut:
+    """gpx_wire_encode_forwards_device: the forwarded requests among the first n of reqs / meta (propose_device's input,
+    with its statuses and payload arena) as REQUEST packets addressed to their coordinators; down_nodes are the nodes
+    the host takes for down.  caps = (packet bytes, packets); GPX_ERANGE as in decode_batch_device.  Returns rstatus
+    uint8 [n] (WE_SENT, WE_VOID, WE_ELECT, WE_NO_NAME), the packet arena, refs [k, 16] in request order and the two host
+    sizes."""
+    down = np.ascontiguousarray(list(down_nodes) or [0], dtype=np.int32)
+    return _encode_device(engine, "wire_encode_forwards_device",
+                          (_dptr(reqs), _dptr(meta), C.c_uint32(n), _dptr(status), _dptr(payload),
+                           C.c_uint32(len(down_nodes)), down.ctypes.data_as(C.c_void_p)), n, reqs.device, caps, stream)
+
+
+def decode_json_requests_device(engine, arena, refs, members, n_members: int, now_ms: int, caps,
+                                stream=None) -> RequestsOut:
+    """gpx_wire_decode_json_requests_device: the REQUEST members among the first n_members rows of `members` (what
+    decode_json_device returned for the same arena and refs; the refs' node column names the receiving node).
+    caps = (requests, payload bytes); GPX_ERANGE as in decode_batch_device.  Returns status int32 [n_members] (the
+    decoded members' statuses, the others copied), reqs [k, 32] and meta [k, 32] grouped by gid (propose_device's input
+    form, client = the member index), the payload arena and the two host sizes."""
+    import torch
+    n, dev = int(n_members), members.device
+    L, st = engine.L, stream_handle(stream)
+    with _on(stream):
+        status = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+        (reqs, meta, pay), caps = _sized(
+            engine, caps, (C.c_uint32, C.c_uint64),
+            lambda c: (torch.empty((max(c[0], 1), 32), dtype=torch.uint8, device=dev),
+                       torch.empty((max(c[0], 1), 32), dtype=torch.uint8, device=dev),
+                       torch.empty(max(c[1], 16), dtype=torch.uint8, device=dev)),
+            lambda o, sz: L.fn("wire_decode_json_requests_device")(
+                engine.handle, C.c_uint32(n), _dptr(arena), C.c_uint64(arena.numel()), _dptr(refs),
+                C.c_uint32(int(refs.shape[0])), _dptr(members), C.c_int64(now_ms), _dptr(status), _dptr(o[0]),
+                _dptr(o[1]), sz[0], _dptr(o[2]), sz[1], st))
+    return RequestsOut(status[:n], reqs[: caps[0]], meta[: caps[0]], pay[: caps[1]], caps)

@@ -1086,6 +1086,71 @@ int gpx_wire_encode_accepts_device(gpx_engine* e, const gpx_accept_rec* accepts,
                                    uint32_t n_reqs, const uint8_t* payload, uint8_t* rstatus, uint8_t* out,
                                    uint64_t* out_bytes, gpx_wire_ref* refs, uint32_t* n_refs, void* stream);
 
+/* ---- forwarding: a non-coordinator's REQUEST packets to the coordinator -------------------------------------------
+ * Clients send to any replica, and the coordinators are spread over the members, so most requests enter at a node that
+ * does not coordinate their group; that node forwards them (PISM.handleProposal :854-885).  gpx_propose_device gives
+ * them GPX_RS_FORWARD.  gpx_wire_encode_forwards_device writes the REQUEST packets the entry node sends, and the
+ * coordinator decodes them with gpx_wire_decode_requests_device -- or, when a Java peer sent them as JSON members of a
+ * BATCHED_PAXOS_PACKET, with gpx_wire_decode_json_requests_device. */
+#define GPX_WE_ELECT 6 /* encode_forwards: the host runs for coordinator (PISM.checkRunForCoordinator) instead */
+
+/* Encode the forwarded requests of a gpx_propose_device call as REQUEST packets.  reqs, meta (parallel to reqs, as in
+ * gpx_wire_encode_accepts_device), status and payload are that call's request array, its gpx_wire_req_meta, its
+ * statuses and its payload arena; run it after gpx_propose_device and before any call that changes the engine's state.
+ *   Which requests: status GPX_RS_FORWARD, and propose_run's routing on the current rows still says FORWARD for the
+ *     gid's run (the entry lane of the run's first request has no usable coordinator, and no local lane serves the
+ *     acceptor's ballot coordinator).  Proposing changes neither the acceptor rows nor whether a coordinator exists, so
+ *     this is k_propose's answer; it tells a forwarded request from one whose wrapped slot equals -2.  A broadcasted
+ *     request (GPX_RM_BROADCASTED) reached every replica already and is not forwarded (:854).
+ *   Packets: consecutive forwarded requests of one gid are cut as k_propose cuts a batch (BATCHING_ENABLED,
+ *     MAX_BATCH_SIZE, the byte bound with the size estimate).  A cut is one REQUEST packet, byte-identical to
+ *     gpx_wire_encode_request: the outer request is the cut's first with forwardCount + 1 (setForwarderID :437-441),
+ *     the others its `batched` REQUEST packets with their own meta, unchanged.
+ *   Destination: the ballot coordinator of the run's entry lane; when it is in down_nodes[n_down] (host, the nodes the
+ *     host takes for down: PaxosManager.isNodeUp), the next member after it in sorted order (getNextCoordinator
+ *     :2232-2241).
+ *   GPX_WE_ELECT for every request of the cut, and no packet, when the destination is a node a local lane serves
+ *     (coordinator == getMyID(), :869), the outer request ping-pongs after the increment (forwardCount > 3,
+ *     RequestPacket.isPingPonging :508), or the ballot coordinator is not a member.
+ * out[*out_bytes] receives the packets, refs[*n_refs] one {off, len, gid, node = destination} per packet in request
+ * order; rstatus[n]: GPX_WE_SENT for every request inside a packet, GPX_WE_VOID for one that is not forwarded,
+ * GPX_WE_ELECT, GPX_WE_NO_NAME.  *out_bytes and *n_refs are HOST pointers, capacities in / sizes out; GPX_ERANGE reports
+ * the sizes and writes nothing else.  All other pointers but down_nodes are device pointers.  Stream-ordered on `stream`
+ * (NULL = the engine's stream) with the other wire calls' scratch; one synchronisation reads the sizes. */
+int gpx_wire_encode_forwards_device(gpx_engine* e, const gpx_request_rec* reqs, const gpx_wire_req_meta* meta,
+                                    uint32_t n, const int32_t* status, const uint8_t* payload, uint32_t n_down,
+                                    const int32_t* down_nodes, uint8_t* rstatus, uint8_t* out, uint64_t* out_bytes,
+                                    gpx_wire_ref* refs, uint32_t* n_refs, void* stream);
+
+/* Decode the REQUEST members of JSON packets (a Java peer's forwards, BATCHED_PAXOS_PACKET members) into proposals.
+ * The input is what gpx_wire_decode_json_device returned for the same arena and refs: members[n_members], whose
+ * wrappers are not read again.  bytes, pkts, members, status, reqs, meta and payload are device pointers.
+ *   Which members: only those listed GPX_WS_UNHANDLED are examined; every other status is copied to status[i].  An
+ *     object with "PT":1 is decoded; any other type stays GPX_WS_UNHANDLED.
+ *   Schema (RequestPacket(net.minidev.json.JSONObject) :584-649, toJSONSmartImpl :697-742): "type" = 90, "PT", "ID"
+ *     (string) and "V" (int) as for every member; "QID" (int64), "QV" (string), "ET" (int64) and "E" (int32) required;
+ *     "NFWDS" (int32), "STOP", "QF", "BC" (bool), "CA", "LA" (string) and "BATCH" (an array of request objects, with
+ *     the same request keys, one level) optional; "FWDR", "DBG" and unknown keys are skipped.  The strictness rules are
+ *     gpx_wire_decode_json_device's.
+ *   status[i]: GPX_WS_MALFORMED for a schema failure, a BATCH entry with a BATCH of its own, or a member ref past
+ *     n_bytes or pkt past n_pkts.  GPX_WS_UNHANDLED when "RV" or "DIG" is present (as in the byte decoder), a "QV" has a
+ *     character above U+00FF, or a "CA" / "LA" is not [anything/]a.b.c.d:port with a port of 1-65535 -- that is
+ *     Util.getInetSocketAddressFromString :278-287 restricted to literal IPv4 addresses; a hostname needs a lookup and
+ *     port 0 means "no address" in the byte form, so the host decides both.  GPX_WS_UNKNOWN_NAME, GPX_WS_VERSION and
+ *     GPX_WS_NOT_LOCAL as gpx_wire_decode_requests_device judges them, the receiving node being pkts[members[i].pkt].node.
+ *   reqs, meta, payload: gpx_wire_decode_requests_device's outputs with client = the member index, byte-identical for
+ *     the same RequestPacket: an "E" of -1 becomes the receiving node and now_ms, an absent address is all zeros, "QV"
+ *     is unescaped into payload at 16-byte aligned offsets.  Grouped by gid, member order within a gid, a request's
+ *     BATCH after it: gpx_propose_device's input form.
+ * One thread handles one member, its BATCH included, so a very long "QV" is copied by one thread.  *n_reqs and
+ * *payload_bytes are HOST pointers, capacities in / sizes out, with GPX_ERANGE as above; stream-ordered, one
+ * synchronisation. */
+int gpx_wire_decode_json_requests_device(gpx_engine* e, uint32_t n_members, const uint8_t* bytes, uint64_t n_bytes,
+                                         const gpx_wire_ref* pkts, uint32_t n_pkts, const gpx_wire_member* members,
+                                         int64_t now_ms, int32_t* status, gpx_request_rec* reqs,
+                                         gpx_wire_req_meta* meta, uint32_t* n_reqs, uint8_t* payload,
+                                         uint64_t* payload_bytes, void* stream);
+
 /* ---- helpers shared with the reference semantics ---------------------------------- */
 int32_t gpx_java_string_hash(const char* s, size_t len); /* String.hashCode() */
 /* PISM.roundRobinCoordinator :2251-2256 on sorted members */
