@@ -354,23 +354,32 @@ __global__ void __launch_bounds__(GPX_BLOCK) k_propose(const __grid_constant__ D
   flush_counters(S, s_ctr);
 }
 
+/* request q's entry and body in the blob of its batched slot, [nreq x gpx_batch_ent][values] (RequestPacket.batched).
+ * copy_tab / copy_dst are payload-area offsets; the constructed blobs start at offset blob1_off, stored at blob1. */
+__device__ __forceinline__ void write_blob_entry(const ProposeArgs& P, const uint8_t* mark, uint32_t q,
+                                                 const uint8_t* payload, uint8_t* blob1, unsigned long long blob1_off) {
+  if (!mk_batched(mark, P.n, q)) return;
+  const gpx_request_rec r = P.reqs[q];
+  gpx_batch_ent be;
+  be.req_id = r.req_id;
+  be.len = r.payload_len;
+  be.flags = r.flags;
+  *reinterpret_cast<int4*>(blob1 + (P.copy_tab[q] - blob1_off)) = *reinterpret_cast<const int4*>(&be);
+  uint8_t* d = blob1 + (P.copy_dst[q] - blob1_off);
+  const uint8_t* sp = payload + r.payload_off;
+  uint32_t b = 0;
+  if ((((uint32_t)(uintptr_t)d | (uint32_t)(uintptr_t)sp) & 15u) == 0)
+    for (; b + 16 <= r.payload_len; b += 16) *reinterpret_cast<int4*>(d + b) = ld_stream4(sp + b);
+  for (; b < r.payload_len; b++) d[b] = sp[b];
+}
+
 /* builds the blobs of batched slots: [nreq x gpx_batch_ent][payloads], one thread per request */
 __global__ void __launch_bounds__(GPX_BLOCK) k_build_blobs(const __grid_constant__ ProposeArgs A,
                                                            const uint8_t* payload, uint8_t* blob1,
                                                            const uint8_t* mark) {
   if (!A.ctl->any_batched) return;
   const uint32_t i = blockIdx.x * GPX_BLOCK + threadIdx.x;
-  if (i >= A.n) return;
-  if (!mk_batched(mark, A.n, i)) return;
-  gpx_request_rec r = A.reqs[i];
-  gpx_batch_ent be;
-  be.req_id = r.req_id;
-  be.len = r.payload_len;
-  be.flags = r.flags;
-  *reinterpret_cast<int4*>(blob1 + (A.copy_tab[i] - A.payload_bytes_al)) = *reinterpret_cast<const int4*>(&be);
-  uint8_t* d = blob1 + (A.copy_dst[i] - A.payload_bytes_al);
-  const uint8_t* s = payload + r.payload_off;
-  for (uint32_t b = 0; b < r.payload_len; b++) d[b] = s[b];
+  if (i < A.n) write_blob_entry(A, mark, i, payload, blob1, A.payload_bytes_al);
 }
 
 /* ============================== shared per-lane steps ============================== */
@@ -420,6 +429,30 @@ __device__ __forceinline__ void make_entry(const int4 q0, const int4 q1, const i
   n0 = make_int4(q0.y, q0.z, q0.w, (int)frame_ref);
   n1 = make_int4(q1.z, q1.w, q2.y,
                  (int)(GPX_ENT_VALID | ((rflags & GPX_F_STOP) ? GPX_ENT_STOP : 0u) | ((uint32_t)q2.z << 16)));
+}
+
+/* lane l's aux word, row and window entry at slot mod W when the group is live; zeros otherwise */
+__device__ __forceinline__ void load_lane(const DevState& S, uint32_t l, uint32_t gid, int slot, bool live,
+                                          uint32_t& aux, int4& row, int4& e0, int4& e1) {
+  aux = 0;
+  row = e0 = e1 = make_int4(0, 0, 0, 0);
+  if (live) {
+    const size_t ri = row_idx(S, l, gid);
+    aux = S.acc_aux[ri];
+    row = S.acc_row[ri];
+    ld256(&S.acc_win[2 * win_idx(S, l, (uint32_t)slot & (S.W - 1), gid)], e0, e1);
+  }
+}
+
+/* AcceptReplyPacket.maxCheckpointedSlot :1139-1143 without GC_MAJORITY_EXECUTED: the last checkpoint at or below
+ * max_cp (lastCheckpointSlot, Java int arithmetic across the wrap) */
+__device__ __forceinline__ int last_cp(int max_cp, int cpi) {
+  int lcp = max_cp - max_cp % cpi;
+  if (lcp < 0) {
+    lcp = jsub(lcp, cpi);
+    if (lcp > 0) lcp = 2147483647 - 2147483647 % cpi;
+  }
+  return lcp;
 }
 
 /* PISM.handleAccept :1080-1166 for one ACCEPT at one lane, on register-resident state.  (e0,e1) is the
@@ -481,16 +514,7 @@ __device__ __forceinline__ void accept_lane(const DevState& S, const AcceptArgs&
   gc_step(row, median_cp); /* :320 */
   /* AcceptReplyPacket :1139-1143 */
   int max_cp = row.x - 1;
-  if (!S.gc_majority_executed) {
-    int cpi = S.cpi_per_group ? S.grp_cpi[gid] : S.cpi_const;
-    int s1 = row.x - 1;
-    int lcp = s1 - s1 % cpi;
-    if (lcp < 0) {
-      lcp = jsub(lcp, cpi);
-      if (lcp > 0) lcp = 2147483647 - 2147483647 % cpi;
-    }
-    max_cp = lcp;
-  }
+  if (!S.gc_majority_executed) max_cp = last_cp(max_cp, S.cpi_per_group ? S.grp_cpi[gid] : S.cpi_const);
   /* toLog :1146-1149 */
   const bool toLog = bcmp(bnum, bcoord, row.y, row.z) >= 0 && jsub(slot, row.w) > 0 &&
                      (!hasPrev || bcmp(e0.y, e0.z, bnum, bcoord) < 0);
@@ -555,6 +579,21 @@ __device__ __forceinline__ void accept_lane(const DevState& S, const AcceptArgs&
     if (st.aux != aux_b) st.fl |= LS_AUXDIRTY;
   }
   if (row.x != row_in.x || row.y != row_in.y || row.z != row_in.z || row.w != row_in.w) st.fl |= LS_ROWDIRTY;
+}
+
+/* writes back what accept_lane (and a commit behind it) left in registers: the accepted window entry (LS_STORE), the
+ * row (LS_ROWDIRTY) and the aux word (LS_AUXDIRTY) of lane l */
+__device__ __forceinline__ void store_accepted_lane(const DevState& S, uint32_t l, const int4 q0, const int4 q1,
+                                                    const int4 q2, const LaneSt& st) {
+  const uint32_t gid = (uint32_t)q0.x;
+  if (st.fl & LS_STORE) {
+    int4 n0, n1;
+    make_entry(q0, q1, q2, st.frame_ref, n0, n1);
+    ST_ACC(S, l, gid, 2 * win_idx(S, l, (uint32_t)q0.y & (S.W - 1), gid), n0, n1);
+  }
+  const size_t ri = row_idx(S, l, gid);
+  if (st.fl & LS_ROWDIRTY) S.acc_row[ri] = st.row;
+  if (st.fl & LS_AUXDIRTY) S.acc_aux[ri] = st.aux;
 }
 
 /* PISM.handleAcceptReply :1248-1365 for one reply at the coordinator lane `cl` (row cached in `crow`) */
@@ -794,6 +833,21 @@ __device__ __forceinline__ void commit_lane(const DevState& S, uint32_t l, uint3
     aux |= (GPX_GF_NEEDS_SYNC << 24);
 }
 
+/* commit_lane on the row and aux word as loaded, each written back only if the commit changed it */
+__device__ __forceinline__ void commit_lane_stored(const DevState& S, uint32_t l, uint32_t gid, int slot, int bnum,
+                                                   int bcoord, int median_cp, int4 row, uint32_t aux, const int4 a0,
+                                                   const int4 a1, gpx_exec_rec* ex, gpx_exec_rec* extra,
+                                                   uint32_t extra_cap, uint32_t* n_extra, int4& img0, int4& img1,
+                                                   unsigned int* s_ctr) {
+  const int4 row_in = row;
+  const uint32_t aux_in = aux;
+  commit_lane(S, l, gid, slot, bnum, bcoord, median_cp, row, aux, a0, a1, ex, extra, extra_cap, n_extra, img0, img1,
+              s_ctr);
+  const size_t ri = row_idx(S, l, gid);
+  if (aux != aux_in) S.acc_aux[ri] = aux;
+  if (row.x != row_in.x || row.y != row_in.y || row.z != row_in.z || row.w != row_in.w) S.acc_row[ri] = row;
+}
+
 __device__ __forceinline__ void write_seg_hdr(const DevState& S, uint32_t l, unsigned long long base, uint16_t type,
                                               uint32_t n_slots, uint32_t n_valid, unsigned long long pay_bytes,
                                               uint32_t rec_bytes, unsigned long long seq) {
@@ -857,6 +911,99 @@ __device__ __forceinline__ void store_void_exec(gpx_exec_rec* ex, uint32_t gid, 
   store_exec(ex, vx);
 }
 
+/* Commit of decision d (decided: d is one) at lane l right behind accept_lane on the same ACCEPT (q0,q1,q2), state
+ * in registers: EXEC record at ex, DECISION log image at ring offset dimg, then the write-back of the entry, row
+ * and aux word. */
+__device__ __forceinline__ void commit_accepted_lane(const DevState& S, const AcceptArgs& A, uint32_t l, uint32_t gid,
+                                                     int slot, bool live, bool decided, const gpx_decision_rec& d,
+                                                     const int4 q0, const int4 q1, const int4 q2, LaneSt& st,
+                                                     gpx_exec_rec* ex, unsigned long long dimg, unsigned int* s_ctr) {
+  const uint32_t Wm = S.W - 1;
+  int4 img0 = make_int4((int)gid, slot, d.bnum, d.bcoord);
+  int4 img1 = make_int4(d.median_cp, (int)(GPX_F_VOID | ((uint32_t)d.dst_mask << 16)),
+                        (int)(unsigned)(d.req_id & 0xffffffffll), (int)(d.req_id >> 32));
+  const size_t ai = 2 * win_idx(S, l, (uint32_t)slot & Wm, gid);
+  int4& row = st.row;
+  uint32_t& aux = st.aux;
+  if (!(decided && ((d.dst_mask >> l) & 1u))) {
+    store_void_exec(ex, gid, slot, l);
+  } else if (!live || !st_usable(aux)) {
+    store_void_exec(ex, gid, slot, l);
+    atomicAdd(&s_ctr[C_DECISIONS_DROPPED], 1u);
+  } else {
+    const int4 row_b = row;
+    const uint32_t aux_b = aux;
+    const bool fast = (st.fl & LS_STORE) && q0.z == d.bnum && q0.w == d.bcoord && slot == row.x &&
+                      !((GPX_AUX_PRESENT(aux) >> ((uint32_t)slot & Wm)) & 1u);
+    if (fast) {
+      /* the accept stored a moment ago is the decided value and it is next in line:
+       * handleBatchedCommit :1488-1501 + the first iteration of extractExecuteAndCheckpoint */
+      atomicAdd(&s_ctr[C_DECISIONS_HANDLED], 1u);
+      int4 n0, n1;
+      make_entry(q0, q1, q2, st.frame_ref, n0, n1);
+      const unsigned efl = (unsigned)n1.w;
+      const bool metaf = S.log_meta != 0;
+      const uint32_t lf = GPX_F_DECISION | (metaf ? GPX_F_META : 0u) | ((efl & GPX_ENT_STOP) ? GPX_F_STOP : 0u);
+      img0 = make_int4((int)gid, slot, d.bnum, d.bcoord);
+      img1 = make_int4(metaf ? -1 : d.median_cp, (int)(lf | ((1u << l) << 16)), n1.x, n1.y);
+      gc_step(row, d.median_cp);
+      DPValue x;
+      x.slot = slot;
+      x.bnum = d.bnum;
+      x.bcoord = d.bcoord;
+      x.median_cp = d.median_cp;
+      x.req_id = ((long long)n1.y << 32) | (unsigned)n1.x;
+      x.frame_ref = st.frame_ref;
+      x.plen = (unsigned)n1.z;
+      x.fl = efl & ~GPX_ENT_VALID;
+      x.valued = true;
+      row.x = (int)((unsigned)row.x + 1u); /* executed(): _slot++ */
+      atomicAdd(&s_ctr[C_EXECUTED], 1u);
+      gpx_exec_rec er = make_exec(S, gid, l, x, false);
+      if (er.flags & GPX_F_CKPT) atomicAdd(&s_ctr[C_CKPTS_DUE], 1u);
+      store_exec(ex, er);
+      bool more = true;
+      if (efl & GPX_ENT_STOP) {
+        aux = (aux & ~0xffu) | GPX_ST_STOPPED; /* stop() + committedRequests.clear() */
+        aux &= ~0x00ffff00u;
+        atomicAdd(&s_ctr[C_STOPS_EXECUTED], 1u);
+        more = false;
+      }
+      if (S.journaling) {
+        /* acceptedProposals.remove(slot): the entry only has to reach HBM (invalidated) when it must
+         * hide an occupant of the ring position whose valid bit is set */
+        if (st.fl & LS_OCCVALID) {
+          n1.w = (int)((unsigned)n1.w & ~GPX_ENT_VALID);
+          ST_ACC(S, l, gid, ai, n0, n1);
+        }
+      } else
+        ST_ACC(S, l, gid, ai, n0, n1);
+      st.fl &= ~LS_STORE;
+      if (more) { /* second iteration: GC with the advanced slot, then any queued commits */
+        gc_step(row, d.median_cp);
+        if ((GPX_AUX_PRESENT(aux) >> ((uint32_t)row.x & Wm)) & 1u)
+          eec(S, l, gid, row, aux, x, nullptr, A.extra, A.extra_cap, A.n_extra, s_ctr, true);
+      }
+    } else {
+      /* general path through memory: make the accepted entry visible, then commit */
+      int4 a0, a1; /* rare path: re-read the entry instead of keeping L x 32 B of registers alive */
+      if (st.fl & LS_STORE) {
+        make_entry(q0, q1, q2, st.frame_ref, a0, a1);
+        ST_ACC(S, l, gid, ai, a0, a1);
+        st.fl &= ~LS_STORE;
+      } else
+        ld256(&S.acc_win[ai], a0, a1);
+      store_void_exec(ex, gid, slot, l);
+      commit_lane(S, l, gid, slot, d.bnum, d.bcoord, d.median_cp, row, aux, a0, a1, ex, A.extra, A.extra_cap,
+                  A.n_extra, img0, img1, s_ctr);
+    }
+    if (aux != aux_b) st.fl |= LS_AUXDIRTY;
+    if (row.x != row_b.x || row.y != row_b.y || row.z != row_b.z || row.w != row_b.w) st.fl |= LS_ROWDIRTY;
+  }
+  store_accepted_lane(S, l, q0, q1, q2, st);
+  st256_stream(ring_ptr(S, l, dimg), img0, img1);
+}
+
 /* ============================== k_accept ====================================== */
 template <int L>
 __global__ void __launch_bounds__(GPX_BLOCK, GPX_ACCEPT_MINB) k_accept(const __grid_constant__ DevState S,
@@ -875,7 +1022,6 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_ACCEPT_MINB) k_accept(const __g
   const uint32_t t0 = i0 ? i0 - 1u : 0u, t1 = min(n, i0 + GPX_BLOCK); /* records [t0, t1) are staged */
   const uint32_t tile_bytes = t1 > t0 ? (t1 - t0) * (uint32_t)sizeof(gpx_accept_rec) : 0u;
   if (threadIdx.x == 0 && tile_bytes) tma_load_1d(s_tile, &A.recs[t0], tile_bytes, &s_bar);
-  const uint32_t Wm = S.W - 1;
   const unsigned long long pay_bytes = A.blob0_bytes + (A.blob1_used_ptr ? *A.blob1_used_ptr : A.blob1_bytes);
   const unsigned long long pay_rel = 64ull + (unsigned long long)A.n_max * 48ull;
   const unsigned long long reserved = (pay_rel + pay_bytes + 31ull) & ~31ull; /* images need 32-B alignment */
@@ -909,17 +1055,8 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_ACCEPT_MINB) k_accept(const __g
         LaneSt st[L];
         int4 e0[L], e1[L];
 #pragma unroll
-        for (int l = 0; l < L; l++) { /* all independent loads first */
-          st[l].aux = 0;
-          st[l].row = make_int4(0, 0, 0, 0);
-          e0[l] = e1[l] = make_int4(0, 0, 0, 0);
-          if (g.live) {
-            const size_t ri = row_idx(S, l, gid);
-            st[l].aux = S.acc_aux[ri];
-            st[l].row = S.acc_row[ri];
-            ld256(&S.acc_win[2 * win_idx(S, l, (uint32_t)slot & Wm, gid)], e0[l], e1[l]);
-          }
-        }
+        for (int l = 0; l < L; l++) /* all independent loads first */
+          load_lane(S, l, gid, slot, g.live, st[l].aux, st[l].row, e0[l], e1[l]);
         uint32_t dstIdx = 0xffu;
         if (g.live)
           for (uint32_t m = 0; m < g.R; m++)
@@ -929,14 +1066,7 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_ACCEPT_MINB) k_accept(const __g
         for (int l = 0; l < L; l++) {
           const unsigned fr = (unsigned)(((payb[l] + payload_off) & (S.ring_cap - 1)) >> 4);
           accept_lane(S, A, l, g.live, g.ms, dstIdx, q0, q1, q2, e0[l], e1[l], fr, st[l], s_ctr);
-          const size_t ri = row_idx(S, l, gid);
-          if (st[l].fl & LS_STORE) {
-            int4 n0, n1;
-            make_entry(q0, q1, q2, st[l].frame_ref, n0, n1);
-            ST_ACC(S, l, gid, 2 * win_idx(S, l, (uint32_t)slot & Wm, gid), n0, n1);
-          }
-          if (st[l].fl & LS_ROWDIRTY) S.acc_row[ri] = st[l].row;
-          if (st[l].fl & LS_AUXDIRTY) S.acc_aux[ri] = st[l].aux;
+          store_accepted_lane(S, l, q0, q1, q2, st[l]);
           if (st[l].fl & LS_LOGGED) logmask |= 1u << l;
           st256_stream(&A.replies[(size_t)j * L + l], make_int4((int)gid, slot, st[l].rbn, st[l].rbc),
                        (GPX_WHO_FLAGS(st[l].rwho) & GPX_F_VOID) ? make_int4(0, (int)st[l].rwho, 0, 0)
@@ -1212,7 +1342,6 @@ __global__ void __launch_bounds__(GPX_BLOCK, 2) k_commit(const __grid_constant__
   uint32_t n = A.n_ptr ? *A.n_ptr : A.n_max;
   if (n > A.n_max) n = A.n_max;
   const uint32_t i = blockIdx.x * GPX_BLOCK + threadIdx.x;
-  const uint32_t Wm = S.W - 1;
   const unsigned long long reserved = 64ull + (unsigned long long)A.n_max * 32ull;
   unsigned long long segb[L];
 #pragma unroll
@@ -1240,34 +1369,18 @@ __global__ void __launch_bounds__(GPX_BLOCK, 2) k_commit(const __grid_constant__
         uint32_t aux[L];
         int4 row[L], e0[L], e1[L];
 #pragma unroll
-        for (int l = 0; l < L; l++) {
-          aux[l] = 0;
-          row[l] = e0[l] = e1[l] = make_int4(0, 0, 0, 0);
-          if (g.live) {
-            const size_t ri = row_idx(S, l, gid);
-            aux[l] = S.acc_aux[ri];
-            row[l] = S.acc_row[ri];
-            ld256(&S.acc_win[2 * win_idx(S, l, (uint32_t)slot & Wm, gid)], e0[l], e1[l]);
-          }
-        }
+        for (int l = 0; l < L; l++) load_lane(S, l, gid, slot, g.live, aux[l], row[l], e0[l], e1[l]);
 #pragma unroll
         for (int l = 0; l < L; l++) {
           gpx_exec_rec* ex = &A.exec[(size_t)j * L + l];
           store_void_exec(ex, gid, slot, l);
           int4 img0 = q0, img1 = make_int4(q1.x, (int)(GPX_F_VOID | (dst_mask << 16)), q1.z, q1.w);
           if (((dst_mask >> l) & 1u) && !(rflags & GPX_F_VOID)) {
-            if (!g.live || !st_usable(aux[l])) {
+            if (!g.live || !st_usable(aux[l]))
               atomicAdd(&s_ctr[C_DECISIONS_DROPPED], 1u);
-            } else {
-              const size_t ri = row_idx(S, l, gid);
-              const int4 row_in = row[l];
-              const uint32_t aux_in = aux[l];
-              commit_lane(S, l, gid, slot, q0.z, q0.w, q1.x, row[l], aux[l], e0[l], e1[l], ex, A.extra, A.extra_cap,
-                          A.n_extra, img0, img1, s_ctr);
-              const int4 r2 = row[l];
-              if (aux[l] != aux_in) S.acc_aux[ri] = aux[l];
-              if (r2.x != row_in.x || r2.y != row_in.y || r2.z != row_in.z || r2.w != row_in.w) S.acc_row[ri] = r2;
-            }
+            else
+              commit_lane_stored(S, l, gid, slot, q0.z, q0.w, q1.x, row[l], aux[l], e0[l], e1[l], ex, A.extra,
+                                 A.extra_cap, A.n_extra, img0, img1, s_ctr);
           }
           st256_stream(ring_ptr(S, l, segb[l] + 64 + (unsigned long long)j * 32), img0, img1);
         }
@@ -1300,7 +1413,6 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_ACT_MINB) k_act(const __grid_co
   uint32_t n = A.n_ptr ? *A.n_ptr : A.n_max;
   if (n > A.n_max) n = A.n_max;
   const uint32_t i = blockIdx.x * GPX_BLOCK + threadIdx.x;
-  const uint32_t Wm = S.W - 1;
   const unsigned long long pay_bytes = A.blob0_bytes + (A.blob1_used_ptr ? *A.blob1_used_ptr : A.blob1_bytes);
   const unsigned long long pay_rel = 64ull + (unsigned long long)A.n_max * 48ull;
   const unsigned long long res_a = (pay_rel + pay_bytes + 31ull) & ~31ull;
@@ -1337,17 +1449,7 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_ACT_MINB) k_act(const __grid_co
         LaneSt st[L];
         int4 e0[L], e1[L];
 #pragma unroll
-        for (int l = 0; l < L; l++) {
-          st[l].aux = 0;
-          st[l].row = make_int4(0, 0, 0, 0);
-          e0[l] = e1[l] = make_int4(0, 0, 0, 0);
-          if (g.live) {
-            const size_t ri = row_idx(S, l, gid);
-            st[l].aux = S.acc_aux[ri];
-            st[l].row = S.acc_row[ri];
-            ld256(&S.acc_win[2 * win_idx(S, l, (uint32_t)slot & Wm, gid)], e0[l], e1[l]);
-          }
-        }
+        for (int l = 0; l < L; l++) load_lane(S, l, gid, slot, g.live, st[l].aux, st[l].row, e0[l], e1[l]);
         uint32_t dstIdx = 0xffu;
         if (g.live)
           for (uint32_t m = 0; m < g.R; m++)
@@ -1409,99 +1511,9 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_ACT_MINB) k_act(const __grid_co
         }
         /* ---- commit the decision at every lane ---- */
 #pragma unroll
-        for (int l = 0; l < L; l++) {
-          gpx_exec_rec* ex = &A.exec[(size_t)j * L + l];
-          int4 img0 = make_int4((int)gid, slot, d.bnum, d.bcoord);
-          int4 img1 = make_int4(d.median_cp, (int)(GPX_F_VOID | ((uint32_t)d.dst_mask << 16)),
-                                (int)(unsigned)(d.req_id & 0xffffffffll), (int)(d.req_id >> 32));
-          const size_t ai = 2 * win_idx(S, l, (uint32_t)slot & Wm, gid);
-          const size_t ri = row_idx(S, l, gid);
-          int4& row = st[l].row;
-          uint32_t& aux = st[l].aux;
-          if (!(decided && ((d.dst_mask >> l) & 1u))) {
-            store_void_exec(ex, gid, slot, l);
-          } else if (!g.live || !st_usable(aux)) {
-            store_void_exec(ex, gid, slot, l);
-            atomicAdd(&s_ctr[C_DECISIONS_DROPPED], 1u);
-          } else {
-            const int4 row_b = row;
-            const uint32_t aux_b = aux;
-            const bool fast = (st[l].fl & LS_STORE) && q0.z == d.bnum && q0.w == d.bcoord && slot == row.x &&
-                              !((GPX_AUX_PRESENT(aux) >> ((uint32_t)slot & Wm)) & 1u);
-            if (fast) {
-              /* the accept stored a moment ago is the decided value and it is next in line:
-               * handleBatchedCommit :1488-1501 + the first iteration of extractExecuteAndCheckpoint */
-              atomicAdd(&s_ctr[C_DECISIONS_HANDLED], 1u);
-              int4 n0, n1;
-              make_entry(q0, q1, q2, st[l].frame_ref, n0, n1);
-              const unsigned efl = (unsigned)n1.w;
-              const bool metaf = S.log_meta != 0;
-              const uint32_t lf = GPX_F_DECISION | (metaf ? GPX_F_META : 0u) | ((efl & GPX_ENT_STOP) ? GPX_F_STOP : 0u);
-              img0 = make_int4((int)gid, slot, d.bnum, d.bcoord);
-              img1 = make_int4(metaf ? -1 : d.median_cp, (int)(lf | ((1u << l) << 16)), n1.x, n1.y);
-              gc_step(row, d.median_cp);
-              DPValue x;
-              x.slot = slot;
-              x.bnum = d.bnum;
-              x.bcoord = d.bcoord;
-              x.median_cp = d.median_cp;
-              x.req_id = ((long long)n1.y << 32) | (unsigned)n1.x;
-              x.frame_ref = st[l].frame_ref;
-              x.plen = (unsigned)n1.z;
-              x.fl = efl & ~GPX_ENT_VALID;
-              x.valued = true;
-              row.x = (int)((unsigned)row.x + 1u); /* executed(): _slot++ */
-              atomicAdd(&s_ctr[C_EXECUTED], 1u);
-              gpx_exec_rec er = make_exec(S, gid, l, x, false);
-              if (er.flags & GPX_F_CKPT) atomicAdd(&s_ctr[C_CKPTS_DUE], 1u);
-              store_exec(ex, er);
-              bool more = true;
-              if (efl & GPX_ENT_STOP) {
-                aux = (aux & ~0xffu) | GPX_ST_STOPPED; /* stop() + committedRequests.clear() */
-                aux &= ~0x00ffff00u;
-                atomicAdd(&s_ctr[C_STOPS_EXECUTED], 1u);
-                more = false;
-              }
-              if (S.journaling) {
-                /* acceptedProposals.remove(slot): the entry only has to reach HBM (invalidated) when it must
-                 * hide an occupant of the ring position whose valid bit is set */
-                if (st[l].fl & LS_OCCVALID) {
-                  n1.w = (int)((unsigned)n1.w & ~GPX_ENT_VALID);
-                  ST_ACC(S, l, gid, ai, n0, n1);
-                }
-              } else
-                ST_ACC(S, l, gid, ai, n0, n1);
-              st[l].fl &= ~LS_STORE;
-              if (more) { /* second iteration: GC with the advanced slot, then any queued commits */
-                gc_step(row, d.median_cp);
-                if ((GPX_AUX_PRESENT(aux) >> ((uint32_t)row.x & Wm)) & 1u)
-                  eec(S, l, gid, row, aux, x, nullptr, A.extra, A.extra_cap, A.n_extra, s_ctr, true);
-              }
-            } else {
-              /* general path through memory: make the accepted entry visible, then commit */
-              int4 a0, a1; /* rare path: re-read the entry instead of keeping L x 32 B of registers alive */
-              if (st[l].fl & LS_STORE) {
-                make_entry(q0, q1, q2, st[l].frame_ref, a0, a1);
-                ST_ACC(S, l, gid, ai, a0, a1);
-                st[l].fl &= ~LS_STORE;
-              } else
-                ld256(&S.acc_win[ai], a0, a1);
-              store_void_exec(ex, gid, slot, l);
-              commit_lane(S, l, gid, slot, d.bnum, d.bcoord, d.median_cp, row, aux, a0, a1, ex, A.extra, A.extra_cap,
-                          A.n_extra, img0, img1, s_ctr);
-            }
-            if (aux != aux_b) st[l].fl |= LS_AUXDIRTY;
-            if (row.x != row_b.x || row.y != row_b.y || row.z != row_b.z || row.w != row_b.w) st[l].fl |= LS_ROWDIRTY;
-          }
-          if (st[l].fl & LS_STORE) {
-            int4 n0, n1;
-            make_entry(q0, q1, q2, st[l].frame_ref, n0, n1);
-            ST_ACC(S, l, gid, ai, n0, n1);
-          }
-          if (st[l].fl & LS_ROWDIRTY) S.acc_row[ri] = row;
-          if (st[l].fl & LS_AUXDIRTY) S.acc_aux[ri] = aux;
-          st256_stream(ring_ptr(S, l, dsegb[l] + 64 + (unsigned long long)j * 32), img0, img1);
-        }
+        for (int l = 0; l < L; l++)
+          commit_accepted_lane(S, A, l, gid, slot, g.live, decided, d, q0, q1, q2, st[l], &A.exec[(size_t)j * L + l],
+                               dsegb[l] + 64 + (unsigned long long)j * 32, s_ctr);
         j++;
         if (j >= n) break;
         rp = reinterpret_cast<const int4*>(&A.recs[j]);

@@ -75,101 +75,6 @@ __device__ __forceinline__ void store_sum(gpx_exec_sum* dst, int slot, uint32_t 
                           * 100 K and 1 M groups */
 #endif
 
-/* commit of decision d at one lane, state in registers (the per-lane part of k_act's commit phase) */
-template <int L>
-__device__ __forceinline__ void commit_team_lane(const DevState& S, const AcceptArgs& A, uint32_t l, uint32_t gid,
-                                                 int slot, bool live, bool decided, const gpx_decision_rec& d,
-                                                 const int4 q0, const int4 q1, const int4 q2, LaneSt& st, uint32_t j,
-                                                 unsigned long long dseg, unsigned int* s_ctr) {
-  const uint32_t Wm = S.W - 1;
-  gpx_exec_rec* ex = &A.exec[(size_t)j * L + l];
-  int4 img0 = make_int4((int)gid, slot, d.bnum, d.bcoord);
-  int4 img1 = make_int4(d.median_cp, (int)(GPX_F_VOID | ((uint32_t)d.dst_mask << 16)),
-                        (int)(unsigned)(d.req_id & 0xffffffffll), (int)(d.req_id >> 32));
-  const size_t ai = 2 * win_idx(S, l, (uint32_t)slot & Wm, gid);
-  const size_t ri = row_idx(S, l, gid);
-  int4& row = st.row;
-  uint32_t& aux = st.aux;
-  if (!(decided && ((d.dst_mask >> l) & 1u))) {
-    store_void_exec(ex, gid, slot, l);
-  } else if (!live || !st_usable(aux)) {
-    store_void_exec(ex, gid, slot, l);
-    atomicAdd(&s_ctr[C_DECISIONS_DROPPED], 1u);
-  } else {
-    const int4 row_b = row;
-    const uint32_t aux_b = aux;
-    const bool fast = (st.fl & LS_STORE) && q0.z == d.bnum && q0.w == d.bcoord && slot == row.x &&
-                      !((GPX_AUX_PRESENT(aux) >> ((uint32_t)slot & Wm)) & 1u);
-    if (fast) {
-      atomicAdd(&s_ctr[C_DECISIONS_HANDLED], 1u);
-      int4 n0, n1;
-      make_entry(q0, q1, q2, st.frame_ref, n0, n1);
-      const unsigned efl = (unsigned)n1.w;
-      const bool metaf = S.log_meta != 0;
-      const uint32_t lf = GPX_F_DECISION | (metaf ? GPX_F_META : 0u) | ((efl & GPX_ENT_STOP) ? GPX_F_STOP : 0u);
-      img0 = make_int4((int)gid, slot, d.bnum, d.bcoord);
-      img1 = make_int4(metaf ? -1 : d.median_cp, (int)(lf | ((1u << l) << 16)), n1.x, n1.y);
-      gc_step(row, d.median_cp);
-      DPValue x;
-      x.slot = slot;
-      x.bnum = d.bnum;
-      x.bcoord = d.bcoord;
-      x.median_cp = d.median_cp;
-      x.req_id = ((long long)n1.y << 32) | (unsigned)n1.x;
-      x.frame_ref = st.frame_ref;
-      x.plen = (unsigned)n1.z;
-      x.fl = efl & ~GPX_ENT_VALID;
-      x.valued = true;
-      row.x = (int)((unsigned)row.x + 1u);
-      atomicAdd(&s_ctr[C_EXECUTED], 1u);
-      gpx_exec_rec er = make_exec(S, gid, l, x, false);
-      if (er.flags & GPX_F_CKPT) atomicAdd(&s_ctr[C_CKPTS_DUE], 1u);
-      store_exec(ex, er);
-      bool more = true;
-      if (efl & GPX_ENT_STOP) {
-        aux = (aux & ~0xffu) | GPX_ST_STOPPED;
-        aux &= ~0x00ffff00u;
-        atomicAdd(&s_ctr[C_STOPS_EXECUTED], 1u);
-        more = false;
-      }
-      if (S.journaling) {
-        if (st.fl & LS_OCCVALID) {
-          n1.w = (int)((unsigned)n1.w & ~GPX_ENT_VALID);
-          ST_ACC(S, l, gid, ai, n0, n1);
-        }
-      } else
-        ST_ACC(S, l, gid, ai, n0, n1);
-      st.fl &= ~LS_STORE;
-      if (more) {
-        gc_step(row, d.median_cp);
-        if ((GPX_AUX_PRESENT(aux) >> ((uint32_t)row.x & Wm)) & 1u)
-          eec(S, l, gid, row, aux, x, nullptr, A.extra, A.extra_cap, A.n_extra, s_ctr, true);
-      }
-    } else {
-      int4 a0, a1;
-      if (st.fl & LS_STORE) {
-        make_entry(q0, q1, q2, st.frame_ref, a0, a1);
-        ST_ACC(S, l, gid, ai, a0, a1);
-        st.fl &= ~LS_STORE;
-      } else
-        ld256(&S.acc_win[ai], a0, a1);
-      store_void_exec(ex, gid, slot, l);
-      commit_lane(S, l, gid, slot, d.bnum, d.bcoord, d.median_cp, row, aux, a0, a1, ex, A.extra, A.extra_cap,
-                  A.n_extra, img0, img1, s_ctr);
-    }
-    if (aux != aux_b) st.fl |= LS_AUXDIRTY;
-    if (row.x != row_b.x || row.y != row_b.y || row.z != row_b.z || row.w != row_b.w) st.fl |= LS_ROWDIRTY;
-  }
-  if (st.fl & LS_STORE) {
-    int4 n0, n1;
-    make_entry(q0, q1, q2, st.frame_ref, n0, n1);
-    ST_ACC(S, l, gid, ai, n0, n1);
-  }
-  if (st.fl & LS_ROWDIRTY) S.acc_row[ri] = row;
-  if (st.fl & LS_AUXDIRTY) S.acc_aux[ri] = aux;
-  st256_stream(ring_ptr(S, l, dseg + 64 + (unsigned long long)j * 32), img0, img1);
-}
-
 /* General path, phase 1, for the run that starts at request index i: RequestBatcher + PCS.propose by team thread 0
  * (propose_run writes the ACCEPTs at their request index, the status of every request of the run and, for batched
  * slots, where each request's table entry and body go).  Returns one past the last request of the run. */
@@ -186,24 +91,6 @@ __device__ __forceinline__ uint32_t round_propose(const DevState& S, const Round
   return k;
 }
 
-/* General path, phase 2, for ONE request q of a left-over run: its entry and body in the blob of a batched slot,
- * [nreq x gpx_batch_ent][values] (RequestPacket.batched) */
-__device__ __forceinline__ void round_build_blob(const RoundArgs& RA, uint32_t q) {
-  if (!mk_batched(RA.mark, RA.P.n, q)) return;
-  const gpx_request_rec r = RA.P.reqs[q];
-  gpx_batch_ent be;
-  be.req_id = r.req_id;
-  be.len = r.payload_len;
-  be.flags = r.flags;
-  *reinterpret_cast<int4*>(RA.blob1w + (RA.P.copy_tab[q] - RA.A.blob0_bytes)) = *reinterpret_cast<const int4*>(&be);
-  uint8_t* d = RA.blob1w + (RA.P.copy_dst[q] - RA.A.blob0_bytes);
-  const uint8_t* sp = RA.A.blob0 + r.payload_off;
-  uint32_t b = 0;
-  if ((((uint32_t)(uintptr_t)d | (uint32_t)(uintptr_t)sp) & 15u) == 0)
-    for (; b + 16 <= r.payload_len; b += 16) *reinterpret_cast<int4*>(d + b) = ld_stream4(sp + b);
-  for (; b < r.payload_len; b++) d[b] = sp[b];
-}
-
 /* General path, phase 3, for the run [i, run_end): accept at every lane, coordinator work by team thread 0 against
  * memory (tally_reply), decision broadcast to the lanes by shuffles, commit at every lane. */
 template <int L, int LP>
@@ -213,7 +100,6 @@ __device__ __forceinline__ void round_general(const DevState& S, const RoundArgs
                                               unsigned int* s_ctr) {
   const AcceptArgs& A = RA.A;
   const uint32_t n = RA.P.n;
-  const uint32_t Wm = S.W - 1;
   const GroupCtx g = group_ctx(S, gid);
   for (uint32_t q = i; q < run_end;) {
     if (!(RA.mark[q] & GPX_MK_HEAD)) break; /* refused / pre-active from here on (propose_run): no further ACCEPT in
@@ -237,13 +123,8 @@ __device__ __forceinline__ void round_general(const DevState& S, const RoundArgs
     st.rwho = GPX_WHO(0xffu, 0xffu, GPX_F_VOID);
     st.rbn = st.rbc = st.rmaxcp = 0;
     if (sub < (uint32_t)L) {
-      int4 e0 = make_int4(0, 0, 0, 0), e1 = e0;
-      if (g.live) {
-        const size_t ri = row_idx(S, sub, gid);
-        st.aux = S.acc_aux[ri];
-        st.row = S.acc_row[ri];
-        ld256(&S.acc_win[2 * win_idx(S, sub, (uint32_t)slot & Wm, gid)], e0, e1);
-      }
+      int4 e0, e1;
+      load_lane(S, sub, gid, slot, g.live, st.aux, st.row, e0, e1);
       const unsigned fr = (unsigned)(((payb + (uint32_t)q2.x) & (S.ring_cap - 1)) >> 4);
       accept_lane(S, A, sub, g.live, g.ms, dstIdx, q0, q1, q2, e0, e1, fr, st, s_ctr);
       write_accept_image(S, sub, seg, n, q, q0, q1, q2, st.img_flags);
@@ -316,7 +197,8 @@ __device__ __forceinline__ void round_general(const DevState& S, const RoundArgs
       dp[1].w = __shfl_sync(tmask, dp[1].w, tbase);
     }
     if (sub < (uint32_t)L)
-      commit_team_lane<L>(S, A, sub, gid, slot, g.live, decided_i != 0, d, q0, q1, q2, st, q, dseg, s_ctr);
+      commit_accepted_lane(S, A, sub, gid, slot, g.live, decided_i != 0, d, q0, q1, q2, st, &A.exec[(size_t)q * L + sub],
+                           dseg + 64 + (unsigned long long)q * 32, s_ctr);
     if (RA.sum) { /* compact mode: the general path reports through the extra queue */
       if (sub < (uint32_t)L) {
         const gpx_exec_rec er = A.exec[(size_t)q * L + sub];
@@ -334,6 +216,36 @@ __device__ __forceinline__ void round_general(const DevState& S, const RoundArgs
 
 template <int L, int LP>
 __global__ void k_round_slow(const __grid_constant__ DevState S, const __grid_constant__ RoundArgs RA);
+
+/* Block 0 of the fast kernels, thread t < L: lane t's two segment headers at its segment base seg, the NEXT launch's
+ * log position and the segment base left for k_round_slow; thread 0 also counts the launch and zeroes the control
+ * block the next round counts into. */
+__device__ __forceinline__ void round_open_segments(const DevState& S, const RoundArgs& RA, uint32_t t,
+                                                    unsigned long long seg, unsigned int* s_ctr) {
+  const uint32_t n = RA.P.n;
+  const unsigned long long sq = seg_seq_of(S, t);
+  write_seg_hdr(S, t, seg, GPX_F_ACCEPT, n, n, RA.pay_bytes, 48, sq);
+  write_seg_hdr(S, t, seg + RA.res_a, GPX_F_DECISION, n, n, 0, 32, sq + 1ull);
+  log_publish(S, t, seg + RA.res_a + RA.res_d, sq + 2ull);
+  S.cur_seg[t] = seg;
+  if (t == 0) {
+    atomicAdd(&s_ctr[C_KERNEL_LAUNCHES], 1u);
+    if (RA.ctl_zero) { /* the control block the next round counts into */
+      int4* z = reinterpret_cast<int4*>(RA.ctl_zero);
+      z[0] = make_int4(0, 0, 0, 0);
+      z[1] = make_int4(0, 0, 0, 0);
+    }
+  }
+}
+
+/* The run that starts at request i goes to k_round_slow; the first left-over run of the round brings that kernel in
+ * (a tail launch from the device, or the host launches it behind every round). */
+template <int L, int LP>
+__device__ __forceinline__ void round_hand_off(const DevState& S, const RoundArgs& RA, uint32_t i) {
+  const uint32_t k = atomicAdd(RA.n_todo, 1u);
+  RA.todo[k] = i;
+  if (k == 0 && RA.tail_launch) k_round_slow<L, LP><<<RA.slow_grid, GPX_BLOCK, 0, cudaStreamTailLaunch>>>(S, RA);
+}
 
 /*
  * The fast kernel.  The whole body is straight-line, predicated code: every shuffle and vote is a full-warp
@@ -386,28 +298,13 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
                                         : 0xffffffffu;
   const uint32_t G = S.G, Wm = S.W - 1;
   /* per-lane log segments of this launch: [ACCEPT seg (n images + payload area)][DECISION seg] */
-  const unsigned long long pay_bytes = RA.pay_bytes, res_a = RA.res_a, res_d = RA.res_d;
+  const unsigned long long res_a = RA.res_a, res_d = RA.res_d;
   const uint32_t pay_rel = RA.pay_rel;
   /* my lane's log position is read from the copy this launch owns (DevState.lp); block 0 writes the next launch's
    * position into the other copy and leaves the segment bases for k_round_slow -- the round needs neither a ticket
    * nor a fence nor a trailing kernel to finish */
   const unsigned long long seg = seg_base(S, sub, res_a + res_d);
-  if (blockIdx.x == 0 && threadIdx.x < (uint32_t)L) { /* thread l writes lane l's two segment headers */
-    const uint32_t t = threadIdx.x;
-    const unsigned long long sq = seg_seq_of(S, t);
-    write_seg_hdr(S, t, seg, GPX_F_ACCEPT, n, n, pay_bytes, 48, sq);
-    write_seg_hdr(S, t, seg + res_a, GPX_F_DECISION, n, n, 0, 32, sq + 1ull);
-    log_publish(S, t, seg + res_a + res_d, sq + 2ull);
-    S.cur_seg[t] = seg;
-    if (t == 0) {
-      atomicAdd(&s_ctr[C_KERNEL_LAUNCHES], 1u);
-      if (RA.ctl_zero) { /* the control block the next round counts into */
-        int4* z = reinterpret_cast<int4*>(RA.ctl_zero);
-        z[0] = make_int4(0, 0, 0, 0);
-        z[1] = make_int4(0, 0, 0, 0);
-      }
-    }
-  }
+  if (blockIdx.x == 0 && threadIdx.x < (uint32_t)L) round_open_segments(S, RA, threadIdx.x, seg, s_ctr);
 
   /* ---- level A: the request record and the neighbours' gids (run-head / single-request tests) ---- */
   const bool valid = i < n;
@@ -510,14 +407,7 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
   gc_step(row, median);   /* acceptAndUpdateBallot -> garbageCollectAccepted :320 */
   const int cpi = cf_cpi_pg ? (sf ? S.grp_cpi[gid] : 1) : S.cpi_const;
   int max_cp = row.x - 1; /* AcceptReplyPacket.maxCheckpointedSlot :1139-1143 */
-  if (!cf_gcme) {
-    int lcp = max_cp - max_cp % cpi;
-    if (lcp < 0) {
-      lcp = jsub(lcp, cpi);
-      if (lcp > 0) lcp = 2147483647 - 2147483647 % cpi;
-    }
-    max_cp = lcp;
-  }
+  if (!cf_gcme) max_cp = last_cp(max_cp, cpi);
   /* tally (handleAcceptReplyMyBallot :597-640): replies arrive in lane order, all for my ballot; the decision is
    * made by reply number L/2 (0-based) with the nodeSlots recorded up to and including it */
   int nsd[LP], mine = my_ns;
@@ -597,10 +487,7 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
       c_team = 1;
     }
   } else if (head && sub == 0) {
-    const uint32_t k = atomicAdd(RA.n_todo, 1u);
-    RA.todo[k] = i; /* the run goes to k_round_slow */
-    if (k == 0 && RA.tail_launch) /* the first left-over run of the round brings the second kernel in */
-      k_round_slow<L, LP><<<RA.slow_grid, GPX_BLOCK, 0, cudaStreamTailLaunch>>>(S, RA);
+    round_hand_off<L, LP>(S, RA, i);
   }
   { /* the staged log images of the warp's fast teams, in runs of contiguous 16 B: s_img index k is half k & 1 of the
      * image of team (k >> 1) % TPW, kind x lane (k >> 1) / TPW; the segment base of lane l comes from warp lane l */
@@ -698,27 +585,13 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
   const uint32_t lane_id = threadIdx.x & 31u, warp = threadIdx.x >> 5;
   const uint32_t i = r0 + threadIdx.x;
   const uint32_t G = S.G, Wm = S.W - 1;
-  const unsigned long long pay_bytes = RA.pay_bytes, res_a = RA.res_a, res_d = RA.res_d;
+  const unsigned long long res_a = RA.res_a, res_d = RA.res_d;
   const uint32_t pay_rel = RA.pay_rel;
   unsigned long long seg[L]; /* every lane's segment base (DevState.lp's copy of log_pos) */
 #pragma unroll
   for (int l = 0; l < L; l++) seg[l] = seg_base(S, l, res_a + res_d);
-  if (blockIdx.x == 0 && threadIdx.x < (uint32_t)L) { /* thread l writes lane l's two segment headers */
-    const uint32_t t = threadIdx.x;
-    const unsigned long long sg = seg_base(S, t, res_a + res_d), sq = seg_seq_of(S, t);
-    write_seg_hdr(S, t, sg, GPX_F_ACCEPT, n, n, pay_bytes, 48, sq);
-    write_seg_hdr(S, t, sg + res_a, GPX_F_DECISION, n, n, 0, 32, sq + 1ull);
-    log_publish(S, t, sg + res_a + res_d, sq + 2ull);
-    S.cur_seg[t] = sg;
-    if (t == 0) {
-      atomicAdd(&s_ctr[C_KERNEL_LAUNCHES], 1u);
-      if (RA.ctl_zero) {
-        int4* z = reinterpret_cast<int4*>(RA.ctl_zero);
-        z[0] = make_int4(0, 0, 0, 0);
-        z[1] = make_int4(0, 0, 0, 0);
-      }
-    }
-  }
+  if (blockIdx.x == 0 && threadIdx.x < (uint32_t)L)
+    round_open_segments(S, RA, threadIdx.x, seg_base(S, threadIdx.x, res_a + res_d), s_ctr);
 
   /* ---- level A: the request record and the neighbours' gids ---- */
   const bool valid = i < n;
@@ -830,14 +703,7 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
   const int median = median_regs<L>(ns, (uint32_t)L); /* AcceptPacket.medianCheckpointedSlot (initCommander) */
   const int cpi = cf_cpi_pg ? (sf ? S.grp_cpi[gid] : 1) : S.cpi_const;
   int max_cp = (int)((unsigned)slot - 1u); /* every lane's maxCheckpointedSlot :1139-1143 (acc_slot == slot) */
-  if (!cf_gcme) {
-    int lcp = max_cp - max_cp % cpi;
-    if (lcp < 0) {
-      lcp = jsub(lcp, cpi);
-      if (lcp > 0) lcp = 2147483647 - 2147483647 % cpi;
-    }
-    max_cp = lcp;
-  }
+  if (!cf_gcme) max_cp = last_cp(max_cp, cpi);
   /* tally: replies in lane order, the decision made by reply L/2 (recordSlotNumber :809-825, plain <) */
   int nsd[L], mine[L];
 #pragma unroll
@@ -905,10 +771,7 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
     crow.z = (int)((unsigned)crow.z + 1u); /* PCS.propose: nextProposalSlotNumber++ */
     S.coord_row[cl * G + gid] = crow;
   } else if (head) {
-    const uint32_t k = atomicAdd(RA.n_todo, 1u);
-    RA.todo[k] = i; /* the run goes to k_round_slow */
-    if (k == 0 && RA.tail_launch)
-      k_round_slow<L, L><<<RA.slow_grid, GPX_BLOCK, 0, cudaStreamTailLaunch>>>(S, RA);
+    round_hand_off<L, L>(S, RA, i);
   }
   const uint32_t sfm = __ballot_sync(FULL, sf); /* bit g: group g of the warp took the fast path */
   const uint32_t i0 = r0 + warp * 32u;         /* request of the warp's group 0 */
@@ -1047,7 +910,7 @@ __global__ void __launch_bounds__(GPX_BLOCK, 2) k_round_slow(const __grid_consta
     for (uint32_t q = blockIdx.x * GPX_BLOCK + threadIdx.x; q < n; q += gridDim.x * GPX_BLOCK) {
       const uint32_t mk = RA.mark[q];
       if (!mk) continue;
-      round_build_blob(RA, q);
+      write_blob_entry(RA.P, RA.mark, q, RA.A.blob0, RA.blob1w, RA.A.blob0_bytes);
       if (mk & GPX_MK_HEAD) continue;
       const int st = RA.P.status[q];
       const uint32_t gid = RA.P.reqs[q].gid;

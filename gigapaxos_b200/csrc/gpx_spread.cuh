@@ -238,7 +238,6 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_PHASE_MINB) k_sp_accept(const _
   const uint32_t t0 = j0 ? j0 - 1u : 0u, t1 = min(cnt, j0 + GPX_BLOCK);
   const uint32_t tile_bytes = (j0 < cnt && t1 > t0) ? (t1 - t0) * (uint32_t)sizeof(gpx_accept_rec) : 0u;
   if (threadIdx.x == 0 && tile_bytes) tma_load_1d(s_tile, &recs[t0], tile_bytes, &s_bar);
-  const uint32_t Wm = S.W - 1;
   /* one ACCEPT segment per round: an image slot per virtual index, payload area = the received blob areas */
   const unsigned long long pay_rel = 64ull + (unsigned long long)A.vtotal * 48ull;
   const unsigned long long reserved = (pay_rel + A.blob_vtotal + 31ull) & ~31ull;
@@ -279,31 +278,15 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_PHASE_MINB) k_sp_accept(const _
         const int slot = q0.y;
         const uint32_t payload_off = (uint32_t)q2.x;
         LaneSt st;
-        int4 e0 = make_int4(0, 0, 0, 0), e1 = e0;
-        st.aux = 0;
-        st.row = make_int4(0, 0, 0, 0);
-        if (g.live) {
-          const size_t ri = row_idx(S, 0, gid);
-          st.aux = S.acc_aux[ri];
-          st.row = S.acc_row[ri];
-          ld256(&S.acc_win[2 * win_idx(S, 0, (uint32_t)slot & Wm, gid)], e0, e1);
-        }
+        int4 e0, e1;
+        load_lane(S, 0, gid, slot, g.live, st.aux, st.row, e0, e1);
         uint32_t dstIdx = 0xffu;
         if (g.live)
           for (uint32_t m = 0; m < g.R; m++)
             if (g.ms->nodes[m] == q2.w) dstIdx = m;
         const unsigned fr = (unsigned)(((payb + payload_off) & (S.ring_cap - 1)) >> 4);
         accept_lane(S, AA, 0, g.live, g.ms, dstIdx, q0, q1, q2, e0, e1, fr, st, s_ctr);
-        if (g.live) {
-          const size_t ri = row_idx(S, 0, gid);
-          if (st.fl & LS_STORE) {
-            int4 n0, n1;
-            make_entry(q0, q1, q2, st.frame_ref, n0, n1);
-            ST_ACC(S, 0, gid, 2 * win_idx(S, 0, (uint32_t)slot & Wm, gid), n0, n1);
-          }
-          if (st.fl & LS_ROWDIRTY) S.acc_row[ri] = st.row;
-          if (st.fl & LS_AUXDIRTY) S.acc_aux[ri] = st.aux;
-        }
+        store_accepted_lane(S, 0, q0, q1, q2, st);
         st256_stream(&replies[jj], make_int4((int)gid, slot, st.rbn, st.rbc),
                      (GPX_WHO_FLAGS(st.rwho) & GPX_F_VOID) ? make_int4(0, (int)st.rwho, 0, 0)
                                                            : make_int4(st.rmaxcp, (int)st.rwho, q1.z, q1.w));
@@ -490,12 +473,8 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_PHASE_MINB) k_sp_commit(const _
           } else {
             int4 row = S.acc_row[ri], e0, e1;
             ld256(&S.acc_win[2 * win_idx(S, 0, (uint32_t)slot & Wm, gid)], e0, e1);
-            const int4 row_in = row;
-            const uint32_t aux_in = aux;
-            commit_lane(S, 0, gid, slot, q0.z, q0.w, q1.x, row, aux, e0, e1, ex, A.extra, A.extra_cap, A.n_extra, img0,
-                        img1, s_ctr);
-            if (aux != aux_in) S.acc_aux[ri] = aux;
-            if (row.x != row_in.x || row.y != row_in.y || row.z != row_in.z || row.w != row_in.w) S.acc_row[ri] = row;
+            commit_lane_stored(S, 0, gid, slot, q0.z, q0.w, q1.x, row, aux, e0, e1, ex, A.extra, A.extra_cap,
+                               A.n_extra, img0, img1, s_ctr);
           }
         }
         st256_stream(ring_ptr(S, 0, segb + 64 + (unsigned long long)vv * 32), img0, img1);
