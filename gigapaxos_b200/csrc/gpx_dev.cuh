@@ -11,7 +11,8 @@
  *   acc_win   2xint4[L][W][G]   accepted pvalue {slot,bnum,bcoord,frame_ref | reqID,plen,fl}  (acceptedProposals :108)
  *   com_win   2xint4[L][W][G]   committed decision {bnum,bcoord,medianCP,frame_ref | reqID,plen,fl} (committedRequests :109)
  *   coord_row int4  [L][G]      {myBallotNum, myBallotCoord, nextProposalSlotNumber, flags|outstanding<<8}
- *   node_slots i32  [L][R][G]   PaxosCoordinatorState.nodeSlotNumbers
+ *   node_slots i32  [L][R][G]   PaxosCoordinatorState.nodeSlotNumbers, when ns_u says so (ns_get / ns_set below)
+ *   ns_u      i32   [L][G]      the value all R members' nodeSlotNumbers share, or GPX_NS_MIXED
  *   prop_win  int4  [L][W][G]   proposal {slot, votes|present|stop, reqID}  (myProposals + WaitforUtility bitmask)
  *   grp_meta  u32   [G]         member-set id | R | live
  *
@@ -98,6 +99,7 @@ struct DevState {
   int4* com_win;
   int4* coord_row;
   int32_t* node_slots;
+  int32_t* ns_u; /* [L][G] compact nodeSlotNumbers (ns_get): null keeps every value in node_slots */
   int4* prop_win;
   uint32_t* grp_meta;
   int32_t* grp_cpi;
@@ -134,6 +136,71 @@ __device__ __forceinline__ size_t win_idx(const DevState& S, uint32_t l, uint32_
 }
 __device__ __forceinline__ size_t ns_idx(const DevState& S, uint32_t l, uint32_t r, uint32_t gid) {
   return ((size_t)l * S.Rcap + r) * S.G + gid;
+}
+
+/*
+ * nodeSlotNumbers of the coordinator at lane c: after an in-order round every member's entry holds the same value, so
+ * a group keeps them in compact form, ONE word ns_u[c][gid], while the entries of its R members are all equal.
+ * GPX_NS_MIXED in ns_u means they are not, and node_slots[c][0..R)[gid] holds them; any other value v means every
+ * member's entry is v and those node_slots words are stale.  Entries of member indices >= R are never read.  INT32_MIN
+ * is the marker because recordSlotNumber only raises an entry (plain <), so no in-order round produces it; a uniform
+ * INT32_MIN is simply kept in the words.  Read and write nodeSlotNumbers through these helpers only.  A DevState
+ * without ns_u (the host-compiled test builds of single kernels) keeps every value in node_slots.
+ */
+#define GPX_NS_MIXED INT32_MIN
+__device__ __forceinline__ int ns_u_get(const DevState& S, uint32_t c, uint32_t gid) {
+  return S.ns_u ? S.ns_u[row_idx(S, c, gid)] : GPX_NS_MIXED;
+}
+__device__ __forceinline__ int ns_get(const DevState& S, uint32_t c, uint32_t m, uint32_t gid) {
+  const int u = ns_u_get(S, c, gid);
+  return u != GPX_NS_MIXED ? u : S.node_slots[ns_idx(S, c, m, gid)];
+}
+/* v[m] = entry m for m < n (n <= N), pad above */
+template <int N>
+__device__ __forceinline__ void ns_load(const DevState& S, uint32_t c, uint32_t gid, uint32_t n, int (&v)[N], int pad) {
+  const int u = ns_u_get(S, c, gid);
+#pragma unroll
+  for (int m = 0; m < N; m++)
+    v[m] = (uint32_t)m >= n ? pad : u != GPX_NS_MIXED ? u : S.node_slots[ns_idx(S, c, (uint32_t)m, gid)];
+}
+/* every member's entry := v */
+__device__ __forceinline__ void ns_set_all(const DevState& S, uint32_t c, uint32_t gid, int v) {
+  if (S.ns_u && v != GPX_NS_MIXED) {
+    S.ns_u[row_idx(S, c, gid)] = v;
+    return;
+  }
+  for (uint32_t m = 0; m < S.Rcap; m++) S.node_slots[ns_idx(S, c, m, gid)] = v;
+  if (S.ns_u) S.ns_u[row_idx(S, c, gid)] = GPX_NS_MIXED;
+}
+/* member m's entry := v; a compact group is written out first (ns_settle folds it back) */
+__device__ __forceinline__ void ns_set(const DevState& S, uint32_t c, uint32_t m, uint32_t gid, int v) {
+  const int u = ns_u_get(S, c, gid);
+  if (u != GPX_NS_MIXED) {
+    if (u == v) return;
+    for (uint32_t k = 0; k < S.Rcap; k++) S.node_slots[ns_idx(S, c, k, gid)] = u;
+    S.ns_u[row_idx(S, c, gid)] = GPX_NS_MIXED;
+  }
+  S.node_slots[ns_idx(S, c, m, gid)] = v;
+}
+/* back to compact form once the R entries are equal again */
+__device__ __forceinline__ void ns_settle(const DevState& S, uint32_t c, uint32_t gid, uint32_t R) {
+  if (!S.ns_u || R == 0 || S.ns_u[row_idx(S, c, gid)] != GPX_NS_MIXED) return;
+  const int v = S.node_slots[ns_idx(S, c, 0, gid)];
+  for (uint32_t m = 1; m < R; m++)
+    if (S.node_slots[ns_idx(S, c, m, gid)] != v) return;
+  if (v != GPX_NS_MIXED) S.ns_u[row_idx(S, c, gid)] = v;
+}
+/* entries 0..R) := v[0..R), the words written out for m < n (n >= R) when they are not all equal */
+__device__ __forceinline__ void ns_put(const DevState& S, uint32_t c, uint32_t gid, uint32_t R, uint32_t n,
+                                       const int* v) {
+  bool same = R > 0;
+  for (uint32_t m = 1; m < R; m++) same = same && v[m] == v[0];
+  if (S.ns_u && same && v[0] != GPX_NS_MIXED) {
+    S.ns_u[row_idx(S, c, gid)] = v[0];
+    return;
+  }
+  for (uint32_t m = 0; m < n; m++) S.node_slots[ns_idx(S, c, m, gid)] = v[m];
+  if (S.ns_u) S.ns_u[row_idx(S, c, gid)] = GPX_NS_MIXED;
 }
 
 /* PISM :456-460: only an ACTIVE acceptor handles packets */
@@ -243,7 +310,7 @@ __device__ __forceinline__ void dump_row(const DevState& S, uint32_t lane, uint3
       r.n_members = (int)R;
       for (uint32_t m = 0; m < R; m++) {
         r.members[m] = ms->nodes[m];
-        r.node_slots[m] = ex ? S.node_slots[ns_idx(S, lane, m, gid)] : 0;
+        r.node_slots[m] = ex ? ns_get(S, lane, m, gid) : 0;
       }
     }
   }
@@ -403,8 +470,10 @@ __device__ __forceinline__ uint8_t* ring_ptr(const DevState& S, uint32_t l, unsi
   return S.ring[l] + (abs_off & (S.ring_cap - 1));
 }
 
-/* PaxosCoordinatorState.getMedianMinus :867-875 over node_slots[lane][0..R)[gid] */
+/* PaxosCoordinatorState.getMedianMinus :867-875 over nodeSlotNumbers[lane][0..R) of gid */
 __device__ __forceinline__ int median_minus(const DevState& S, uint32_t lane, uint32_t gid, uint32_t R) {
+  const int u = ns_u_get(S, lane, gid);
+  if (u != GPX_NS_MIXED) return u;
   if (R == 3) {
     int a = S.node_slots[ns_idx(S, lane, 0, gid)], b = S.node_slots[ns_idx(S, lane, 1, gid)],
         c = S.node_slots[ns_idx(S, lane, 2, gid)];

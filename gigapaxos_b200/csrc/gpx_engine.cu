@@ -247,6 +247,7 @@ int gpx_engine_create(const gpx_config* cfg, gpx_engine** out) {
   TRY(e->dalloc(&S.com_win, 2 * L * W * G));
   TRY(e->dalloc(&S.coord_row, L * G));
   TRY(e->dalloc(&S.node_slots, L * R * G));
+  TRY(e->dalloc(&S.ns_u, L * G));
   TRY(e->dalloc(&S.prop_win, L * W * G));
   TRY(e->dalloc(&S.grp_meta, G));
   TRY(e->dalloc(&S.grp_cpi, G));
@@ -276,6 +277,7 @@ int gpx_engine_create(const gpx_config* cfg, gpx_engine** out) {
     cudaMemset(S.acc_dirty, 0, L * G);
     cudaMemset(S.com_win, 0, 2 * L * W * G * sizeof(int4));
     cudaMemset(S.prop_win, 0, L * W * G * sizeof(int4));
+    cudaMemset(S.ns_u, 0, L * G * 4); /* compact, 0: what group creation writes */
   }
   for (size_t l = 0; l < GPX_MAX_LANES; l++) S.lane_node[l] = l < L ? cfg->lane_node[l] : INT32_MIN;
   S.cpi_const = cfg->checkpoint_interval;

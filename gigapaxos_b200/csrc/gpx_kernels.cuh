@@ -301,8 +301,7 @@ __global__ void __launch_bounds__(GPX_BLOCK) k_propose(const __grid_constant__ D
       aux = S.acc_aux[ri];
       Ae = S.acc_row[ri];
       Ce = S.coord_row[ri];
-#pragma unroll
-      for (int m = 0; m < 8; m++) ns[m] = (uint32_t)m < S.Rcap ? S.node_slots[ns_idx(S, entry, (uint32_t)m, rq.gid)] : 0;
+      ns_load<8>(S, entry, rq.gid, S.Rcap, ns, 0);
     }
   }
   uint32_t base = block_reserve(head ? nb : 0u, &A.ctl->n_accepts, s_scan);
@@ -617,9 +616,9 @@ __device__ __forceinline__ bool tally_reply(const DevState& S, uint32_t cl, uint
         atomicAdd(&s_ctr[C_PREEMPTED], 1u);
       }
     } else if (c == 0) { /* handleAcceptReplyMyBallot :597-640 */
-      if (accIdx < R) {  /* recordSlotNumber :809-825 (plain <) */
-        const size_t ni = ns_idx(S, cl, accIdx, gid);
-        if (S.node_slots[ni] < max_cp) S.node_slots[ni] = max_cp;
+      if (accIdx < R && ns_get(S, cl, accIdx, gid) < max_cp) { /* recordSlotNumber :809-825 (plain <) */
+        ns_set(S, cl, accIdx, gid, max_cp);
+        ns_settle(S, cl, gid, R);
       }
       int4 pe = S.prop_win[pi];
       if (((unsigned)pe.y & GPX_PV_PRESENT) && pe.x == slot) {
@@ -674,8 +673,7 @@ __device__ __forceinline__ bool tally_slot_regs(const DevState& S, uint32_t cl, 
   const size_t pi = win_idx(S, cl, (uint32_t)slot & Wm, gid);
   const int4 pe0 = S.prop_win[pi];
   int ns0[8];
-#pragma unroll
-  for (int m = 0; m < 8; m++) ns0[m] = (uint32_t)m < R ? S.node_slots[ns_idx(S, cl, (uint32_t)m, gid)] : 2147483647;
+  ns_load<8>(S, cl, gid, R, ns0, 2147483647);
   return tally_slot_core<NR>(S, cl, gid, R, ms, crow, dirty, slot, r0, r1, nrep, pe0, ns0, d, s_ctr);
 }
 
@@ -750,9 +748,10 @@ __device__ __forceinline__ bool tally_slot_core(const DevState& S, uint32_t cl, 
   }
   if (handled) atomicAdd(&s_ctr[C_REPLIES_HANDLED], handled);
   if (pe.y != pe_in.y) S.prop_win[pi] = pe;
+  bool ns_changed = false;
 #pragma unroll
-  for (int m = 0; m < 8; m++)
-    if ((uint32_t)m < R && ns[m] != ns_in[m]) S.node_slots[ns_idx(S, cl, (uint32_t)m, gid)] = ns[m];
+  for (int m = 0; m < 8; m++) ns_changed = ns_changed || ((uint32_t)m < R && ns[m] != ns_in[m]);
+  if (ns_changed) ns_put(S, cl, gid, R, R, ns);
   return decided;
 }
 
@@ -1220,8 +1219,7 @@ __global__ void __launch_bounds__(GPX_BLOCK) k_tally_slots(const __grid_constant
         int4 crow = S.coord_row[ri];
         const int4 pe0 = S.prop_win[win_idx(S, dst, (uint32_t)slot & (S.W - 1), gid)];
         int ns0[8];
-#pragma unroll
-        for (int m = 0; m < 8; m++) ns0[m] = (uint32_t)m < S.Rcap ? S.node_slots[ns_idx(S, dst, (uint32_t)m, gid)] : 0;
+        ns_load<8>(S, dst, gid, S.Rcap, ns0, 0);
         const uint32_t R = (meta >> 16) & 0xffu;
         if ((meta & (GPX_META_LIVE | GPX_META_IDENT)) == (GPX_META_LIVE | GPX_META_IDENT) && R <= 8u && st_usable(aux)) {
           bool dirty = false;
@@ -1569,7 +1567,7 @@ __global__ void k_init_groups(const __grid_constant__ DevState S, const InitRec*
     S.acc_aux[ri] = GPX_ST_ACTIVE_1;
     const bool am_coord = (r.coord0 == S.lane_node[l]);
     S.coord_row[ri] = am_coord ? make_int4(0, r.coord0, 1, (int)(GPX_CF_EXISTS | GPX_CF_ACTIVE)) : make_int4(0, 0, 0, 0);
-    for (uint32_t m = 0; m < S.Rcap; m++) S.node_slots[ns_idx(S, l, m, r.gid)] = am_coord ? (batch ? 0 : -1) : 0;
+    ns_set_all(S, l, r.gid, am_coord ? (batch ? 0 : -1) : 0);
   }
 }
 
@@ -1615,7 +1613,8 @@ __global__ void k_load_rows(const __grid_constant__ DevState S, const LoadRec* r
   if (r.coord_exists) {
     S.coord_row[ri] =
         make_int4(r.coord_bnum, r.coord_bcoord, r.next_proposal_slot, (int)(GPX_CF_EXISTS | (r.coord_active ? GPX_CF_ACTIVE : 0u)));
-    for (int m = 0; m < r.n_members && m < (int)S.Rcap; m++) S.node_slots[ns_idx(S, l, m, gid)] = r.node_slots[m];
+    const uint32_t nm = r.n_members > 0 ? min((uint32_t)r.n_members, S.Rcap) : 0u;
+    ns_put(S, l, gid, nm, nm, r.node_slots);
   } else
     S.coord_row[ri] = make_int4(0, 0, 0, 0);
 }
@@ -1658,7 +1657,7 @@ __global__ void k_patch(const __grid_constant__ DevState S, const gpx_patch_rec*
       break;
     case GPX_PATCH_INSTALL_COORD: {
       S.coord_row[ri] = make_int4(r.a, r.b, r.c, (int)(GPX_CF_EXISTS | (r.d ? GPX_CF_ACTIVE : 0u)));
-      for (uint32_t m = 0; m < S.Rcap; m++) S.node_slots[ns_idx(S, r.lane, m, r.gid)] = -1;
+      ns_set_all(S, r.lane, r.gid, -1);
       for (uint32_t w = 0; w < S.W; w++) S.prop_win[win_idx(S, r.lane, w, r.gid)] = make_int4(0, 0, 0, 0);
       break;
     }
@@ -1669,8 +1668,10 @@ __global__ void k_patch(const __grid_constant__ DevState S, const gpx_patch_rec*
     case GPX_PATCH_SET_GC: row.w = r.a; break;
     case GPX_PATCH_SET_NODE_SLOT: /* PCS.recordSlotNumber(PrepareReplyPacket) :786-807 */
       if ((((unsigned)S.coord_row[ri].w) & GPX_CF_EXISTS) && r.a >= 0 && (uint32_t)r.a < S.Rcap) {
-        const size_t ni = ns_idx(S, r.lane, (uint32_t)r.a, r.gid);
-        if (jsub(S.node_slots[ni], r.b) < 0) S.node_slots[ni] = r.b;
+        if (jsub(ns_get(S, r.lane, (uint32_t)r.a, r.gid), r.b) < 0) {
+          ns_set(S, r.lane, (uint32_t)r.a, r.gid, r.b);
+          ns_settle(S, r.lane, r.gid, (S.grp_meta[r.gid] >> 16) & 0xffu);
+        }
       }
       break;
     default: break;

@@ -195,11 +195,9 @@ __global__ void __launch_bounds__(GPX_P1B_BLOCK) k_prepare_tally(const __grid_co
         /* ... and the new one starts ACTIVE at the plan's first slot (GPX_PATCH_INSTALL_COORD + SET_NODE_SLOT x R;
          * setCoordinatorActive :577-587) */
         S.coord_row[row_idx(S, el.lane, gid)] = make_int4(bn, bc, installed, (int)(GPX_CF_EXISTS | GPX_CF_ACTIVE));
-        for (uint32_t m = 0; m < S.Rcap; m++) {
-          int v = -1;
-          if (m < R && jsub(-1, ns[m]) < 0) v = ns[m];
-          S.node_slots[ns_idx(S, el.lane, m, gid)] = v;
-        }
+        int nv[GPX_MAX_GROUP_SIZE];
+        for (uint32_t m = 0; m < S.Rcap; m++) nv[m] = m < R && jsub(-1, ns[m]) < 0 ? ns[m] : -1;
+        ns_put(S, el.lane, gid, R, S.Rcap, nv);
       }
     }
   }

@@ -327,9 +327,9 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
   /* ---- level B (depends on gid only): group meta, my lane's acceptor + coordinator rows; the first chunk of
    * the payload rides along ---- */
   uint32_t meta = 0, my_aux = 0, my_dirty = 1;
-  int ns_all[L];
+  int ns_all[L], nsu_all[L]; /* [c]: nodeSlotNumbers[c][sub], and ns_u[c] (GPX_NS_MIXED: ns_all came from node_slots) */
 #pragma unroll
-  for (int c = 0; c < L; c++) ns_all[c] = 0;
+  for (int c = 0; c < L; c++) ns_all[c] = nsu_all[c] = 0;
   int4 my_row = make_int4(0, 0, 0, 0), my_crow = my_row, pv = my_row;
   const uint32_t ri = sub * G + gid; /* 32-bit plane indices: checked against 2^32 at engine creation */
   const uint8_t* const psrc = A.blob0 + poff;
@@ -341,8 +341,10 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
     my_crow = S.coord_row[ri];
     if (cf_journaling) my_dirty = S.acc_dirty[ri]; /* 0: no accept was ever stored here -> skip the window read */
 #pragma unroll
-    for (int c = 0; c < L; c++) /* nodeSlotNumbers[c][sub] of every lane that may turn out to coordinate: 4 B each, */
-      ns_all[c] = S.node_slots[((uint32_t)c * S.Rcap + sub) * G + gid]; /* saves a whole dependent load level   */
+    for (int c = 0; c < L; c++) { /* nodeSlotNumbers[c][sub] of every lane that may turn out to coordinate: saves a */
+      nsu_all[c] = S.ns_u[(uint32_t)c * G + gid]; /* whole dependent load level while the group is compact          */
+      ns_all[c] = nsu_all[c] != GPX_NS_MIXED ? nsu_all[c] : S.node_slots[((uint32_t)c * S.Rcap + sub) * G + gid];
+    }
     if (plen) {
       if (pal)
         pv = ld_stream4(psrc);
@@ -385,14 +387,17 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
 
   /* ---- level C (depends on the slot / the coordinator lane): window entry, nodeSlotNumbers ---- */
   int4 e0 = make_int4(0, 0, 0, 0), e1 = e0;
-  int my_ns = 0;
+  int my_ns = 0, my_nsu = 0;
   const uint32_t wi = 2u * ((sub * S.W + ((uint32_t)slot & Wm)) * G + gid);
   const uint32_t ni = (cl * S.Rcap + sub) * G + gid;
   if (sf) {
     if (my_dirty) ld256(&S.acc_win[wi], e0, e1);
 #pragma unroll
     for (int c = 0; c < L; c++)
-      if (cl == (uint32_t)c) my_ns = ns_all[c];
+      if (cl == (uint32_t)c) {
+        my_ns = ns_all[c];
+        my_nsu = nsu_all[c];
+      }
   }
   { /* an accept already sitting at this slot -> general path */
     const bool ent_live = ((unsigned)e1.w & GPX_ENT_VALID) && jsub(e0.x, my_row.w) > 0 && e0.x == slot;
@@ -472,7 +477,10 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
             make_int4(rq0.z, rq0.w, (int)plen, (int)(GPX_ENT_VALID | (1u << 16))));
     gc_step(row, dmed); /* second EEC iteration: GC with the advanced slot; nothing is queued (checked above) */
     S.acc_row[ri] = row;
-    if (mine != my_ns) S.node_slots[ni] = mine; /* nodeSlotNumbers[cl][sub] */
+    if (my_nsu != GPX_NS_MIXED) { /* compact: every lane's `mine` is the same value */
+      if (sub == 0 && mine != my_nsu) S.ns_u[cl * G + gid] = mine;
+    } else if (mine != my_ns)
+      S.node_slots[ni] = mine; /* nodeSlotNumbers[cl][sub] */
     c_lane = 1;
     if (sub == 0) {
       constexpr uint32_t lane_mask = (1u << L) - 1u;
@@ -552,7 +560,7 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
  * The fast kernel with one THREAD per group: the thread owns request i and all L lanes of its group.  Same inputs,
  * load levels, in-order predicate and durable outputs as k_round; the team vote is an AND over the lanes held in
  * registers, the entry lane's and the coordinator lane's rows are register selects, and nothing is shuffled.  A warp
- * serves 32 adjacent groups, so every per-lane plane access (acc_row, acc_aux, coord_row, node_slots, the frame
+ * serves 32 adjacent groups, so every per-lane plane access (acc_row, acc_aux, coord_row, ns_u, the frame
  * records) is 32 x 4..16 B contiguous: whole lines per instruction.  The log images are staged per warp as in
  * k_round; a warp whose 32 groups all took the fast path stages its EXEC rows too and stores them as 16-byte pieces.
  */
@@ -610,18 +618,17 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
   const bool head = valid && (i == 0 || gprev != gid);
   const bool cand = head && gnext != gid && gid < G && entry < (uint32_t)L && !(rflags & GPX_F_STOP);
 
-  /* ---- level B: group meta and, for every lane, its acceptor row, aux word, coordinator row and the
-   * nodeSlotNumbers it holds for every lane that may coordinate; the first payload chunk ---- */
+  /* ---- level B: group meta and, for every lane, its acceptor row, aux word, coordinator row and the compact
+   * nodeSlotNumbers of the lane as coordinator; the first payload chunk ---- */
   uint32_t meta = 0, aux[L], dirty[L];
   int4 arow[L], crw[L];
-  int ns_all[L][L]; /* [coordinator lane c][lane l] */
+  int nsu[L]; /* ns_u[c]: the value every member's nodeSlotNumbers entry holds at coordinator lane c */
 #pragma unroll
   for (int l = 0; l < L; l++) {
     aux[l] = 0;
     dirty[l] = 1;
     arow[l] = crw[l] = make_int4(0, 0, 0, 0);
-#pragma unroll
-    for (int c = 0; c < L; c++) ns_all[c][l] = 0;
+    nsu[l] = 0;
   }
   int4 pv = make_int4(0, 0, 0, 0);
   const uint8_t* const psrc = A.blob0 + poff;
@@ -635,8 +642,7 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
       arow[l] = S.acc_row[ri];
       crw[l] = S.coord_row[ri];
       if (cf_journaling) dirty[l] = S.acc_dirty[ri];
-#pragma unroll
-      for (int c = 0; c < L; c++) ns_all[c][l] = S.node_slots[((uint32_t)c * S.Rcap + l) * G + gid];
+      nsu[l] = S.ns_u[ri];
     }
     if (plen) {
       if (pal)
@@ -665,23 +671,20 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
     cl = fl >= 0 ? (uint32_t)fl : 0u;
   }
   int4 crow = crw[0];
-  int af_y = arow[0].y, af_z = arow[0].z;
-  int ns[L];
-#pragma unroll
-  for (int l = 0; l < L; l++) ns[l] = ns_all[0][l];
+  int af_y = arow[0].y, af_z = arow[0].z, u = nsu[0];
 #pragma unroll
   for (int c = 1; c < L; c++)
     if (cl == (uint32_t)c) {
       crow = crw[c];
       af_y = arow[c].y;
       af_z = arow[c].z;
-#pragma unroll
-      for (int l = 0; l < L; l++) ns[l] = ns_all[c][l];
+      u = nsu[c];
     }
-  /* an ACTIVE coordinator whose ballot is not behind its acceptor, no proposal outstanding; every lane the plain
-   * in-order case */
+  /* an ACTIVE coordinator whose ballot is not behind its acceptor, no proposal outstanding, its nodeSlotNumbers in
+   * compact form; every lane the plain in-order case */
   const int slot = crow.z;
-  sf = sf && ((unsigned)crow.w == (GPX_CF_EXISTS | GPX_CF_ACTIVE)) && bcmp(crow.x, crow.y, af_y, af_z) >= 0;
+  sf = sf && ((unsigned)crow.w == (GPX_CF_EXISTS | GPX_CF_ACTIVE)) && bcmp(crow.x, crow.y, af_y, af_z) >= 0 &&
+       u != GPX_NS_MIXED;
 #pragma unroll
   for (int l = 0; l < L; l++)
     sf = sf && st_usable(aux[l]) && arow[l].y == crow.x && arow[l].z == crow.y && arow[l].x == slot &&
@@ -700,21 +703,16 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
       }
     }
   }
-  const int median = median_regs<L>(ns, (uint32_t)L); /* AcceptPacket.medianCheckpointedSlot (initCommander) */
+  const int median = u; /* AcceptPacket.medianCheckpointedSlot (initCommander): the median of L equal entries */
   const int cpi = cf_cpi_pg ? (sf ? S.grp_cpi[gid] : 1) : S.cpi_const;
   int max_cp = (int)((unsigned)slot - 1u); /* every lane's maxCheckpointedSlot :1139-1143 (acc_slot == slot) */
   if (!cf_gcme) max_cp = last_cp(max_cp, cpi);
-  /* tally: replies in lane order, the decision made by reply L/2 (recordSlotNumber :809-825, plain <) */
-  int nsd[L], mine[L];
-#pragma unroll
-  for (int k = 0; k < L; k++) {
-    nsd[k] = mine[k] = ns[k];
-    if (ns[k] < max_cp) {
-      if (k <= L / 2) nsd[k] = max_cp;
-      mine[k] = max_cp;
-    }
-  }
-  const int dmed = median_regs<L>(nsd, (uint32_t)L); /* makeDecision(getMajorityCommittedSlot()) :630 */
+  /* tally: replies in lane order, the decision made by reply L/2 (recordSlotNumber :809-825, plain <).  Every lane's
+   * entry moves from u to the same value `mine`: u, or max_cp when that is above u (so never GPX_NS_MIXED), and the
+   * group stays compact.  The decision sees the entries of replies 0..L/2 at `mine` and the rest at u, and the
+   * median of those is `mine` at every L */
+  const int mine = u < max_cp ? max_cp : u;
+  const int dmed = mine; /* makeDecision(getMajorityCommittedSlot()) :630 */
 
   const bool ckpt = sf && (slot % cpi) == 0;
   if (sf) {
@@ -754,8 +752,8 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
       } else
         st256(&S.acc_win[wi], make_int4(slot, crow.x, crow.y, (int)frame_ref),
               make_int4(rq0.z, rq0.w, (int)plen, (int)(GPX_ENT_VALID | (1u << 16))));
-      if (mine[l] != ns[l]) S.node_slots[(cl * S.Rcap + l) * G + gid] = mine[l]; /* nodeSlotNumbers[cl][l] */
     }
+    if (mine != u) S.ns_u[cl * G + gid] = mine; /* nodeSlotNumbers[cl][*] */
     if (plen > 1 && !pal) { /* unaligned body: byte by byte, every lane */
 #pragma unroll 1
       for (uint32_t b = 1; b < plen; b++) {
