@@ -37,6 +37,14 @@ struct WireRd {
   uint32_t len, n;
   bool ok;
 };
+__device__ __forceinline__ WireRd wr_open(const uint8_t* p, uint32_t len, bool ok) {
+  WireRd r;
+  r.p = p;
+  r.len = len;
+  r.n = 0;
+  r.ok = ok;
+  return r;
+}
 __device__ __forceinline__ bool wr_need(WireRd& r, uint32_t k) {
   if (!r.ok || k > r.len - r.n) {
     r.ok = false;
@@ -83,6 +91,18 @@ __device__ __forceinline__ bool wr_header(WireRd& r, WireHdr& h) {
   h.id_at = r.n;
   wr_skip(r, h.id_len);
   return r.ok && pp == GPX_PT_PAXOS_PACKET && h.id_len <= GPX_WIRE_MAX_ID;
+}
+#define GPX_PT_BIT(t) (1ull << (t))
+/* packet ref of the arena bytes[0..n_bytes): its reader r and header h.  GPX_WS_UNHANDLED for a JSON packet or a type
+ * outside `types` (GPX_PT_BIT of each), GPX_WS_MALFORMED for a span past the arena or a bad header, else GPX_WS_OK with
+ * r just past the header */
+__device__ __forceinline__ int32_t wr_packet(const uint8_t* bytes, uint64_t n_bytes, const gpx_wire_ref& ref,
+                                             uint64_t types, WireRd& r, WireHdr& h) {
+  r = wr_open(bytes + ref.off, ref.len, (uint64_t)ref.off + ref.len <= n_bytes);
+  if (r.ok && ref.len > 0 && r.p[0] == '{') return GPX_WS_UNHANDLED; /* JSON packet */
+  if (!wr_header(r, h)) return GPX_WS_MALFORMED;
+  if ((uint32_t)h.type >= 64u || !(types & GPX_PT_BIT(h.type))) return GPX_WS_UNHANDLED;
+  return GPX_WS_OK;
 }
 
 /* RequestPacket(ByteBuffer) :956-1024 up to the batched requests: the fields the engine keeps */
@@ -134,6 +154,50 @@ __device__ __forceinline__ void wr_request_body(WireRd& r, WireReq& q, WireReqMo
   }
   q.n_batched = wr_i32(r);
   if (q.n_batched < 0) r.ok = false;
+}
+
+/* the next latched request {int length}{REQUEST packet} (:929-936) at r.n: its reader s and body sq.  False (r.ok
+ * false) when it does not fit in r, or is not a whole REQUEST packet without latched requests of its own
+ * (RequestBatcher latches one level). */
+__device__ __forceinline__ bool wr_latched(WireRd& r, WireRd& s, WireReq& sq, WireReqMore* sx) {
+  const int32_t l = wr_i32(r);
+  if (l < 0 || !wr_need(r, (uint32_t)l)) {
+    r.ok = false;
+    return false;
+  }
+  s = wr_open(r.p + r.n, (uint32_t)l, true);
+  WireHdr sh;
+  const bool hok = wr_header(s, sh);
+  wr_request_body(s, sq, sx);
+  if (!hok || !s.ok || sq.n_batched != 0 || s.n != s.len) r.ok = false;
+  r.n += (uint32_t)l;
+  return r.ok;
+}
+/* a request body and its latched requests, as AcceptPacket and RequestPacket carry them */
+struct WireBatch {
+  uint32_t sub_at, n_sub; /* where the latched requests start in r, and how many there are */
+  uint32_t val, pay;      /* all value bytes, and the same with each value padded to 16 */
+  uint32_t stop;          /* one of the requests is a STOP */
+  bool host_only;         /* with x: one carries a digest or a responseValue */
+};
+__device__ __forceinline__ void wr_request_batch(WireRd& r, WireReq& q, WireReqMore* x, WireBatch& B) {
+  wr_request_body(r, q, x);
+  B.sub_at = r.n;
+  B.n_sub = r.ok ? (uint32_t)q.n_batched : 0u;
+  B.val = q.val_len;
+  B.pay = (q.val_len + 15u) & ~15u;
+  B.stop = q.stop;
+  B.host_only = x && (x->digest_len != 0 || x->resp_len != 0);
+  for (uint32_t b = 0; b < B.n_sub && r.ok; b++) {
+    WireRd s;
+    WireReq sq;
+    WireReqMore sx;
+    if (!wr_latched(r, s, sq, x ? &sx : nullptr)) break;
+    B.val += sq.val_len;
+    B.pay += (sq.val_len + 15u) & ~15u;
+    B.stop |= sq.stop;
+    B.host_only = B.host_only || (x && (sx.digest_len != 0 || sx.resp_len != 0));
+  }
 }
 
 __device__ __forceinline__ void wire_copy(uint8_t* d, const uint8_t* s, uint32_t n) {
@@ -265,6 +329,48 @@ __device__ __forceinline__ uint32_t wire_entry_bits(const DevState& S, int32_t e
     if (S.lane_node[l] == entry) return l << 8;
   return 0xfu << 8;
 }
+/* gid (wire_name_find's, GPX_NAME_NONE included) as a packet's group at the packet's version: GPX_WS_UNKNOWN_NAME
+ * without a live gid, GPX_WS_VERSION at another version (PISM :441-447), else GPX_WS_OK with its context in g */
+__device__ __forceinline__ int32_t wire_group(const DevState& S, const WireNames& W, uint32_t gid, int32_t version,
+                                              GroupCtx& g) {
+  g = group_ctx(S, gid);
+  if (gid == GPX_NAME_NONE || !g.live) return GPX_WS_UNKNOWN_NAME;
+  if (W.version[gid] != version) return GPX_WS_VERSION;
+  return GPX_WS_OK;
+}
+/* a request's receiving node: the lane serving it, which must also be a member of g (else GPX_WS_NOT_LOCAL) */
+__device__ __forceinline__ int32_t wire_recv_lane(const DevState& S, const GroupCtx& g, int32_t node, uint32_t& lane) {
+  lane = S.L;
+  for (uint32_t l = 0; l < S.L; l++)
+    if (S.lane_node[l] == node) lane = l;
+  return lane == S.L || wire_member_idx(g.ms, g.R, node) == 0xffu ? GPX_WS_NOT_LOCAL : GPX_WS_OK;
+}
+/* the records a BatchedAcceptReply / BatchedCommit gives per slot, but the slot (and a reply's requestID) */
+__device__ __forceinline__ gpx_accept_reply_rec wire_reply_rec(uint32_t gid, int32_t bnum, int32_t bcoord,
+                                                               int32_t max_cp, uint32_t who) {
+  gpx_accept_reply_rec x;
+  x.gid = gid;
+  x.slot = 0;
+  x.bnum = bnum;
+  x.bcoord = bcoord;
+  x.max_cp = max_cp;
+  x.who = who;
+  x.req_id = 0;
+  return x;
+}
+__device__ __forceinline__ gpx_decision_rec wire_decision_rec(uint32_t gid, int32_t bnum, int32_t bcoord,
+                                                              int32_t median, uint16_t dst_mask) {
+  gpx_decision_rec d;
+  d.gid = gid;
+  d.slot = 0;
+  d.bnum = bnum;
+  d.bcoord = bcoord;
+  d.median_cp = median;
+  d.flags = GPX_F_DECISION;
+  d.dst_mask = dst_mask;
+  d.req_id = 0; /* a BatchedCommit carries slots only: the value is the accept the acceptor holds */
+  return d;
+}
 
 /* one thread per packet.  Pass 0 (emit == 0) parses and validates the packet, looks its name up and writes its status
  * and output sizes; pass 1 parses it again and writes its records at the scanned offsets. */
@@ -275,55 +381,20 @@ __global__ void k_wire_decode(const __grid_constant__ DevState S, const __grid_c
   if (A.emit && A.status[k] != GPX_WS_OK) return;
   const gpx_wire_ref ref = A.pkts[k];
   uint32_t c[WD_NCNT] = {0, 0, 0, 0};
-  int32_t st = GPX_WS_OK;
   WireRd r;
-  r.p = A.bytes + ref.off;
-  r.len = ref.len;
-  r.n = 0;
-  r.ok = (uint64_t)ref.off + ref.len <= A.n_bytes;
   WireHdr h;
-  uint32_t gid = GPX_NAME_NONE, R = 0;
-  const MsetInfo* ms = nullptr;
-  if (r.ok && ref.len > 0 && r.p[0] == '{') {
-    st = GPX_WS_UNHANDLED; /* JSON packet */
-  } else if (!wr_header(r, h)) {
-    st = GPX_WS_MALFORMED;
-  } else if (h.type != GPX_PT_ACCEPT && h.type != GPX_PT_BATCHED_ACCEPT_REPLY && h.type != GPX_PT_BATCHED_COMMIT) {
-    st = GPX_WS_UNHANDLED;
-  }
+  int32_t st = wr_packet(A.bytes, A.n_bytes, ref,
+                         GPX_PT_BIT(GPX_PT_ACCEPT) | GPX_PT_BIT(GPX_PT_BATCHED_ACCEPT_REPLY) |
+                             GPX_PT_BIT(GPX_PT_BATCHED_COMMIT),
+                         r, h);
   /* body: parsed in full before anything is looked up, so a malformed packet is malformed whatever its name */
   WireReq q;
-  uint32_t sub_at = 0, n_sub = 0, val_total = 0, stop_any = 0;
+  WireBatch B = {};
   int32_t slot = 0, bnum = 0, bcoord = 0, median = 0, sender = 0, acceptor = 0, max_cp = 0, cnt_slots = 0, n_group = 0;
   uint32_t slots_at = 0;
   if (st == GPX_WS_OK) {
     if (h.type == GPX_PT_ACCEPT) { /* AcceptPacket :95-138 */
-      wr_request_body(r, q);
-      sub_at = r.n;
-      n_sub = r.ok ? (uint32_t)q.n_batched : 0u;
-      val_total = q.val_len;
-      stop_any = q.stop;
-      for (uint32_t b = 0; b < n_sub && r.ok; b++) { /* {int length}{REQUEST packet} :929-936 */
-        const int32_t l = wr_i32(r);
-        if (l < 0 || !wr_need(r, (uint32_t)l)) {
-          r.ok = false;
-          break;
-        }
-        WireRd s;
-        s.p = r.p + r.n;
-        s.len = (uint32_t)l;
-        s.n = 0;
-        s.ok = true;
-        WireHdr sh;
-        WireReq sq;
-        const bool hok = wr_header(s, sh);
-        wr_request_body(s, sq);
-        /* a latched request carries no latched requests of its own (RequestBatcher latches one level) */
-        if (!hok || !s.ok || sq.n_batched != 0 || s.n != s.len) r.ok = false;
-        val_total += sq.val_len;
-        stop_any |= sq.stop;
-        r.n += (uint32_t)l;
-      }
+      wr_request_batch(r, q, nullptr, B);
       slot = wr_i32(r);
       bnum = wr_i32(r);
       bcoord = wr_i32(r);
@@ -356,32 +427,28 @@ __global__ void k_wire_decode(const __grid_constant__ DevState S, const __grid_c
     }
     if (!r.ok || r.n != r.len) st = GPX_WS_MALFORMED;
   }
+  uint32_t gid = GPX_NAME_NONE;
+  GroupCtx g;
   uint8_t acc_idx = 0xffu, dst_idx = 0xffu;
   if (st == GPX_WS_OK) {
     gid = wire_name_find(W, r.p + h.id_at, h.id_len);
-    const GroupCtx g = group_ctx(S, gid);
-    if (gid == GPX_NAME_NONE || !g.live) {
-      st = GPX_WS_UNKNOWN_NAME;
-    } else if (W.version[gid] != h.version) {
-      st = GPX_WS_VERSION; /* PISM :441-447 */
-    } else {
-      ms = g.ms;
-      R = g.R;
-      if (h.type == GPX_PT_BATCHED_ACCEPT_REPLY) {
-        acc_idx = wire_member_idx(ms, R, acceptor);
-        dst_idx = wire_member_idx(ms, R, bcoord);
-        if (acc_idx == 0xffu || dst_idx == 0xffu) st = GPX_WS_MALFORMED; /* acceptor / coordinator not a member */
-        else if (ms->lane_of_idx[dst_idx] == 0xffu) st = GPX_WS_NOT_LOCAL;
-      } else if (ms->lane_mask == 0) {
-        st = GPX_WS_NOT_LOCAL;
-      }
+    st = wire_group(S, W, gid, h.version, g);
+  }
+  if (st == GPX_WS_OK) {
+    if (h.type == GPX_PT_BATCHED_ACCEPT_REPLY) {
+      acc_idx = wire_member_idx(g.ms, g.R, acceptor);
+      dst_idx = wire_member_idx(g.ms, g.R, bcoord);
+      if (acc_idx == 0xffu || dst_idx == 0xffu) st = GPX_WS_MALFORMED; /* acceptor / coordinator not a member */
+      else if (g.ms->lane_of_idx[dst_idx] == 0xffu) st = GPX_WS_NOT_LOCAL;
+    } else if (g.ms->lane_mask == 0) {
+      st = GPX_WS_NOT_LOCAL;
     }
   }
   if (st == GPX_WS_OK) {
     if (h.type == GPX_PT_ACCEPT) {
       c[WD_ACC] = 1;
-      const uint32_t nreq = 1u + n_sub;
-      c[WD_BLOB] = ((nreq > 1 ? 16u * nreq : 0u) + val_total + 15u) & ~15u;
+      const uint32_t nreq = 1u + B.n_sub;
+      c[WD_BLOB] = ((nreq > 1 ? 16u * nreq : 0u) + B.val + 15u) & ~15u;
     } else if (h.type == GPX_PT_BATCHED_ACCEPT_REPLY) {
       c[WD_REP] = (uint32_t)cnt_slots;
     } else {
@@ -395,7 +462,7 @@ __global__ void k_wire_decode(const __grid_constant__ DevState S, const __grid_c
   }
   if (h.type == GPX_PT_ACCEPT) {
     const uint32_t o = A.off[(size_t)WD_ACC * A.n + k], bo = A.off[(size_t)WD_BLOB * A.n + k];
-    const uint32_t nreq = 1u + n_sub;
+    const uint32_t nreq = 1u + B.n_sub;
     uint8_t* blob = A.blob + bo;
     if (nreq == 1) {
       wire_copy(blob, r.p + q.val_at, q.val_len);
@@ -408,32 +475,20 @@ __global__ void k_wire_decode(const __grid_constant__ DevState S, const __grid_c
       wire_copy(blob, reinterpret_cast<const uint8_t*>(&be), 16);
       wire_copy(blob + vo, r.p + q.val_at, q.val_len);
       vo += q.val_len;
-      WireRd rr;
-      rr.p = r.p;
-      rr.len = r.len;
-      rr.n = sub_at;
-      rr.ok = true;
-      for (uint32_t b = 0; b < n_sub; b++) {
-        const int32_t l = wr_i32(rr);
+      WireRd rr = wr_open(r.p + B.sub_at, r.len - B.sub_at, true);
+      for (uint32_t b = 0; b < B.n_sub; b++) {
         WireRd s;
-        s.p = rr.p + rr.n;
-        s.len = (uint32_t)l;
-        s.n = 0;
-        s.ok = true;
-        WireHdr sh;
         WireReq sq;
-        wr_header(s, sh);
-        wr_request_body(s, sq);
+        wr_latched(rr, s, sq, nullptr);
         be.req_id = sq.req_id;
         be.len = sq.val_len;
         be.flags = (sq.stop ? GPX_F_STOP : 0u) | wire_entry_bits(S, sq.entry);
         wire_copy(blob + 16u * (1u + b), reinterpret_cast<const uint8_t*>(&be), 16);
         wire_copy(blob + vo, s.p + sq.val_at, sq.val_len);
         vo += sq.val_len;
-        rr.n += (uint32_t)l;
       }
     }
-    const uint32_t used = (nreq > 1 ? 16u * nreq : 0u) + val_total;
+    const uint32_t used = (nreq > 1 ? 16u * nreq : 0u) + B.val;
     for (uint32_t b = used; b < c[WD_BLOB]; b++) blob[b] = 0;
     gpx_accept_rec a;
     a.h.gid = gid;
@@ -441,8 +496,8 @@ __global__ void k_wire_decode(const __grid_constant__ DevState S, const __grid_c
     a.h.bnum = bnum;
     a.h.bcoord = bcoord;
     a.h.median_cp = median;
-    a.h.flags = (uint16_t)(GPX_F_ACCEPT | (stop_any ? GPX_F_STOP : 0u));
-    a.h.dst_mask = ms->lane_mask;
+    a.h.flags = (uint16_t)(GPX_F_ACCEPT | (B.stop ? GPX_F_STOP : 0u));
+    a.h.dst_mask = g.ms->lane_mask;
     a.h.req_id = q.req_id;
     a.payload_off = bo;
     a.payload_len = used;
@@ -452,40 +507,20 @@ __global__ void k_wire_decode(const __grid_constant__ DevState S, const __grid_c
     A.acc_key[o] = gid;
   } else if (h.type == GPX_PT_BATCHED_ACCEPT_REPLY) {
     const uint32_t o = A.off[(size_t)WD_REP * A.n + k];
-    WireRd s;
-    s.p = r.p;
-    s.len = r.len;
-    s.n = slots_at;
-    s.ok = true;
+    WireRd s = wr_open(r.p + slots_at, r.len - slots_at, true);
+    gpx_accept_reply_rec x = wire_reply_rec(gid, bnum, bcoord, max_cp, GPX_WHO(acc_idx, dst_idx, 0u));
     for (uint32_t j = 0; j < (uint32_t)cnt_slots; j++) {
-      gpx_accept_reply_rec x;
-      x.gid = gid;
       x.slot = wr_i32(s);
-      x.bnum = bnum;
-      x.bcoord = bcoord;
-      x.max_cp = max_cp;
-      x.who = GPX_WHO(acc_idx, dst_idx, 0u);
       x.req_id = wr_i64(s);
       A.rep[o + j] = x;
       A.rep_key[o + j] = gid;
     }
   } else {
     const uint32_t o = A.off[(size_t)WD_DEC * A.n + k];
-    WireRd s;
-    s.p = r.p;
-    s.len = r.len;
-    s.n = slots_at;
-    s.ok = true;
+    WireRd s = wr_open(r.p + slots_at, r.len - slots_at, true);
+    gpx_decision_rec d = wire_decision_rec(gid, bnum, bcoord, median, g.ms->lane_mask);
     for (uint32_t j = 0; j < (uint32_t)cnt_slots; j++) {
-      gpx_decision_rec d;
-      d.gid = gid;
       d.slot = wr_i32(s);
-      d.bnum = bnum;
-      d.bcoord = bcoord;
-      d.median_cp = median;
-      d.flags = GPX_F_DECISION;
-      d.dst_mask = ms->lane_mask;
-      d.req_id = 0; /* a BatchedCommit carries slots only: the value is the accept the acceptor holds */
       A.dec[o + j] = d;
       A.dec_key[o + j] = gid;
     }
@@ -512,32 +547,39 @@ struct WireReqDecodeArgs {
   int emit;
 };
 
-/* one request of a REQUEST packet at staged position o, its value at payload offset *po (advanced) */
-__device__ __forceinline__ void wire_put_request(const WireReqDecodeArgs& A, uint32_t o, uint32_t* po, uint32_t gid,
-                                                 uint32_t k, int32_t node, uint32_t lane, const WireRd& r,
-                                                 const WireReq& q, const WireReqMore& x) {
+/* where a packet's requests go: staged position o and payload offset po, both advanced per request, and what the
+ * packet's requests share (their gid, client handle, receiving node and the lane serving it) */
+struct WireReqTo {
+  uint32_t o, po, gid, client, lane;
+  int32_t node;
+};
+/* one request: its record, meta and sort key at t.o, and the zero padding of its value to 16 bytes.  Returns where the
+ * caller writes the val_len value bytes.  Args: WireReqDecodeArgs, or the JSON decoder's WireJsonReqArgs. */
+template <typename Args>
+__device__ __forceinline__ uint8_t* wire_put_request(const Args& A, WireReqTo& t, int64_t req_id, bool stop,
+                                                     int32_t entry, uint32_t val_len, gpx_wire_req_meta m) {
   gpx_request_rec rq;
-  rq.gid = gid;
-  rq.flags = (q.stop ? GPX_F_STOP : 0u) | (lane << 8);
-  rq.req_id = q.req_id;
-  rq.payload_off = *po;
-  rq.payload_len = q.val_len;
-  gpx_wire_req_meta m = x.m;
-  if (q.entry == -1) { /* IntegerMap.NULL_INT_NODE: setEntryReplica :393-403 with the call's clock */
-    rq.entry_node = node;
+  rq.gid = t.gid;
+  rq.flags = (stop ? GPX_F_STOP : 0u) | (t.lane << 8);
+  rq.req_id = req_id;
+  rq.payload_off = t.po;
+  rq.payload_len = val_len;
+  if (entry == -1) { /* IntegerMap.NULL_INT_NODE: setEntryReplica :393-403 with the call's clock */
+    rq.entry_node = t.node;
     m.entry_time = A.now_ms;
   } else {
-    rq.entry_node = q.entry;
+    rq.entry_node = entry;
   }
-  rq.client = k;
-  A.req[o] = rq;
-  A.meta[o] = m;
-  A.key[o] = gid;
-  uint8_t* d = A.payload + *po;
-  wire_copy(d, r.p + q.val_at, q.val_len);
-  const uint32_t padded = (q.val_len + 15u) & ~15u;
-  for (uint32_t b = q.val_len; b < padded; b++) d[b] = 0;
-  *po += padded;
+  rq.client = t.client;
+  A.req[t.o] = rq;
+  A.meta[t.o] = m;
+  A.key[t.o] = t.gid;
+  t.o++;
+  uint8_t* d = A.payload + t.po;
+  const uint32_t padded = (val_len + 15u) & ~15u;
+  for (uint32_t b = val_len; b < padded; b++) d[b] = 0;
+  t.po += padded;
+  return d;
 }
 
 /* one thread per packet.  Pass 0 (emit == 0) parses and validates the packet (the request part of k_wire_decode's
@@ -549,97 +591,39 @@ __global__ void k_wire_req_decode(const __grid_constant__ DevState S, const __gr
   if (k >= A.n) return;
   if (A.emit && A.status[k] != GPX_WS_OK) return;
   const gpx_wire_ref ref = A.pkts[k];
-  int32_t st = GPX_WS_OK;
   WireRd r;
-  r.p = A.bytes + ref.off;
-  r.len = ref.len;
-  r.n = 0;
-  r.ok = (uint64_t)ref.off + ref.len <= A.n_bytes;
   WireHdr h;
-  if (r.ok && ref.len > 0 && r.p[0] == '{') {
-    st = GPX_WS_UNHANDLED; /* JSON packet */
-  } else if (!wr_header(r, h)) {
-    st = GPX_WS_MALFORMED;
-  } else if (h.type != GPX_PT_REQUEST) {
-    st = GPX_WS_UNHANDLED;
-  }
+  int32_t st = wr_packet(A.bytes, A.n_bytes, ref, GPX_PT_BIT(GPX_PT_REQUEST), r, h);
   WireReq q;
   WireReqMore x;
-  uint32_t sub_at = 0, n_sub = 0, pay = 0;
-  bool host_only = false;
+  WireBatch B = {};
   if (st == GPX_WS_OK) {
-    wr_request_body(r, q, &x);
-    sub_at = r.n;
-    n_sub = r.ok ? (uint32_t)q.n_batched : 0u;
-    pay = (q.val_len + 15u) & ~15u;
-    host_only = x.digest_len != 0 || x.resp_len != 0;
-    for (uint32_t b = 0; b < n_sub && r.ok; b++) { /* {int length}{REQUEST packet} :929-936 */
-      const int32_t l = wr_i32(r);
-      if (l < 0 || !wr_need(r, (uint32_t)l)) {
-        r.ok = false;
-        break;
-      }
-      WireRd s;
-      s.p = r.p + r.n;
-      s.len = (uint32_t)l;
-      s.n = 0;
-      s.ok = true;
-      WireHdr sh;
-      WireReq sq;
-      WireReqMore sx;
-      const bool hok = wr_header(s, sh);
-      wr_request_body(s, sq, &sx);
-      /* a latched request carries no latched requests of its own (RequestBatcher latches one level) */
-      if (!hok || !s.ok || sq.n_batched != 0 || s.n != s.len) r.ok = false;
-      pay += (sq.val_len + 15u) & ~15u;
-      host_only = host_only || sx.digest_len != 0 || sx.resp_len != 0;
-      r.n += (uint32_t)l;
-    }
+    wr_request_batch(r, q, &x, B);
     if (!r.ok || r.n != r.len) st = GPX_WS_MALFORMED;
-    else if (host_only) st = GPX_WS_UNHANDLED; /* digest mode / a response: the host's */
+    else if (B.host_only) st = GPX_WS_UNHANDLED; /* digest mode / a response: the host's */
   }
   uint32_t gid = GPX_NAME_NONE, lane = 0;
+  GroupCtx g;
   if (st == GPX_WS_OK) {
     gid = wire_name_find(W, r.p + h.id_at, h.id_len);
-    const GroupCtx g = group_ctx(S, gid);
-    if (gid == GPX_NAME_NONE || !g.live) {
-      st = GPX_WS_UNKNOWN_NAME;
-    } else if (W.version[gid] != h.version) {
-      st = GPX_WS_VERSION; /* PISM :441-447 */
-    } else {
-      lane = S.L;
-      for (uint32_t l = 0; l < S.L; l++)
-        if (S.lane_node[l] == ref.node) lane = l;
-      if (lane == S.L || wire_member_idx(g.ms, g.R, ref.node) == 0xffu) st = GPX_WS_NOT_LOCAL;
-    }
+    st = wire_group(S, W, gid, h.version, g);
   }
+  if (st == GPX_WS_OK) st = wire_recv_lane(S, g, ref.node, lane);
   if (!A.emit) {
     A.status[k] = st;
-    A.cnt[k] = st == GPX_WS_OK ? 1u + n_sub : 0u;
-    A.cnt[A.n + k] = st == GPX_WS_OK ? pay : 0u;
+    A.cnt[k] = st == GPX_WS_OK ? 1u + B.n_sub : 0u;
+    A.cnt[A.n + k] = st == GPX_WS_OK ? B.pay : 0u;
     return;
   }
-  uint32_t o = A.off[k], po = A.off[A.n + k];
-  wire_put_request(A, o++, &po, gid, k, ref.node, lane, r, q, x);
-  WireRd rr;
-  rr.p = r.p;
-  rr.len = r.len;
-  rr.n = sub_at;
-  rr.ok = true;
-  for (uint32_t b = 0; b < n_sub; b++) {
-    const int32_t l = wr_i32(rr);
+  WireReqTo t = {A.off[k], A.off[A.n + k], gid, k, lane, ref.node};
+  wire_copy(wire_put_request(A, t, q.req_id, q.stop, q.entry, q.val_len, x.m), r.p + q.val_at, q.val_len);
+  WireRd rr = wr_open(r.p + B.sub_at, r.len - B.sub_at, true);
+  for (uint32_t b = 0; b < B.n_sub; b++) {
     WireRd s;
-    s.p = rr.p + rr.n;
-    s.len = (uint32_t)l;
-    s.n = 0;
-    s.ok = true;
-    WireHdr sh;
     WireReq sq;
     WireReqMore sx;
-    wr_header(s, sh);
-    wr_request_body(s, sq, &sx);
-    wire_put_request(A, o++, &po, gid, k, ref.node, lane, s, sq, sx);
-    rr.n += (uint32_t)l;
+    wr_latched(rr, s, sq, &sx);
+    wire_copy(wire_put_request(A, t, sq.req_id, sq.stop, sq.entry, sq.val_len, sx.m), s.p + sq.val_at, sq.val_len);
   }
 }
 
@@ -695,6 +679,15 @@ __global__ void k_wire_enc_keys_replies(const __grid_constant__ DevState S, cons
   A.rstatus[i] = st;
   A.key[i] = st == GPX_WE_SENT ? lane * S.G + x.gid : GPX_WIRE_NOKEY;
 }
+/* a decision or an ACCEPT for every member: GPX_WE_VOID (a void record, or its group is gone), GPX_WE_LOCAL (every
+ * member is a local lane), GPX_WE_NO_NAME, else GPX_WE_SENT */
+__device__ __forceinline__ uint8_t wire_enc_status(const DevState& S, const WireNames& W, uint32_t gid, bool void_rec) {
+  const GroupCtx g = group_ctx(S, gid);
+  if (void_rec || !g.live) return GPX_WE_VOID;
+  if (wire_popc(g.ms->lane_mask) >= g.R) return GPX_WE_LOCAL;
+  if (W.slot == nullptr || W.slot[gid] == GPX_NAME_NONE) return GPX_WE_NO_NAME;
+  return GPX_WE_SENT;
+}
 __global__ void k_wire_enc_keys_decisions(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
                                           const __grid_constant__ WireEncodeArgs A) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -704,11 +697,7 @@ __global__ void k_wire_enc_keys_decisions(const __grid_constant__ DevState S, co
     return;
   }
   const gpx_decision_rec d = reinterpret_cast<const gpx_decision_rec*>(A.recs)[i];
-  uint8_t st = GPX_WE_SENT;
-  const GroupCtx g = group_ctx(S, d.gid);
-  if ((d.flags & GPX_F_VOID) || !g.live) st = GPX_WE_VOID;
-  else if (wire_popc(g.ms->lane_mask) >= g.R) st = GPX_WE_LOCAL; /* every member is a local lane */
-  else if (W.slot == nullptr || W.slot[d.gid] == GPX_NAME_NONE) st = GPX_WE_NO_NAME;
+  const uint8_t st = wire_enc_status(S, W, d.gid, d.flags & GPX_F_VOID);
   A.rstatus[i] = st;
   A.key[i] = st == GPX_WE_SENT ? d.gid : GPX_WIRE_NOKEY;
 }
@@ -833,6 +822,22 @@ __global__ void k_wire_enc_replies(const __grid_constant__ DevState S, const __g
   A.refs[A.off[A.n + p]] = r;
 }
 
+/* the packet of sorted position p (len bytes at A.off[p]) indexed once per member node of g that no local lane serves,
+ * from index A.off[A.n + p] on; pass 0 counts g.R - wire_popc(g.ms->lane_mask) of them */
+__device__ __forceinline__ void wire_refs_remote(const WireEncodeArgs& A, uint32_t p, const GroupCtx& g, uint32_t gid,
+                                                 uint32_t len) {
+  uint32_t ri = A.off[A.n + p];
+  for (uint32_t m = 0; m < g.R; m++) {
+    if (g.ms->lane_of_idx[m] != 0xffu) continue;
+    gpx_wire_ref r;
+    r.off = A.off[p];
+    r.len = len;
+    r.gid = gid;
+    r.node = g.ms->nodes[m];
+    A.refs[ri++] = r;
+  }
+}
+
 /* one thread per sorted position; a position that starts a (gid, ballot) run writes one BatchedCommit
  * (PaxosPacketBatcher.fuseBatchedCommits :389-417, BatchedCommit.addCommit :113-121: medianCheckpointedSlot is the
  * wrap-aware maximum, gpx_wire_fuse_commits' rule), stored once and indexed once per member node that no local lane
@@ -876,16 +881,7 @@ __global__ void k_wire_enc_decisions(const __grid_constant__ DevState S, const _
   ww_i32(o + b, (int32_t)g.R);
   b += 4;
   for (uint32_t m = 0; m < g.R; m++, b += 4) ww_i32(o + b, g.ms->nodes[m]);
-  uint32_t ri = A.off[A.n + p];
-  for (uint32_t m = 0; m < g.R; m++) {
-    if (g.ms->lane_of_idx[m] != 0xffu) continue;
-    gpx_wire_ref r;
-    r.off = A.off[p];
-    r.len = b;
-    r.gid = d.gid;
-    r.node = g.ms->nodes[m];
-    A.refs[ri++] = r;
-  }
+  wire_refs_remote(A, p, g, d.gid, b);
 }
 
 /* ---- ACCEPTs -> AcceptPacket bytes (gpx_wire_encode_accepts_device) --------------------------------------------------- */
@@ -907,15 +903,8 @@ __global__ void k_wire_enc_keys_accepts(const __grid_constant__ DevState S, cons
     return;
   }
   const gpx_accept_rec a = reinterpret_cast<const gpx_accept_rec*>(A.recs)[i];
-  uint8_t st = GPX_WE_SENT;
-  const GroupCtx g = group_ctx(S, a.h.gid);
-  if ((a.h.flags & GPX_F_VOID) || !g.live) {
-    st = GPX_WE_VOID;
-  } else if (wire_popc(g.ms->lane_mask) >= g.R) {
-    st = GPX_WE_LOCAL; /* every member is a local lane */
-  } else if (W.slot == nullptr || W.slot[a.h.gid] == GPX_NAME_NONE) {
-    st = GPX_WE_NO_NAME;
-  } else {
+  uint8_t st = wire_enc_status(S, W, a.h.gid, a.h.flags & GPX_F_VOID);
+  if (st == GPX_WE_SENT) {
     const uint32_t q = X.head[i];
     if (a.nreq == 0 || q >= X.n_reqs || a.nreq > X.n_reqs - q || X.reqs[q].gid != a.h.gid) st = GPX_WE_BAD_HEAD;
   }
@@ -953,9 +942,25 @@ __device__ __forceinline__ uint32_t ww_request(uint8_t* p, int32_t type, const W
   ww_i32(p + b + 4, (int32_t)n_batched);
   return b + 8;
 }
-/* bytes of one RequestPacket without batched requests: header, 55 fixed bytes, the value */
-__device__ __forceinline__ uint32_t wire_request_bytes(const WireNames& W, uint32_t gid, uint32_t val_len) {
-  return 13u + W.name[(size_t)gid * GPX_NAME_BYTES] + 55u + val_len;
+/* requests q0 .. q0 + n - 1 as one packet: the first of type `type`, the others its latched REQUESTs
+ * ({int length}{REQUEST packet} :929-936); returns the bytes written */
+__device__ __forceinline__ uint32_t ww_requests(uint8_t* p, int32_t type, const WireNames& W, uint32_t gid,
+                                                const WireAccArgs& X, uint32_t q0, uint32_t n) {
+  uint32_t b = ww_request(p, type, W, gid, X, q0, n - 1u);
+  for (uint32_t q = q0 + 1; q < q0 + n; q++) {
+    const uint32_t l = ww_request(p + b + 4, GPX_PT_REQUEST, W, gid, X, q, 0u);
+    ww_i32(p + b, (int32_t)l);
+    b += 4u + l;
+  }
+  return b;
+}
+/* the bytes ww_requests writes: per request the header, 55 fixed bytes and the value, and 4 per latched one */
+__device__ __forceinline__ uint32_t wire_requests_bytes(const WireNames& W, uint32_t gid, const gpx_request_rec* reqs,
+                                                        uint32_t q0, uint32_t n) {
+  uint32_t bytes = 0;
+  for (uint32_t q = q0; q < q0 + n; q++)
+    bytes += 13u + W.name[(size_t)gid * GPX_NAME_BYTES] + 55u + reqs[q].payload_len + (q > q0 ? 4u : 0u);
+  return bytes;
 }
 
 /* one thread per sorted position; every encoded ACCEPT is one AcceptPacket (AcceptPacket.toBytes :95-138), stored once
@@ -972,10 +977,7 @@ __global__ void k_wire_enc_accepts(const __grid_constant__ DevState S, const __g
     if (sent) {
       const gpx_accept_rec a = recs[i];
       const GroupCtx g = group_ctx(S, a.h.gid);
-      const uint32_t q0 = X.head[i];
-      bytes = 22u;
-      for (uint32_t q = q0; q < q0 + a.nreq; q++)
-        bytes += wire_request_bytes(W, a.h.gid, X.reqs[q].payload_len) + (q > q0 ? 4u : 0u);
+      bytes = wire_requests_bytes(W, a.h.gid, X.reqs, X.head[i], a.nreq) + 22u;
       n_remote = g.R - wire_popc(g.ms->lane_mask);
     }
     A.cnt[p] = bytes;
@@ -985,14 +987,8 @@ __global__ void k_wire_enc_accepts(const __grid_constant__ DevState S, const __g
   if (!sent) return;
   const gpx_accept_rec a = recs[i];
   const GroupCtx g = group_ctx(S, a.h.gid);
-  const uint32_t q0 = X.head[i];
   uint8_t* o = A.out + A.off[p];
-  uint32_t b = ww_request(o, GPX_PT_ACCEPT, W, a.h.gid, X, q0, a.nreq - 1u);
-  for (uint32_t q = q0 + 1; q < q0 + a.nreq; q++) { /* {int length}{REQUEST packet} :929-936 */
-    const uint32_t l = ww_request(o + b + 4, GPX_PT_REQUEST, W, a.h.gid, X, q, 0u);
-    ww_i32(o + b, (int32_t)l);
-    b += 4u + l;
-  }
+  uint32_t b = ww_requests(o, GPX_PT_ACCEPT, W, a.h.gid, X, X.head[i], a.nreq);
   ww_i32(o + b, a.h.slot);
   ww_i32(o + b + 4, a.h.bnum);
   ww_i32(o + b + 8, a.h.bcoord);
@@ -1001,14 +997,5 @@ __global__ void k_wire_enc_accepts(const __grid_constant__ DevState S, const __g
   o[b + 17] = 0; /* noCoalesce */
   ww_i32(o + b + 18, a.sender);
   b += 22;
-  uint32_t ri = A.off[A.n + p];
-  for (uint32_t m = 0; m < g.R; m++) {
-    if (g.ms->lane_of_idx[m] != 0xffu) continue;
-    gpx_wire_ref r;
-    r.off = A.off[p];
-    r.len = b;
-    r.gid = a.h.gid;
-    r.node = g.ms->nodes[m];
-    A.refs[ri++] = r;
-  }
+  wire_refs_remote(A, p, g, a.h.gid, b);
 }

@@ -98,25 +98,18 @@ __global__ void k_wire_fwd(const __grid_constant__ DevState S, const __grid_cons
     if (st == GPX_WE_SENT && fc > 3) st = GPX_WE_ELECT; /* isPingPonging :508 */
     if (st == GPX_WE_SENT && !named) st = GPX_WE_NO_NAME;
     if (!A.emit) {
-      uint32_t bytes = 0;
       for (uint32_t q = k; q < b; q++) {
         A.rstatus[q] = st;
         A.cnt[q] = A.cnt[A.n + q] = 0;
-        bytes += wire_request_bytes(W, gid, A.reqs[q].payload_len) + (q > k ? 4u : 0u);
       }
       if (st == GPX_WE_SENT) {
-        A.cnt[k] = bytes;
+        A.cnt[k] = wire_requests_bytes(W, gid, A.reqs, k, b - k);
         A.cnt[A.n + k] = 1;
       }
     } else if (st == GPX_WE_SENT) {
       uint8_t* o = A.out + A.off[k];
-      uint32_t len = ww_request(o, GPX_PT_REQUEST, W, gid, X, k, b - k - 1u);
+      const uint32_t len = ww_requests(o, GPX_PT_REQUEST, W, gid, X, k, b - k);
       ww_i32(o + 13u + W.name[(size_t)gid * GPX_NAME_BYTES] + 34u, fc); /* the outer request's forwardCount */
-      for (uint32_t q = k + 1; q < b; q++) { /* {int length}{REQUEST packet} :929-936 */
-        const uint32_t l = ww_request(o + len + 4, GPX_PT_REQUEST, W, gid, X, q, 0u);
-        ww_i32(o + len, (int32_t)l);
-        len += 4u + l;
-      }
       gpx_wire_ref r;
       r.off = A.off[k];
       r.len = len;
@@ -283,17 +276,9 @@ struct WireJsonReqArgs {
   int emit;
 };
 
-/* one request at staged position o, its value unescaped at payload offset *po (advanced): k_wire_req_decode's record
- * (wire_put_request) for the same RequestPacket */
-__device__ __forceinline__ void json_put_request(const WireJsonReqArgs& A, uint32_t o, uint32_t* po, uint32_t gid,
-                                                 uint32_t i, int32_t node, uint32_t lane, const JRd& J0,
+/* one request with its value unescaped: k_wire_req_decode's record (wire_put_request) for the same RequestPacket */
+__device__ __forceinline__ void json_put_request(const WireJsonReqArgs& A, WireReqTo& t, const JRd& J0,
                                                  const JsonReq& f) {
-  gpx_request_rec rq;
-  rq.gid = gid;
-  rq.flags = (f.stop ? GPX_F_STOP : 0u) | (lane << 8);
-  rq.req_id = f.qid;
-  rq.payload_off = *po;
-  rq.payload_len = f.qv_len;
   gpx_wire_req_meta m;
   memset(&m, 0, sizeof m);
   for (int b = 0; b < 4; b++) {
@@ -305,17 +290,7 @@ __device__ __forceinline__ void json_put_request(const WireJsonReqArgs& A, uint3
   m.forward_count = f.nfwds;
   m.entry_time = f.et;
   m.flags = (f.qf ? GPX_RM_RETURN_VALUE : 0u) | (f.bc ? GPX_RM_BROADCASTED : 0u);
-  if (f.e == -1) { /* IntegerMap.NULL_INT_NODE: setEntryReplica :393-403 with the call's clock */
-    rq.entry_node = node;
-    m.entry_time = A.now_ms;
-  } else {
-    rq.entry_node = f.e;
-  }
-  rq.client = i;
-  A.req[o] = rq;
-  A.meta[o] = m;
-  A.key[o] = gid;
-  uint8_t* d = A.payload + *po;
+  uint8_t* d = wire_put_request(A, t, f.qid, f.stop, f.e, f.qv_len, m);
   JRd Q = J0;
   Q.n = f.qv_at + 1u;
   for (uint32_t b = 0; b < f.qv_len; b++) { /* one thread copies the whole value, however long */
@@ -323,9 +298,6 @@ __device__ __forceinline__ void json_put_request(const WireJsonReqArgs& A, uint3
     jr_unit(Q, &u);
     d[b] = (uint8_t)u;
   }
-  const uint32_t padded = (f.qv_len + 15u) & ~15u;
-  for (uint32_t b = f.qv_len; b < padded; b++) d[b] = 0;
-  *po += padded;
 }
 
 /* one thread per member.  Pass 0 (emit == 0): a member listed GPX_WS_UNHANDLED that is a REQUEST object (PT 1) is
@@ -400,23 +372,17 @@ __global__ void k_json_req(const __grid_constant__ DevState S, const __grid_cons
         if (!ok) st = GPX_WS_MALFORMED;
       }
     }
+    GroupCtx g;
     if (st == GPX_WS_OK) {
       JRd I = J;
       I.n = pos[JQ_ID];
       const JStr id = jr_string(I);
       gid = json_id_gid(W, J, pos[JQ_ID], id);
-      const GroupCtx g = group_ctx(S, gid);
-      if (gid == GPX_NAME_NONE || !g.live) {
-        st = GPX_WS_UNKNOWN_NAME;
-      } else if (W.version[gid] != ver) {
-        st = GPX_WS_VERSION; /* PISM :441-447 */
-      } else {
-        node = A.pkts[mb.pkt].node;
-        lane = S.L;
-        for (uint32_t l = 0; l < S.L; l++)
-          if (S.lane_node[l] == node) lane = l;
-        if (lane == S.L || wire_member_idx(g.ms, g.R, node) == 0xffu) st = GPX_WS_NOT_LOCAL;
-      }
+      st = wire_group(S, W, gid, ver, g);
+    }
+    if (st == GPX_WS_OK) {
+      node = A.pkts[mb.pkt].node;
+      st = wire_recv_lane(S, g, node, lane);
     }
   }
   if (!A.emit) {
@@ -425,8 +391,8 @@ __global__ void k_json_req(const __grid_constant__ DevState S, const __grid_cons
     A.cnt[A.n + i] = st == GPX_WS_OK ? pay : 0u;
     return;
   }
-  uint32_t o = A.off[i], po = A.off[A.n + i];
-  json_put_request(A, o++, &po, gid, i, node, lane, J, f);
+  WireReqTo t = {A.off[i], A.off[A.n + i], gid, i, lane, node};
+  json_put_request(A, t, J, f);
   if (!pos[JQ_BATCH]) return;
   JRd B = J;
   B.n = pos[JQ_BATCH] + 1u;
@@ -437,7 +403,7 @@ __global__ void k_json_req(const __grid_constant__ DevState S, const __grid_cons
     json_keys_t<JsonReqKeys>(B, sp, nullptr, &ppc);
     JsonReq g;
     json_req_fields(B, sp, g);
-    json_put_request(A, o++, &po, gid, i, node, lane, B, g);
+    json_put_request(A, t, B, g);
     jr_ws(B);
     if (jr_peek(B) != ',') return;
     B.n++;

@@ -744,8 +744,7 @@ struct JsonDecSink { /* BatchedCommit SLOTS */
 };
 
 /* the gid named by the "ID" string at `at` (id: what jr_string read of it), unescaped before the lookup, or
- * GPX_NAME_NONE; a name with a character above U+00FF or longer than GPX_WIRE_MAX_ID names no gid.  k_json_req calls
- * it; k_json_member below keeps the same steps inline, which leaves its instructions as they were. */
+ * GPX_NAME_NONE; a name with a character above U+00FF or longer than GPX_WIRE_MAX_ID names no gid */
 __device__ __forceinline__ uint32_t json_id_gid(const WireNames& W, const JRd& J, uint32_t at, const JStr& id) {
   if (id.wide || id.len > GPX_WIRE_MAX_ID) return GPX_NAME_NONE;
   uint8_t buf[GPX_WIRE_MAX_ID];
@@ -870,42 +869,21 @@ __global__ void k_json_member(const __grid_constant__ DevState S, const __grid_c
   if (!ok) st = GPX_WS_MALFORMED;
   else if (!(reply || pt == GPX_PT_BATCHED_COMMIT) || (pt == GPX_PT_ACCEPT_REPLY && nack)) st = GPX_WS_UNHANDLED;
   uint32_t gid = GPX_NAME_NONE;
+  GroupCtx g;
   uint8_t acc_idx = 0xffu, dst_idx = 0xffu;
-  const MsetInfo* ms = nullptr;
   if (st == GPX_WS_OK) {
-    if (id.wide || id.len > GPX_WIRE_MAX_ID) {
-      st = GPX_WS_UNKNOWN_NAME; /* no gid can have this name */
-    } else {
-      uint8_t buf[GPX_WIRE_MAX_ID];
-      const uint8_t* name = J.b + pos[JK_ID] + 1u;
-      if (id.esc) {
-        JRd I = J;
-        I.n = pos[JK_ID] + 1u;
-        uint32_t u = 0;
-        for (uint32_t q = 0; q < id.len; q++) {
-          jr_unit(I, &u);
-          buf[q] = (uint8_t)u;
-        }
-        name = buf;
-      }
-      gid = wire_name_find(W, name, id.len);
-      const GroupCtx g = group_ctx(S, gid);
-      if (gid == GPX_NAME_NONE || !g.live) {
-        st = GPX_WS_UNKNOWN_NAME;
-      } else if (W.version[gid] != ver) {
-        st = GPX_WS_VERSION; /* PISM :441-447 */
-      } else {
-        ms = g.ms;
-        if (reply) {
-          acc_idx = wire_member_idx(ms, g.R, sndr);
-          /* a singleton reply goes to the node that received it: a NACK's ballot names another coordinator */
-          dst_idx = wire_member_idx(ms, g.R, pt == GPX_PT_ACCEPT_REPLY ? r.node : bcoord);
-          if (acc_idx == 0xffu || (pt == GPX_PT_BATCHED_ACCEPT_REPLY && dst_idx == 0xffu)) st = GPX_WS_MALFORMED;
-          else if (dst_idx == 0xffu || ms->lane_of_idx[dst_idx] == 0xffu) st = GPX_WS_NOT_LOCAL;
-        } else if (ms->lane_mask == 0) {
-          st = GPX_WS_NOT_LOCAL;
-        }
-      }
+    gid = json_id_gid(W, J, pos[JK_ID], id);
+    st = wire_group(S, W, gid, ver, g);
+  }
+  if (st == GPX_WS_OK) {
+    if (reply) {
+      acc_idx = wire_member_idx(g.ms, g.R, sndr);
+      /* a singleton reply goes to the node that received it: a NACK's ballot names another coordinator */
+      dst_idx = wire_member_idx(g.ms, g.R, pt == GPX_PT_ACCEPT_REPLY ? r.node : bcoord);
+      if (acc_idx == 0xffu || (pt == GPX_PT_BATCHED_ACCEPT_REPLY && dst_idx == 0xffu)) st = GPX_WS_MALFORMED;
+      else if (dst_idx == 0xffu || g.ms->lane_of_idx[dst_idx] == 0xffu) st = GPX_WS_NOT_LOCAL;
+    } else if (g.ms->lane_mask == 0) {
+      st = GPX_WS_NOT_LOCAL;
     }
   }
   if (!A.emit) {
@@ -925,12 +903,8 @@ __global__ void k_json_member(const __grid_constant__ DevState S, const __grid_c
   if (st != GPX_WS_OK) return;
   if (reply) {
     JsonRepSink s;
-    s.x.gid = gid;
+    s.x = wire_reply_rec(gid, bnum, bcoord, cp, GPX_WHO(acc_idx, dst_idx, 0u));
     s.x.slot = slot;
-    s.x.bnum = bnum;
-    s.x.bcoord = bcoord;
-    s.x.max_cp = cp;
-    s.x.who = GPX_WHO(acc_idx, dst_idx, 0u);
     s.x.req_id = (int64_t)(int32_t)(uint32_t)(uint64_t)qid; /* AcceptReplyPacket(JSONObject) :115 reads QID with getInt */
     const uint32_t o = A.moff[A.cap_mem + i];
     s.out = A.rep + o;
@@ -943,14 +917,7 @@ __global__ void k_json_member(const __grid_constant__ DevState S, const __grid_c
     }
   } else {
     JsonDecSink s;
-    s.d.gid = gid;
-    s.d.slot = 0;
-    s.d.bnum = bnum;
-    s.d.bcoord = bcoord;
-    s.d.median_cp = gc;
-    s.d.flags = GPX_F_DECISION;
-    s.d.dst_mask = ms->lane_mask;
-    s.d.req_id = 0; /* a BatchedCommit carries slots only: the value is the accept the acceptor holds */
+    s.d = wire_decision_rec(gid, bnum, bcoord, gc, g.ms->lane_mask);
     const uint32_t o = A.moff[2 * A.cap_mem + i];
     s.out = A.dec + o;
     s.key = A.dec_key + o;
