@@ -549,21 +549,33 @@ class Engine:
         self.L.check(self.L.fn("reset_counters")(self._h))
 
 
-def parse_log(buf: np.ndarray, ring_cap: Optional[int] = None):
-    """Walk the segments of a log ring image.  Yields (hdr, images, payload_area, payload_ring_off)."""
+def seg_end(off: int, hdr) -> int:
+    """Where the segment whose header `hdr` sits at ring offset `off` ends (seg_end in gpx_dev.cuh)."""
+    return (off + 64 + int(hdr["n_slots"]) * int(hdr["rec_bytes"]) + ((int(hdr["payload_bytes"]) + 15) & ~15)
+            + 31) & ~31
+
+
+def parse_log(buf: np.ndarray, ring_cap: Optional[int] = None, base: int = 0):
+    """Walk the segments of a log ring image.  Returns [(hdr, images, payload_area, payload_ring_off)].
+
+    Without ring_cap the walk stops at the first header whose magic does not match.  With ring_cap, buf holds a
+    device ring's bytes from the absolute ring offset `base` on, and a segment counts only when its magic matches and
+    its ring_off is base + its offset in buf (the rule k_log_dir applies).  Anything else is the tail a launch skipped
+    because it would have straddled the ring end, and may hold stale segments of an earlier lap: the walk goes on at
+    the next lap."""
     out = []
     off = 0
     n = buf.size
     while off + 64 <= n:
         hdr = buf[off: off + 64].view(seg_hdr_dtype)[0]
-        if int(hdr["magic"]) != SEG_MAGIC:
-            if ring_cap:  # wrap padding: skip to the next ring boundary
-                nxt = (off // ring_cap + 1) * ring_cap
-                if nxt <= off or nxt + 64 > n:
-                    break
-                off = nxt
-                continue
-            break
+        if int(hdr["magic"]) != SEG_MAGIC or (ring_cap and int(hdr["ring_off"]) != base + off):
+            if not ring_cap:
+                break
+            nxt = ((base + off) // ring_cap + 1) * ring_cap - base
+            if nxt <= off or nxt + 64 > n:
+                break
+            off = nxt
+            continue
         rec = int(hdr["rec_bytes"])
         ns = int(hdr["n_slots"])
         nv = int(hdr["n_valid"])
@@ -582,5 +594,5 @@ def parse_log(buf: np.ndarray, ring_cap: Optional[int] = None):
         pay_off = off + 64 + ns * rec
         payload = buf[pay_off: pay_off + pb]
         out.append((hdr, imgs, payload, pay_off))
-        off = (pay_off + ((pb + 15) & ~15) + 31) & ~31
+        off = seg_end(base + off, hdr) - base
     return out

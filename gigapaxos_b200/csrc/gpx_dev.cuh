@@ -449,6 +449,29 @@ struct DPValue {
   bool valued;
 };
 
+/*
+ * The log ring's segment layout (DESIGN §3), shared by the logging kernels, the host's mirror of the ring heads and
+ * the readers.  n is the number of images a segment reserves.
+ *   ACCEPT             [64 B header][n x 32 B images][n x 16 B extensions][payload], rounded up to 32 B
+ *   DECISION, PREPARE  [64 B header][n x 32 B images]
+ * Macros rather than inline functions: nvcc simplifies an inline function before it inlines it, and as functions
+ * these changed the instructions of k_accept, k_act and k_round_slow (an image and its extension no longer shared
+ * the address arithmetic of their segment).
+ */
+/* where image j, and the extension of ACCEPT image j of n, start in the segment at `seg` (ring position or pointer) */
+#define GPX_SEG_IMG(seg, j) ((seg) + 64ull + (unsigned long long)(j) * 32ull)
+#define GPX_SEG_EXT(seg, n, j) ((seg) + 64ull + (unsigned long long)(n) * 32ull + (unsigned long long)(j) * 16ull)
+/* where an ACCEPT segment's payload area starts, relative to the segment */
+#define GPX_SEG_PAY_OFF(n) (64ull + (unsigned long long)(n) * 48ull)
+/* segment sizes: ACCEPT with `pay` payload bytes (the images need 32-B alignment), DECISION or PREPARE */
+#define GPX_SEG_ACC_BYTES(n, pay) ((GPX_SEG_PAY_OFF(n) + (pay) + 31ull) & ~31ull)
+#define GPX_SEG_DEC_BYTES(n) (64ull + (unsigned long long)(n) * 32ull)
+/* reader form: where the segment whose header `h` sits at `pos` ends (payload padded as the writers pad it) */
+__host__ __device__ __forceinline__ unsigned long long seg_end(unsigned long long pos, const gpx_log_seg_hdr& h) {
+  return (pos + 64ull + (unsigned long long)h.n_slots * h.rec_bytes + ((h.payload_bytes + 15ull) & ~15ull) + 31ull) &
+         ~31ull;
+}
+
 /* segment base of this launch for one lane: skip to the ring start if it would wrap */
 __device__ __forceinline__ unsigned long long seg_base(const DevState& S, uint32_t l, unsigned long long reserved) {
   unsigned long long head = S.log_pos[((size_t)S.lp * GPX_MAX_LANES + l) * 2];

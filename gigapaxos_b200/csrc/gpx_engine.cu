@@ -550,6 +550,10 @@ int gpx_patch(gpx_engine* e, uint32_t n, const gpx_patch_rec* p) {
 }
 
 static void log_advance(gpx_engine* e, uint64_t reserved, bool exact);
+/* the constructed blobs a round reserves room for in its ACCEPT segment, before it knows how many it builds */
+static uint64_t round_blob1(const gpx_engine* e, uint32_t n, uint64_t pal) {
+  return e->cfg.batching_enabled ? std::min<uint64_t>(e->blob1_cap, 16ull * n + pal) : 0;
+}
 /* every launch that appends to the log reads log_pos[lp] and writes log_pos[lp ^ 1]: flip after the launch */
 static inline void log_flip(gpx_engine* e) { e->S.lp ^= 1u; }
 
@@ -607,11 +611,9 @@ static int launch_accept(gpx_engine* e, bool fused, const gpx_accept_rec* d_recs
   A.extra_cap = e->extra_cap;
   A.n_extra = &e->d_ctl->n_extra;
   const uint32_t grid = cdiv(n_max, GPX_BLOCK);
-  { /* host mirror of the ring heads: the kernels' own arithmetic (k_accept: one segment; k_act: two, back to back) */
-    const unsigned long long pay_rel = 64ull + (unsigned long long)n_max * 48ull;
-    const unsigned long long res_a = (pay_rel + blob0_bytes + blob1_bytes + 31ull) & ~31ull;
-    log_advance(e, fused ? res_a + 64ull + (unsigned long long)n_max * 32ull : res_a, blob1_used_ptr == nullptr);
-  }
+  /* host mirror of the ring heads (k_accept: one segment; k_act: two, back to back) */
+  log_advance(e, GPX_SEG_ACC_BYTES(n_max, blob0_bytes + blob1_bytes) + (fused ? GPX_SEG_DEC_BYTES(n_max) : 0ull),
+              blob1_used_ptr == nullptr);
   if (fused) {
     GPX_DISPATCH_L(e->cfg.n_lanes, k_act, grid, st, e->S, A);
   } else {
@@ -649,7 +651,7 @@ static int launch_commit(gpx_engine* e, const gpx_decision_rec* d_dec, const uin
   A.extra = e->d_extra;
   A.extra_cap = e->extra_cap;
   A.n_extra = &e->d_ctl->n_extra;
-  log_advance(e, 64ull + (unsigned long long)n_max * 32ull, true);
+  log_advance(e, GPX_SEG_DEC_BYTES(n_max), true);
   GPX_DISPATCH_L(e->cfg.n_lanes, k_commit, cdiv(n_max, GPX_BLOCK), st, e->S, A);
   log_flip(e);
   CK(cudaGetLastError());
@@ -740,12 +742,12 @@ static int launch_round(gpx_engine* e, const gpx_request_rec* d_reqs, const uint
   RA.todo_end = e->d_todo + e->cfg.max_batch_recs;
   RA.mark = e->d_mark;
   RA.n_todo = &d_ctl->n_todo;
-  RA.blob1_res = e->cfg.batching_enabled ? std::min<uint64_t>(e->blob1_cap, 16ull * n + pal) : 0;
+  RA.blob1_res = round_blob1(e, n, pal);
   RA.A.blob1_bytes = RA.blob1_res;
   RA.pay_bytes = pal + RA.blob1_res;
-  RA.pay_rel = 64u + n * 48u;
-  RA.res_a = ((unsigned long long)RA.pay_rel + RA.pay_bytes + 31ull) & ~31ull;
-  RA.res_d = 64ull + (unsigned long long)n * 32ull;
+  RA.pay_rel = (uint32_t)GPX_SEG_PAY_OFF(n);
+  RA.res_a = GPX_SEG_ACC_BYTES(n, RA.pay_bytes);
+  RA.res_d = GPX_SEG_DEC_BYTES(n);
   log_advance(e, RA.res_a + RA.res_d, true);
   const uint32_t L = e->cfg.n_lanes;
   const uint32_t teams_per_block = (GPX_RBLOCK / 32u) * (32u / L); /* teams of L adjacent lanes */
@@ -808,6 +810,12 @@ static int ring_fits(gpx_engine* e, uint64_t reserved) {
   }
   return GPX_OK;
 }
+/* the bounds the calls pass to ring_fits: an ACCEPT segment of n images and `pay` payload bytes counts its padding to
+ * 32 B as a whole 32 bytes; a call that also logs the DECISIONs adds GPX_SEG_DEC_BYTES(n); a round keeps 32 bytes more */
+static uint64_t acc_bound(uint64_t n, uint64_t pay) { return GPX_SEG_PAY_OFF(n) + pay + 32ull; }
+static uint64_t round_bound(const gpx_engine* e, uint32_t n, uint64_t pal) {
+  return acc_bound(n, pal + round_blob1(e, n, pal)) + GPX_SEG_DEC_BYTES(n) + 32ull;
+}
 static int check_batch(gpx_engine* e, uint32_t n, uint64_t payload_bytes) {
   if (n > e->cfg.max_batch_recs) return fail(GPX_ERANGE, "n > max_batch_recs");
   if (payload_bytes > e->cfg.max_batch_payload) return fail(GPX_ERANGE, "payload_bytes > max_batch_payload");
@@ -865,7 +873,7 @@ int gpx_handle_accepts(gpx_engine* e, uint32_t n, const gpx_accept_rec* accepts,
   if (blob_bytes & 15) return fail(GPX_EINVAL, "blob_bytes must be a multiple of 16");
   if (n > e->cfg.max_batch_recs) return fail(GPX_ERANGE, "n > max_batch_recs");
   if (blob_bytes > e->blob1_cap) return fail(GPX_ERANGE, "blob too large");
-  int rc = ring_fits(e, 96ull + 48ull * n + blob_bytes);
+  int rc = ring_fits(e, acc_bound(n, blob_bytes));
   if (rc) return rc;
   cudaStream_t st = e->stream;
   const uint32_t L = e->cfg.n_lanes;
@@ -919,7 +927,7 @@ int gpx_handle_decisions(gpx_engine* e, uint32_t n, const gpx_decision_rec* deci
   if (n == 0) return GPX_OK;
   if (!decisions || !out_exec) return fail(GPX_EINVAL, "null argument");
   if (n > (uint64_t)e->cfg.max_batch_recs) return fail(GPX_ERANGE, "n > max_batch_recs");
-  int rc = ring_fits(e, 64ull + 32ull * n);
+  int rc = ring_fits(e, GPX_SEG_DEC_BYTES(n));
   if (rc) return rc;
   cudaStream_t st = e->stream;
   const uint32_t L = e->cfg.n_lanes;
@@ -946,7 +954,7 @@ int gpx_handle_prepares(gpx_engine* e, uint32_t n, const gpx_pvalue_hdr* prepare
   if (n == 0) return GPX_OK;
   if (!prepares || !out_replies) return fail(GPX_EINVAL, "null argument");
   if (n > e->cfg.max_batch_recs) return fail(GPX_ERANGE, "n > max_batch_recs");
-  int rc = ring_fits(e, 64ull + 32ull * n);
+  int rc = ring_fits(e, GPX_SEG_DEC_BYTES(n));
   if (rc) return rc;
   const uint32_t L = e->cfg.n_lanes;
   const size_t out_bytes = (size_t)n * L * sizeof(gpx_prepare_reply_rec);
@@ -958,7 +966,7 @@ int gpx_handle_prepares(gpx_engine* e, uint32_t n, const gpx_pvalue_hdr* prepare
   A.recs = e->d_decisions;
   A.n = n;
   A.replies = (gpx_prepare_reply_rec*)e->d_misc;
-  log_advance(e, 64ull + 32ull * n, true);
+  log_advance(e, GPX_SEG_DEC_BYTES(n), true);
   GPX_DISPATCH_L(L, k_prepare, cdiv(n, GPX_BLOCK), st, e->S, A);
   log_flip(e);
   CK(cudaGetLastError());
@@ -1018,7 +1026,7 @@ int gpx_handle_accepts_fused(gpx_engine* e, uint32_t n, const gpx_accept_rec* ac
   if (blob_bytes & 15) return fail(GPX_EINVAL, "blob_bytes must be a multiple of 16");
   if (n > e->cfg.max_batch_recs) return fail(GPX_ERANGE, "n > max_batch_recs");
   if (blob_bytes > e->blob1_cap) return fail(GPX_ERANGE, "blob too large");
-  int rc = ring_fits(e, 160ull + 80ull * n + blob_bytes);
+  int rc = ring_fits(e, acc_bound(n, blob_bytes) + GPX_SEG_DEC_BYTES(n));
   if (rc) return rc;
   cudaStream_t st = e->stream;
   const uint32_t L = e->cfg.n_lanes;
@@ -1136,8 +1144,7 @@ static int round_host(gpx_engine* e, bool fused, uint32_t n, const gpx_request_r
   int rc = check_batch(e, n, payload_bytes);
   if (rc) return rc;
   const uint64_t pal = (payload_bytes + 15) & ~15ull;
-  const uint64_t b1 = e->cfg.batching_enabled ? std::min<uint64_t>(e->blob1_cap, 16ull * n + pal) : 0;
-  rc = ring_fits(e, 192ull + 80ull * n + pal + b1);
+  rc = ring_fits(e, round_bound(e, n, pal));
   if (rc) return rc;
   cudaStream_t st = e->stream;
   const uint32_t L = e->cfg.n_lanes;
@@ -1300,7 +1307,7 @@ int gpx_accepts_device(gpx_engine* e, gpx_accept_rec* recs, uint32_t n, const ui
   if (blob_bytes & 15) return fail(GPX_EINVAL, "blob_bytes must be a multiple of 16");
   if (n_chunks > GPX_ROUTE_ND || (n_chunks && (!chunk_rec_end || !chunk_blob_base))) return fail(GPX_EINVAL, "chunks");
   if (n > e->cfg.max_batch_recs) return fail(GPX_ERANGE, "n > max_batch_recs");
-  int rc = ring_fits(e, 96ull + 48ull * n + blob_bytes);
+  int rc = ring_fits(e, acc_bound(n, blob_bytes));
   if (rc) return rc;
   cudaStream_t st = stream ? (cudaStream_t)stream : e->stream;
   {
@@ -1336,7 +1343,7 @@ int gpx_decisions_device(gpx_engine* e, gpx_decision_rec* decisions, uint32_t n,
   if (n == 0) return GPX_OK;
   if (!decisions || !out_exec) return fail(GPX_EINVAL, "null argument");
   if (n > e->cfg.max_batch_recs) return fail(GPX_ERANGE, "n > max_batch_recs");
-  int rc = ring_fits(e, 64ull + 32ull * n);
+  int rc = ring_fits(e, GPX_SEG_DEC_BYTES(n));
   if (rc) return rc;
   cudaStream_t st = stream ? (cudaStream_t)stream : e->stream;
   {
@@ -1387,8 +1394,7 @@ int gpx_round_submit(gpx_engine* e, const gpx_round_io* io, uint64_t* ticket) {
   int rc = check_batch(e, n, io->payload_bytes);
   if (rc) return rc;
   const uint64_t pal = (io->payload_bytes + 15) & ~15ull;
-  const uint64_t b1 = e->cfg.batching_enabled ? std::min<uint64_t>(e->blob1_cap, 16ull * n + pal) : 0;
-  rc = ring_fits(e, 192ull + 80ull * n + pal + b1);
+  rc = ring_fits(e, round_bound(e, n, pal));
   if (rc) return rc;
   rc = pipe_init(e);
   if (rc) return rc;
@@ -1525,9 +1531,9 @@ int gpx_log_find(gpx_engine* e, uint32_t lane, uint64_t from, uint32_t n, const 
   }
   CK(cudaDeviceSynchronize()); /* rounds may have been issued on a caller's stream; the head is read on the device */
   const size_t cells = (size_t)n * GPX_LOG_SPAN;
-  /* a segment is at least 96 bytes; a directory of 2^20 entries (32 MiB) covers every ring the launches of this engine
-   * can fill with fewer segments than that, else LOGF_TOO_MANY */
-  const uint64_t seg_cap64 = std::min<uint64_t>(e->cfg.log_ring_bytes / 96 + 2, 1ull << 20);
+  /* a segment is at least GPX_SEG_DEC_BYTES(1) = 96 bytes; a directory of 2^20 entries (32 MiB) covers every ring the
+   * launches of this engine can fill with fewer segments than that, else LOGF_TOO_MANY */
+  const uint64_t seg_cap64 = std::min<uint64_t>(e->cfg.log_ring_bytes / GPX_SEG_DEC_BYTES(1) + 2, 1ull << 20);
   const size_t want_bytes = ((size_t)n * sizeof(gpx_log_want) + 31) & ~(size_t)31;
   const size_t seg_bytes = (size_t)seg_cap64 * sizeof(LogSeg);
   const size_t best_bytes = 2 * cells * 8;

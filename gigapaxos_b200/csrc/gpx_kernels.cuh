@@ -896,8 +896,8 @@ __device__ __forceinline__ void copy_blob(const DevState& S, const AcceptArgs& A
 __device__ __forceinline__ void write_accept_image(const DevState& S, uint32_t l, unsigned long long segb,
                                                    uint32_t n_max, uint32_t j, const int4 q0, const int4 q1,
                                                    const int4 q2, uint32_t img_flags) {
-  st256_stream(ring_ptr(S, l, segb + 64 + (unsigned long long)j * 32), q0, make_int4(q1.x, (int)img_flags, q1.z, q1.w));
-  st_stream4(ring_ptr(S, l, segb + 64 + (unsigned long long)n_max * 32 + (unsigned long long)j * 16), q2);
+  st256_stream(ring_ptr(S, l, GPX_SEG_IMG(segb, j)), q0, make_int4(q1.x, (int)img_flags, q1.z, q1.w));
+  st_stream4(ring_ptr(S, l, GPX_SEG_EXT(segb, n_max, j)), q2);
 }
 
 __device__ __forceinline__ void store_void_exec(gpx_exec_rec* ex, uint32_t gid, int slot, uint32_t l) {
@@ -1022,8 +1022,8 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_ACCEPT_MINB) k_accept(const __g
   const uint32_t tile_bytes = t1 > t0 ? (t1 - t0) * (uint32_t)sizeof(gpx_accept_rec) : 0u;
   if (threadIdx.x == 0 && tile_bytes) tma_load_1d(s_tile, &A.recs[t0], tile_bytes, &s_bar);
   const unsigned long long pay_bytes = A.blob0_bytes + (A.blob1_used_ptr ? *A.blob1_used_ptr : A.blob1_bytes);
-  const unsigned long long pay_rel = 64ull + (unsigned long long)A.n_max * 48ull;
-  const unsigned long long reserved = (pay_rel + pay_bytes + 31ull) & ~31ull; /* images need 32-B alignment */
+  const unsigned long long pay_rel = GPX_SEG_PAY_OFF(A.n_max);
+  const unsigned long long reserved = GPX_SEG_ACC_BYTES(A.n_max, pay_bytes);
   unsigned long long segb[L], payb[L];
 #pragma unroll
   for (int l = 0; l < L; l++) {
@@ -1340,7 +1340,7 @@ __global__ void __launch_bounds__(GPX_BLOCK, 2) k_commit(const __grid_constant__
   uint32_t n = A.n_ptr ? *A.n_ptr : A.n_max;
   if (n > A.n_max) n = A.n_max;
   const uint32_t i = blockIdx.x * GPX_BLOCK + threadIdx.x;
-  const unsigned long long reserved = 64ull + (unsigned long long)A.n_max * 32ull;
+  const unsigned long long reserved = GPX_SEG_DEC_BYTES(A.n_max);
   unsigned long long segb[L];
 #pragma unroll
   for (int l = 0; l < L; l++) segb[l] = seg_base(S, l, reserved);
@@ -1380,7 +1380,7 @@ __global__ void __launch_bounds__(GPX_BLOCK, 2) k_commit(const __grid_constant__
               commit_lane_stored(S, l, gid, slot, q0.z, q0.w, q1.x, row[l], aux[l], e0[l], e1[l], ex, A.extra,
                                  A.extra_cap, A.n_extra, img0, img1, s_ctr);
           }
-          st256_stream(ring_ptr(S, l, segb[l] + 64 + (unsigned long long)j * 32), img0, img1);
+          st256_stream(ring_ptr(S, l, GPX_SEG_IMG(segb[l], j)), img0, img1);
         }
         j++;
         if (j >= n) break;
@@ -1412,9 +1412,9 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_ACT_MINB) k_act(const __grid_co
   if (n > A.n_max) n = A.n_max;
   const uint32_t i = blockIdx.x * GPX_BLOCK + threadIdx.x;
   const unsigned long long pay_bytes = A.blob0_bytes + (A.blob1_used_ptr ? *A.blob1_used_ptr : A.blob1_bytes);
-  const unsigned long long pay_rel = 64ull + (unsigned long long)A.n_max * 48ull;
-  const unsigned long long res_a = (pay_rel + pay_bytes + 31ull) & ~31ull;
-  const unsigned long long res_d = 64ull + (unsigned long long)A.n_max * 32ull;
+  const unsigned long long pay_rel = GPX_SEG_PAY_OFF(A.n_max);
+  const unsigned long long res_a = GPX_SEG_ACC_BYTES(A.n_max, pay_bytes);
+  const unsigned long long res_d = GPX_SEG_DEC_BYTES(A.n_max);
   unsigned long long segb[L], payb[L], dsegb[L];
 #pragma unroll
   for (int l = 0; l < L; l++) {
@@ -1511,7 +1511,7 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_ACT_MINB) k_act(const __grid_co
 #pragma unroll
         for (int l = 0; l < L; l++)
           commit_accepted_lane(S, A, l, gid, slot, g.live, decided, d, q0, q1, q2, st[l], &A.exec[(size_t)j * L + l],
-                               dsegb[l] + 64 + (unsigned long long)j * 32, s_ctr);
+                               GPX_SEG_IMG(dsegb[l], j), s_ctr);
         j++;
         if (j >= n) break;
         rp = reinterpret_cast<const int4*>(&A.recs[j]);

@@ -90,7 +90,7 @@ __global__ void k_log_dir(const __grid_constant__ DevState S, const __grid_const
       err = LOGF_CORRUPT;
       break;
     }
-    const unsigned long long next = (pos + 64ull + body + ((h.payload_bytes + 15ull) & ~15ull) + 31ull) & ~31ull;
+    const unsigned long long next = seg_end(pos, h);
     if (next - pos > cap) {
       err = LOGF_CORRUPT;
       break;
@@ -123,7 +123,7 @@ __global__ void __launch_bounds__(GPX_LOGF_BLOCK) k_log_scan(const __grid_consta
     const uint32_t j = (uint32_t)(idx - sg.first_img);
     const bool isAcc = sg.rec_bytes == 48u, isDec = sg.rec_bytes == 32u && sg.type == GPX_F_DECISION;
     if (!isAcc && !isDec) continue; /* logged PREPAREs */
-    const gpx_pvalue_hdr* img = reinterpret_cast<const gpx_pvalue_hdr*>(ring_ptr(S, A.lane, sg.pos + 64ull + (unsigned long long)j * 32ull));
+    const gpx_pvalue_hdr* img = reinterpret_cast<const gpx_pvalue_hdr*>(ring_ptr(S, A.lane, GPX_SEG_IMG(sg.pos, j)));
     const uint32_t gid = img->gid;
     if (img->flags & GPX_F_VOID) continue;
     uint32_t a = 0, b = A.n; /* the want of this group */
@@ -153,19 +153,19 @@ __global__ void __launch_bounds__(GPX_LOGF_BLOCK) k_log_hits(const __grid_consta
     if (bd) {
       const LogSeg sg = A.segs[(uint32_t)((bd - 1ull) >> 32)];
       const uint32_t j = (uint32_t)((bd - 1ull) & 0xffffffffull);
-      hit.decision = *reinterpret_cast<const gpx_decision_rec*>(ring_ptr(S, A.lane, sg.pos + 64ull + (unsigned long long)j * 32ull));
+      hit.decision = *reinterpret_cast<const gpx_decision_rec*>(ring_ptr(S, A.lane, GPX_SEG_IMG(sg.pos, j)));
     }
     if (ba) {
       const LogSeg sg = A.segs[(uint32_t)((ba - 1ull) >> 32)];
       const uint32_t j = (uint32_t)((ba - 1ull) & 0xffffffffull);
-      hit.accept.h = *reinterpret_cast<const gpx_pvalue_hdr*>(ring_ptr(S, A.lane, sg.pos + 64ull + (unsigned long long)j * 32ull));
+      hit.accept.h = *reinterpret_cast<const gpx_pvalue_hdr*>(ring_ptr(S, A.lane, GPX_SEG_IMG(sg.pos, j)));
       const uint32_t* x = reinterpret_cast<const uint32_t*>(
-          ring_ptr(S, A.lane, sg.pos + 64ull + (unsigned long long)sg.n_slots * 32ull + (unsigned long long)j * 16ull));
+          ring_ptr(S, A.lane, GPX_SEG_EXT(sg.pos, sg.n_slots, j)));
       hit.accept.payload_off = x[0];
       hit.accept.payload_len = x[1];
       hit.accept.nreq = x[2];
       hit.accept.sender = (int32_t)x[3];
-      hit.blob_pos = sg.pos + 64ull + (unsigned long long)sg.n_slots * 48ull + x[0];
+      hit.blob_pos = sg.pos + GPX_SEG_PAY_OFF(sg.n_slots) + x[0];
     }
   }
   A.hits[t] = hit;

@@ -198,7 +198,7 @@ __device__ __forceinline__ void round_general(const DevState& S, const RoundArgs
     }
     if (sub < (uint32_t)L)
       commit_accepted_lane(S, A, sub, gid, slot, g.live, decided_i != 0, d, q0, q1, q2, st, &A.exec[(size_t)q * L + sub],
-                           dseg + 64 + (unsigned long long)q * 32, s_ctr);
+                           GPX_SEG_IMG(dseg, q), s_ctr);
     if (RA.sum) { /* compact mode: the general path reports through the extra queue */
       if (sub < (uint32_t)L) {
         const gpx_exec_rec er = A.exec[(size_t)q * L + sub];
@@ -438,7 +438,7 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
     int4* const img = &s_img[threadIdx.x >> 5][(sub * TPW + team_in_warp) * 2];
     img[0] = q0;
     img[1] = make_int4(median, (int)(GPX_F_ACCEPT | ((1u << sub) << 16)), rq0.z, rq0.w);
-    st_stream4(seg_p + 64 + (size_t)n * 32 + (size_t)i * 16, make_int4((int)poff, (int)plen, 1, crow.y));
+    st_stream4(GPX_SEG_EXT(seg_p, n, i), make_int4((int)poff, (int)plen, 1, crow.y));
     if (plen) {
       uint8_t* dst = seg_p + pay_rel + poff;
       if (pal) {
@@ -508,8 +508,7 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
       const uint32_t k = k0 + lane_id, r = k >> 1, team = r % TPW, kl = r / TPW, l = kl % L;
       const unsigned long long seg_l = __shfl_sync(FULL, seg, l);
       if (k < NIMG && ((sfm >> (team * LP)) & 1u))
-        st_stream4(ring_ptr(S, l, seg_l + (kl >= (uint32_t)L ? res_a : 0ull) + 64ull +
-                                      (unsigned long long)(i0 + team) * 32ull + (k & 1u) * 16u),
+        st_stream4(ring_ptr(S, l, GPX_SEG_IMG(seg_l + (kl >= (uint32_t)L ? res_a : 0ull), i0 + team) + (k & 1u) * 16u),
                    s_img[threadIdx.x >> 5][k]);
     }
   }
@@ -730,7 +729,7 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
       img[(L + l) * 64 + 1] =
           make_int4(metaf ? -1 : dmed, (int)((GPX_F_DECISION | (metaf ? GPX_F_META : 0u)) | ((1u << l) << 16)),
                     rq0.z, rq0.w);
-      st_stream4(seg_p + 64 + (size_t)n * 32 + (size_t)i * 16, make_int4((int)poff, (int)plen, 1, crow.y));
+      st_stream4(GPX_SEG_EXT(seg_p, n, i), make_int4((int)poff, (int)plen, 1, crow.y));
       if (plen) {
         uint8_t* dst = seg_p + pay_rel + poff;
         if (pal)
@@ -780,8 +779,7 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
     for (uint32_t k0 = 0; k0 < 4u * L * 32u; k0 += 32u) {
       const uint32_t kl = k0 >> 6, l = kl % L, k = k0 + lane_id, g = (k >> 1) & 31u;
       if ((sfm >> g) & 1u)
-        st_stream4(ring_ptr(S, l, seg[l] + (kl >= (uint32_t)L ? res_a : 0ull) + 64ull +
-                                     (unsigned long long)(i0 + g) * 32ull + (k & 1u) * 16u),
+        st_stream4(ring_ptr(S, l, GPX_SEG_IMG(seg[l] + (kl >= (uint32_t)L ? res_a : 0ull), i0 + g) + (k & 1u) * 16u),
                    s_img[warp][k]);
     }
   }
@@ -916,7 +914,7 @@ __global__ void __launch_bounds__(GPX_BLOCK, 2) k_round_slow(const __grid_consta
 #pragma unroll
       for (int l = 0; l < L; l++) {
         write_accept_image(S, l, segl[l], n, q, z0, z1, make_int4(0, 0, 0, 0), GPX_F_VOID);
-        st256_stream(ring_ptr(S, l, segl[l] + res_a + 64 + (unsigned long long)q * 32), z0, z1);
+        st256_stream(ring_ptr(S, l, GPX_SEG_IMG(segl[l] + res_a, q)), z0, z1);
         store_void_exec(&A.exec[(size_t)q * L + l], gid, 0, l);
       }
       st256_stream(&A.decisions[q], z0, z1);

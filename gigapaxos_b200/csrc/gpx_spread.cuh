@@ -239,8 +239,8 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_PHASE_MINB) k_sp_accept(const _
   const uint32_t tile_bytes = (j0 < cnt && t1 > t0) ? (t1 - t0) * (uint32_t)sizeof(gpx_accept_rec) : 0u;
   if (threadIdx.x == 0 && tile_bytes) tma_load_1d(s_tile, &recs[t0], tile_bytes, &s_bar);
   /* one ACCEPT segment per round: an image slot per virtual index, payload area = the received blob areas */
-  const unsigned long long pay_rel = 64ull + (unsigned long long)A.vtotal * 48ull;
-  const unsigned long long reserved = (pay_rel + A.blob_vtotal + 31ull) & ~31ull;
+  const unsigned long long pay_rel = GPX_SEG_PAY_OFF(A.vtotal);
+  const unsigned long long reserved = GPX_SEG_ACC_BYTES(A.vtotal, A.blob_vtotal);
   const unsigned long long segb = seg_base(S, 0, reserved);
   const unsigned long long payb = segb + pay_rel + B.blob_off;
   if (v == 0) {
@@ -430,7 +430,7 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_PHASE_MINB) k_sp_commit(const _
   if (cnt > B.cap) cnt = B.cap;
   const gpx_decision_rec* recs = reinterpret_cast<const gpx_decision_rec*>(sp_recs(B));
   const uint32_t Wm = S.W - 1;
-  const unsigned long long reserved = 64ull + (unsigned long long)A.vtotal * 32ull;
+  const unsigned long long reserved = GPX_SEG_DEC_BYTES(A.vtotal);
   const unsigned long long segb = seg_base(S, 0, reserved);
   if (v == 0) {
     const unsigned long long sq = seg_seq_of(S, 0);
@@ -446,7 +446,7 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_PHASE_MINB) k_sp_commit(const _
   const bool valid = B.cap && j < cnt;
   if (v < A.vtotal && !valid) { /* hole: VOID exec + VOID image */
     store_void_exec(&A.exec[v], 0, 0, 0);
-    st256_stream(ring_ptr(S, 0, segb + 64 + (unsigned long long)v * 32), make_int4(0, 0, 0, 0),
+    st256_stream(ring_ptr(S, 0, GPX_SEG_IMG(segb, v)), make_int4(0, 0, 0, 0),
                  make_int4(0, (int)GPX_F_VOID, 0, 0));
   }
   if (valid) {
@@ -477,7 +477,7 @@ __global__ void __launch_bounds__(GPX_BLOCK, GPX_PHASE_MINB) k_sp_commit(const _
                                A.n_extra, img0, img1, s_ctr);
           }
         }
-        st256_stream(ring_ptr(S, 0, segb + 64 + (unsigned long long)vv * 32), img0, img1);
+        st256_stream(ring_ptr(S, 0, GPX_SEG_IMG(segb, vv)), img0, img1);
         jj++;
         if (jj >= cnt) break;
         int4 t0, t1;

@@ -138,7 +138,7 @@ class LogDrainer:
             return 0
         buf = self.engine.log_read(self.lane, self.offset, head - self.offset)
         n = 0
-        for hdr, imgs, payload, _ in abi.parse_log(buf):
+        for hdr, imgs, payload, _ in abi.parse_log(buf, self.engine.cfg.log_ring_bytes, self.offset):
             if int(hdr["rec_bytes"]) == 48:
                 for a in imgs:
                     if a["flags"] & abi.F_VOID:

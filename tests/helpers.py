@@ -197,3 +197,30 @@ def make_requests_fast(gids, payload_len=1, seed=1, entry_lane=0, entry_node=100
     reqs["entry_node"] = entry_node
     reqs["client"] = np.arange(n, dtype=np.uint32)
     return reqs, pay.reshape(-1)
+
+
+def relay_into_small_ring(buf, heads, cap):
+    """lay the calls of an (unwrapped) oracle ring image into a ring of `cap` bytes the way the device does: a call that
+    would straddle the ring end skips to the ring start (gpx_dev.cuh seg_base), later laps overwrite earlier ones, every
+    segment header names its new absolute position.  -> (ring bytes, new head, {old segment offset: new position},
+    [new position of every call])"""
+    ring = np.zeros(cap, dtype=np.uint8)
+    pos, seg_map, call_pos = 0, {}, []
+    for b0, b1 in zip(heads[:-1], heads[1:]):
+        n = b1 - b0
+        assert n <= cap
+        if (pos % cap) + n > cap:
+            pos += cap - pos % cap
+        call_pos.append(pos)
+        chunk = buf[b0:b1].copy()
+        off = 0
+        while off + 64 <= n:  # re-stamp ring_off of every segment of the call
+            hdr = chunk[off: off + 64].view(abi.seg_hdr_dtype)[0]
+            assert int(hdr["magic"]) == abi.SEG_MAGIC and int(hdr["ring_off"]) == b0 + off
+            seg_map[b0 + off] = pos + off
+            chunk[off: off + 64].view(abi.seg_hdr_dtype)[0]["ring_off"] = pos + off
+            off = abi.seg_end(off, hdr)
+        assert off == n
+        ring[pos % cap: pos % cap + n] = chunk
+        pos += n
+    return ring, pos, seg_map, call_pos

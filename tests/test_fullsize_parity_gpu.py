@@ -20,20 +20,10 @@ pytestmark = pytest.mark.gpu
 
 
 def read_new_log(e, lane, prev_head, ring_cap=None):
-    """segments appended since prev_head: [(hdr, images, payload)], new head.  On the device a launch that would
-    straddle the ring wrap starts at the ring start instead: skip the padding."""
+    """segments appended since prev_head: [(hdr, images, payload)], new head"""
     head = e.log_head(lane)
     buf = e.log_read(lane, prev_head, head - prev_head)
-    segs = abi.parse_log(buf)
-    used = 0
-    if segs:
-        hdr, imgs, pay, pay_off = segs[-1]
-        used = (pay_off + ((int(hdr["payload_bytes"]) + 15) & ~15) + 31) & ~31
-    if ring_cap and used < len(buf):  # wrap padding after the parsed prefix (or before the first segment)
-        nxt = ((prev_head + used) // ring_cap + 1) * ring_cap - prev_head
-        if nxt < len(buf):
-            segs += abi.parse_log(buf[nxt:])
-    return [(h, i, p) for (h, i, p, _) in segs], head
+    return [(h, i, p) for (h, i, p, _) in abi.parse_log(buf, ring_cap, prev_head)], head
 
 
 def compare_round_logs(eo, eg, heads_o, heads_g, n_lanes, ring_cap):

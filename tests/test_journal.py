@@ -2,21 +2,22 @@
 ({int32 BE len}{packet}*, SQLPaxosLogger.java:1000-1003: ACCEPTs byteified, DECISIONs as the JSON string of the meta
 decision, :1084-1098) and read back the way SQLPaxosLogger's reader walks a file (:685-848)."""
 import os
+import types
 
 import numpy as np
 import pytest
 
 from gigapaxos_b200 import journal, wire
 from gigapaxos_b200.paxos_manager import NoopPaxosApp, PaxosManager
-from helpers import Engine, abi, make_config
+from helpers import Engine, abi, group_descs, make_config, make_requests, relay_into_small_ring
 
 NODES = [100, 101, 102]
 
 
-def run(lib, tmp_path):
-    eng = Engine(lib, make_config(lib, max_groups=32, max_batch_recs=1024, max_batch_payload=1 << 18))
+def run(lib, tmp_path, n_groups=6, rounds=6, **cfg):
+    eng = Engine(lib, make_config(lib, max_groups=32, max_batch_recs=1024, max_batch_payload=1 << 18, **cfg))
     pm = PaxosManager(eng, [NoopPaxosApp() for _ in NODES], NODES)
-    names = [f"NoopPaxosApp{i}" for i in range(6)]
+    names = [f"NoopPaxosApp{i}" for i in range(n_groups)]
     pm.createPaxosInstanceBatch({n: None for n in names}, NODES)
     meta = {}
     sent = {}
@@ -27,7 +28,7 @@ def run(lib, tmp_path):
     drainers = [journal.LogDrainer(eng, l, journal.Journaler(str(tmp_path) + "/", NODES[l], max_log_file_size=2000),
                                    lookup) for l in range(3)]
     rng = np.random.default_rng(4)
-    for r in range(6):
+    for r in range(rounds):
         for n in names:
             for _ in range(int(rng.integers(1, 4))):
                 val = bytes(rng.integers(97, 123, size=int(rng.integers(1, 30))).astype(np.uint8))
@@ -82,15 +83,14 @@ def test_journal_roundtrip_cpu(oracle_lib, tmp_path):
     check(*run(oracle_lib, tmp_path))
 
 
-@pytest.mark.gpu
-def test_journal_roundtrip_gpu(cuda_lib, oracle_lib, tmp_path):
-    pm, dr, sent = run(cuda_lib, tmp_path / "gpu")
-    check(pm, dr, sent)
-    pm2, dr2, _ = run(oracle_lib, tmp_path / "cpu")
-    # same packets in the same order on both (entry times differ: compare with entryTime masked)
-    for a, b in zip(dr, dr2):
-        pa = [p for f in a.j.files for p in journal.read_journal(f)]
-        pb = [p for f in b.j.files for p in journal.read_journal(f)]
+def packets(drainer):
+    return [p for f in drainer.j.files for p in journal.read_journal(f)]
+
+
+def same_packets(drainers_a, drainers_b):
+    """same packets in the same order on both (entry times differ: compare with entryTime masked)"""
+    for a, b in zip(drainers_a, drainers_b):
+        pa, pb = packets(a), packets(b)
         assert len(pa) == len(pb)
         for x, y in zip(pa, pb):
             vx, vy = journal.parse_packet(x), journal.parse_packet(y)
@@ -99,3 +99,74 @@ def test_journal_roundtrip_gpu(cuda_lib, oracle_lib, tmp_path):
                     if vx["kind"] == "ACCEPT" else ("paxos_id", "request_id", "slot", "bnum", "bcoord", "median_cp", "stop"))
             for k in keys:
                 assert vx[k] == vy[k]
+
+
+@pytest.mark.gpu
+def test_journal_roundtrip_gpu(cuda_lib, oracle_lib, tmp_path):
+    pm, dr, sent = run(cuda_lib, tmp_path / "gpu")
+    check(pm, dr, sent)
+    pm2, dr2, _ = run(oracle_lib, tmp_path / "cpu")
+    same_packets(dr, dr2)
+
+
+@pytest.mark.gpu
+def test_journal_roundtrip_gpu_across_ring_wraps(cuda_lib, oracle_lib, tmp_path):
+    """a 64 KiB ring, ~8 KB per lane and round: it wraps at least twice, and drains see the skips to the ring start"""
+    ring = 1 << 16
+    kw = dict(n_groups=30, rounds=24, log_ring_bytes=ring)
+    pm, dr, sent = run(cuda_lib, tmp_path / "gpu", **kw)
+    check(pm, dr, sent)
+    assert all(pm.engine.log_head(l) > 2 * ring for l in range(3)), "the ring was sized to wrap twice"
+    pm2, dr2, _ = run(oracle_lib, tmp_path / "cpu", **kw)
+    same_packets(dr, dr2)
+
+
+class RelaidRing:
+    """log_head / log_read of one lane over a ring that an (unwrapped) oracle log was re-laid into the way the device
+    lays it out (relay_into_small_ring)"""
+
+    def __init__(self, ring, head, cap):
+        self.cfg = types.SimpleNamespace(log_ring_bytes=cap)
+        self.ring, self.head, self.cap = ring, head, cap
+
+    def log_head(self, lane):
+        return self.head
+
+    def log_read(self, lane, start, nbytes):
+        return self.ring.take(np.arange(start, start + nbytes) % self.cap)
+
+
+def test_drain_across_ring_wraps_journals_every_segment(oracle_lib, tmp_path):
+    """Drained once per call from a ring that wraps, the journal equals the one drained from the unwrapped ring: the
+    segments after a skip to the ring start are journaled, and stale segments in the skipped tail are not."""
+    G = 40
+    eng = Engine(oracle_lib, make_config(oracle_lib, max_groups=G, max_batch_recs=4096, max_batch_payload=1 << 20))
+    eng.create_groups(group_descs(G))
+    rng = np.random.default_rng(6)
+    heads = [0]
+    for r in range(12):
+        sel = np.arange(G)[rng.random(G) < 0.8]
+        reqs, pay = make_requests(np.repeat(sel, np.where(rng.random(len(sel)) < 0.2, 2, 1)), payload_len=3 + r,
+                                  seed=6, round_no=r)
+        eng.round(reqs, pay)
+        heads.append(eng.log_head(0))
+
+    def lookup(gid, rid):
+        return f"NoopPaxosApp{gid}", 0, NODES[0], 0
+
+    want = journal.LogDrainer(eng, 0, journal.Journaler(str(tmp_path / "flat") + "/", NODES[0]), lookup)
+    want.drain()
+    want.j.close()
+    buf = eng.log_read(0)
+    cap = 1 << int(np.ceil(np.log2(2.2 * max(b - a for a, b in zip(heads[:-1], heads[1:])))))
+    got = journal.LogDrainer(None, 0, journal.Journaler(str(tmp_path / "ring") + "/", NODES[0]), lookup)
+    for k in range(2, len(heads) + 1):  # the ring as it is after each call
+        ring, head, _, _ = relay_into_small_ring(buf, heads[:k], cap)
+        got.engine = RelaidRing(ring, head, cap)
+        got.drain()
+    got.j.close()
+    assert head > 2 * cap, "the ring wraps more than twice"
+    assert got.accepts_written == want.accepts_written > 0
+    assert got.decisions_written == want.decisions_written > 0
+    assert packets(got) == packets(want)
+    eng.close()

@@ -14,29 +14,6 @@ from helpers import Engine, GpxErrorT, abi, canon, exec_by_lane, group_descs, ma
 pytestmark = pytest.mark.gpu
 
 
-def parse_stream(chunks, ring_cap):
-    """chunks: [(abs_from, bytes)] of one lane, contiguous in absolute ring offsets -> list of (hdr, images, payload).
-    A segment is genuine iff its header says it lives at exactly this absolute offset (hdr.ring_off): the padding a
-    launch leaves when it skips to the ring start still holds stale segments of earlier laps."""
-    if not chunks:
-        return []
-    base = chunks[0][0]
-    buf = np.concatenate([c[1] for c in chunks])
-    out, off = [], 0
-    while off + 64 <= len(buf):
-        hdr = buf[off: off + 64].view(abi.seg_hdr_dtype)[0]
-        if int(hdr["magic"]) == abi.SEG_MAGIC and int(hdr["ring_off"]) == base + off:
-            (h, im, pay, pay_off), = abi.parse_log(buf[off:])[:1]
-            out.append((h, im, pay))
-            off += (pay_off + ((int(h["payload_bytes"]) + 15) & ~15) + 31) & ~31
-            continue
-        nxt = ((base + off) // ring_cap + 1) * ring_cap - base  # wrap padding: the next segment starts at the ring start
-        if nxt <= off:
-            break
-        off = nxt
-    return out
-
-
 @pytest.mark.parametrize("mode", ["round", "round_phases"])
 def test_backpressure_and_drain_keep_every_byte(oracle_lib, cuda_lib, mode):
     import torch
@@ -86,7 +63,8 @@ def test_backpressure_and_drain_keep_every_byte(oracle_lib, cuda_lib, mode):
     for l in range(R):
         assert all(drained[l][k][0] + len(drained[l][k][1]) == drained[l][k + 1][0] for k in range(len(drained[l]) - 1))
         assert drained[l][-1][0] + len(drained[l][-1][1]) > 8 * ring, "many wraps"
-        sg_ = parse_stream(drained[l], ring)
+        buf = np.concatenate([c[1] for c in drained[l]])
+        sg_ = [(h, im, p) for (h, im, p, _) in abi.parse_log(buf, ring, drained[l][0][0])]
         so_ = [(h, im, p) for (h, im, p, _) in abi.parse_log(eo.log_read(l))]
         assert len(sg_) == len(so_) > 0, (l, len(sg_), len(so_))
         for (ho, io_, po), (hg, ig, pg) in zip(so_, sg_):

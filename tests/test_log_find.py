@@ -18,7 +18,7 @@ import pytest
 import os as _os
 EMU_SANITIZE = ["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"] if _os.environ.get("GPX_EMU_SANITIZE") else []
 
-from helpers import ROOT, Engine, abi, group_descs, make_config, make_requests
+from helpers import ROOT, Engine, abi, group_descs, make_config, make_requests, relay_into_small_ring
 
 NODES = [100, 101, 102]
 
@@ -212,33 +212,6 @@ def test_kernel_source_on_the_host_equals_oracle(oracle_lib, emu_lib, seed, grid
     assert int(ctl[2]) == 3 and np.all(got["decision"]["flags"] == abi.F_VOID) and np.all(got["accept"]["flags"] == abi.F_VOID)
     got, ctl = emu_find(emu_lib, ring, cap, head + 2 * cap, 0, 2, wants)
     assert int(ctl[2]) == 1
-
-
-def relay_into_small_ring(buf, heads, cap):
-    """lay the calls of an (unwrapped) oracle ring image into a ring of `cap` bytes the way the device does: a call that
-    would straddle the ring end skips to the ring start (gpx_dev.cuh seg_base), later laps overwrite earlier ones, every
-    segment header names its new absolute position.  -> (ring bytes, new head, {old segment offset: new position},
-    [new position of every call])"""
-    ring = np.zeros(cap, dtype=np.uint8)
-    pos, seg_map, call_pos = 0, {}, []
-    for b0, b1 in zip(heads[:-1], heads[1:]):
-        n = b1 - b0
-        assert n <= cap
-        if (pos % cap) + n > cap:
-            pos += cap - pos % cap
-        call_pos.append(pos)
-        chunk = buf[b0:b1].copy()
-        off = 0
-        while off + 64 <= n:  # re-stamp ring_off of every segment of the call
-            hdr = chunk[off: off + 64].view(abi.seg_hdr_dtype)[0]
-            assert int(hdr["magic"]) == abi.SEG_MAGIC and int(hdr["ring_off"]) == b0 + off
-            seg_map[b0 + off] = pos + off
-            chunk[off: off + 64].view(abi.seg_hdr_dtype)[0]["ring_off"] = pos + off
-            off = (off + 64 + int(hdr["n_slots"]) * int(hdr["rec_bytes"]) + ((int(hdr["payload_bytes"]) + 15) & ~15) + 31) & ~31
-        assert off == n
-        ring[pos % cap: pos % cap + n] = chunk
-        pos += n
-    return ring, pos, seg_map, call_pos
 
 
 @pytest.mark.parametrize("seed", [6, 7])

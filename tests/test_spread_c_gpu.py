@@ -66,6 +66,7 @@ class Cluster:
         self.extra = [torch.zeros(4096 * 24, dtype=torch.uint8, device=self.dev) for _ in range(N)]
         self.status = [torch.zeros(4 * G, dtype=torch.int32, device=self.dev) for _ in range(N)]
         self.keep = []
+        self.drain = np.empty(int(self.engines[0].cfg.log_ring_bytes), dtype=np.uint8)
 
     def round(self, reqs, pay, fixed=None):
         """split the global batch by coordinator node and run one spread round; returns per node (status, exec)"""
@@ -179,6 +180,10 @@ def check_round(cl, res, index, so, xo):
         for f in ("gid", "slot", "req_id"):
             assert np.array_equal(want[f], got[f]), f"node {i} exec {f}"
         assert np.array_equal(want["flags"] & ~np.uint32(0xF000), got["flags"] & ~np.uint32(0xF000))
+    for i, e in enumerate(cl.engines):  # the host's mirror of the ring head (what a drain copies up to) follows the kernels
+        f, nb = e.log_drain_async(0, cl.drain.ctypes.data, len(cl.drain))
+        e.log_drain_wait()
+        assert f + nb == e.log_head(0), f"node {i}: ring head mirror"
 
 
 @pytest.mark.parametrize("N,G,P,graph,p2p", [(4, 600, 1, False, False), (3, 200, 40, False, False), (5, 333, 17, False, False),
