@@ -207,6 +207,9 @@ int gpx_engine_create(const gpx_config* cfg, gpx_engine** out) {
   if (!cfg || !out) return fail(GPX_EINVAL, "null argument");
   if (cfg->abi_version != GPX_ABI_VERSION) return fail(GPX_EINVAL, "abi_version mismatch");
   if (cfg->n_lanes == 0 || cfg->n_lanes > GPX_MAX_LANES) return fail(GPX_EINVAL, "n_lanes out of range");
+  for (uint32_t a = 0; a < cfg->n_lanes; a++) /* a node holds one instance of a group: one lane per node */
+    for (uint32_t b = a + 1; b < cfg->n_lanes; b++)
+      if (cfg->lane_node[a] == cfg->lane_node[b]) return fail(GPX_EINVAL, "two lanes serve the same node");
   if (cfg->window == 0 || cfg->window > GPX_MAX_WINDOW || (cfg->window & (cfg->window - 1)))
     return fail(GPX_EINVAL, "window must be 1,2,4 or 8");
   if (cfg->max_group_size == 0 || cfg->max_group_size > GPX_MAX_GROUP_SIZE)
@@ -364,8 +367,7 @@ void gpx_engine_destroy(gpx_engine* e) {
 /* ---- groups ----------------------------------------------------------------------- */
 static int names_drop(gpx_engine* e, uint32_t n, const uint32_t* gids, const uint8_t* only); /* gpx_wire_host.inc */
 
-static int intern_mset(gpx_engine* e, std::vector<int32_t> m, uint32_t* id, bool* added) {
-  std::sort(m.begin(), m.end()); /* PISM ctor sorts groupMembers :205 */
+static int intern_mset(gpx_engine* e, const std::vector<int32_t>& m, uint32_t* id) { /* m sorted */
   auto it = e->mset_ids.find(m);
   if (it != e->mset_ids.end()) {
     *id = it->second;
@@ -392,43 +394,67 @@ static int intern_mset(gpx_engine* e, std::vector<int32_t> m, uint32_t* id, bool
   *id = (uint32_t)e->msets.size();
   e->msets.push_back(mi);
   e->mset_ids[m] = *id;
-  *added = true;
   return GPX_OK;
 }
-static int push_msets(gpx_engine* e) {
-  CK(cudaMemcpyAsync(e->d_msets, e->msets.data(), e->msets.size() * sizeof(MsetInfo), cudaMemcpyHostToDevice,
-                     e->stream));
+/* the members of one group desc or row, sorted (PISM ctor sorts groupMembers :205); a node listed twice is refused:
+ * groupMembers is a set, and a node holds one instance of a group */
+static int sorted_members(const int32_t* members, int32_t n, std::vector<int32_t>* m) {
+  m->assign(members, members + n);
+  std::sort(m->begin(), m->end());
+  if (std::adjacent_find(m->begin(), m->end()) != m->end()) return fail(GPX_ERANGE, "a member is listed twice");
   return GPX_OK;
+}
+/* a call interns its member sets all or none: the sets it added since the table held n0 are uploaded when it succeeds
+ * and forgotten when it is refused, so the device copy always holds exactly the host table (the kernels index it
+ * with the ids recorded in grp_meta) */
+static int end_msets(gpx_engine* e, size_t n0, int rc) {
+  if (rc == GPX_OK && e->msets.size() > n0) {
+    cudaError_t err = cudaMemcpyAsync(e->d_msets + n0, e->msets.data() + n0, (e->msets.size() - n0) * sizeof(MsetInfo),
+                                      cudaMemcpyHostToDevice, e->stream);
+    if (err != cudaSuccess) rc = fail(GPX_ECUDA, cudaGetErrorString(err));
+  }
+  if (rc != GPX_OK) {
+    for (size_t i = n0; i < e->msets.size(); i++)
+      e->mset_ids.erase(std::vector<int32_t>(e->msets[i].nodes, e->msets[i].nodes + e->msets[i].R));
+    e->msets.resize(n0);
+  }
+  return rc;
 }
 
 int gpx_create_groups(gpx_engine* e, uint32_t n, const gpx_group_desc* d) {
   if (!e || (!d && n)) return fail(GPX_EINVAL, "null argument");
   if (n == 0) return GPX_OK;
   std::vector<InitRec> recs(n);
-  bool added = false;
+  const size_t n0 = e->msets.size();
+  int rc = GPX_OK;
   for (uint32_t k = 0; k < n; k++) {
-    if (d[k].gid >= e->cfg.max_groups) return fail(GPX_ERANGE, "gid >= max_groups");
-    if (d[k].n_members <= 0 || d[k].n_members > (int)e->cfg.max_group_size)
-      return fail(GPX_ERANGE, "group size exceeds max_group_size");
-    std::vector<int32_t> m(d[k].members, d[k].members + d[k].n_members);
-    std::sort(m.begin(), m.end());
-    uint32_t id;
-    int rc = intern_mset(e, m, &id, &added);
-    if (rc) return rc;
+    if (d[k].gid >= e->cfg.max_groups) {
+      rc = fail(GPX_ERANGE, "gid >= max_groups");
+      break;
+    }
+    if (d[k].n_members <= 0 || d[k].n_members > (int)e->cfg.max_group_size) {
+      rc = fail(GPX_ERANGE, "group size exceeds max_group_size");
+      break;
+    }
+    std::vector<int32_t> m;
+    uint32_t id = 0;
+    rc = sorted_members(d[k].members, d[k].n_members, &m);
+    if (rc == GPX_OK) rc = intern_mset(e, m, &id);
+    if (rc != GPX_OK) break;
     recs[k].gid = d[k].gid;
     recs[k].mset = id;
     recs[k].coord0 = gpx_round_robin_coordinator(d[k].name_hash, m.data(), (int32_t)m.size(), 0);
     recs[k].cpi = gpx_get_cpi(e->cfg.checkpoint_interval, e->cfg.cpi_noise, d[k].name_hash);
     recs[k].init_mode = d[k].init_mode;
     recs[k].R = (uint32_t)m.size();
+  }
+  rc = end_msets(e, n0, rc);
+  if (rc) return rc;
+  for (uint32_t k = 0; k < n; k++) {
     e->h_version[d[k].gid] = d[k].version;
     e->h_name_hash[d[k].gid] = d[k].name_hash;
   }
-  if (added) {
-    int rc = push_msets(e);
-    if (rc) return rc;
-  }
-  int rc = e->ensure_misc(n * sizeof(InitRec));
+  rc = e->ensure_misc(n * sizeof(InitRec));
   if (rc) return rc;
   CK(cudaMemcpyAsync(e->d_misc, recs.data(), n * sizeof(InitRec), cudaMemcpyHostToDevice, e->stream));
   k_init_groups<<<cdiv(n, 256), 256, 0, e->stream>>>(e->S, (const InitRec*)e->d_misc, n);
@@ -481,26 +507,34 @@ int gpx_load_rows(gpx_engine* e, uint32_t n, const gpx_row* rows) {
   if (!e || (!rows && n)) return fail(GPX_EINVAL, "null argument");
   if (n == 0) return GPX_OK;
   std::vector<LoadRec> recs(n);
-  bool added = false;
+  const size_t n0 = e->msets.size();
+  int rc = GPX_OK;
   for (uint32_t k = 0; k < n; k++) {
     const gpx_row& r = rows[k];
-    if (r.gid >= e->cfg.max_groups || r.lane >= e->cfg.n_lanes) return fail(GPX_ERANGE, "gid/lane");
-    if (r.n_members <= 0 || r.n_members > (int)e->cfg.max_group_size) return fail(GPX_ERANGE, "n_members");
-    std::vector<int32_t> m(r.members, r.members + r.n_members);
-    uint32_t id;
-    int rc = intern_mset(e, m, &id, &added);
-    if (rc) return rc;
+    if (r.gid >= e->cfg.max_groups || r.lane >= e->cfg.n_lanes) {
+      rc = fail(GPX_ERANGE, "gid/lane");
+      break;
+    }
+    if (r.n_members <= 0 || r.n_members > (int)e->cfg.max_group_size) {
+      rc = fail(GPX_ERANGE, "n_members");
+      break;
+    }
+    std::vector<int32_t> m;
+    uint32_t id = 0;
+    rc = sorted_members(r.members, r.n_members, &m);
+    if (rc == GPX_OK) rc = intern_mset(e, m, &id);
+    if (rc != GPX_OK) break;
     recs[k].row = r;
     recs[k].mset = id;
     recs[k].cpi = gpx_get_cpi(e->cfg.checkpoint_interval, e->cfg.cpi_noise, r.name_hash); /* getCPI(paxosID) */
-    e->h_version[r.gid] = r.version;
-    e->h_name_hash[r.gid] = r.name_hash;
   }
-  if (added) {
-    int rc = push_msets(e);
-    if (rc) return rc;
+  rc = end_msets(e, n0, rc);
+  if (rc) return rc;
+  for (uint32_t k = 0; k < n; k++) {
+    e->h_version[rows[k].gid] = rows[k].version;
+    e->h_name_hash[rows[k].gid] = rows[k].name_hash;
   }
-  int rc = e->ensure_misc(n * sizeof(LoadRec));
+  rc = e->ensure_misc(n * sizeof(LoadRec));
   if (rc) return rc;
   CK(cudaMemcpyAsync(e->d_misc, recs.data(), n * sizeof(LoadRec), cudaMemcpyHostToDevice, e->stream));
   k_load_rows<<<cdiv(n, 128), 128, 0, e->stream>>>(e->S, (const LoadRec*)e->d_misc, n);

@@ -241,7 +241,8 @@ typedef struct gpx_group_desc {
   int32_t version;
   int32_t name_hash; /* Java String.hashCode() of the paxosID */
   int32_t n_members;
-  int32_t members[GPX_MAX_GROUP_SIZE]; /* node ids, any order (sorted by the engine) */
+  int32_t members[GPX_MAX_GROUP_SIZE]; /* distinct node ids, any order (sorted by the engine); a call with a
+                                        * node listed twice is refused (GPX_ERANGE) and changes nothing */
   int32_t init_mode;                   /* GPX_INIT_* */
 } gpx_group_desc;
 
@@ -271,7 +272,7 @@ typedef struct gpx_config {
   int32_t device;            /* CUDA device ordinal */
   uint32_t max_groups;       /* PINSTANCES_CAPACITY analogue: rows per lane */
   uint32_t n_lanes;          /* co-located replicas */
-  int32_t lane_node[GPX_MAX_LANES]; /* node id served by each lane */
+  int32_t lane_node[GPX_MAX_LANES]; /* node id served by each lane, distinct (GPX_EINVAL otherwise) */
   uint32_t window;           /* W: 1,2,4,8 */
   uint32_t max_group_size;   /* <= GPX_MAX_GROUP_SIZE: node_slots columns allocated */
   uint64_t log_ring_bytes;   /* per lane, power of two; 0 => logging disabled (DISABLE_LOGGING) */

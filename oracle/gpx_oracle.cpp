@@ -44,6 +44,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -577,6 +578,7 @@ struct gpxo_engine {
   std::vector<Group> groups;
   std::vector<Lane> lanes;
   gpx_counters ctr;
+  std::set<std::vector<i32>> msets; /* the distinct sorted member sets seen (the engine's table holds GPX_MAX_MSETS) */
   u32 L() const { return cfg.n_lanes; }
   int W() const { return (int)cfg.window; }
 
@@ -708,6 +710,10 @@ void gpxo_config_defaults(gpx_config* c) {
 int gpxo_engine_create(const gpx_config* cfg, gpxo_engine** out) {
   if (!cfg || !out || cfg->abi_version != GPX_ABI_VERSION) return GPX_EINVAL;
   if (cfg->n_lanes == 0 || cfg->n_lanes > GPX_MAX_LANES) return GPX_EINVAL;
+  if (cfg->max_group_size == 0 || cfg->max_group_size > GPX_MAX_GROUP_SIZE) return GPX_EINVAL;
+  for (u32 a = 0; a < cfg->n_lanes; a++) /* a node holds one instance of a group: one lane per node */
+    for (u32 b = a + 1; b < cfg->n_lanes; b++)
+      if (cfg->lane_node[a] == cfg->lane_node[b]) return GPX_EINVAL;
   if (cfg->window != 0 && (cfg->window > GPX_MAX_WINDOW || (cfg->window & (cfg->window - 1)))) return GPX_EINVAL;
   gpxo_engine* e = new gpxo_engine();
   e->cfg = *cfg;
@@ -724,17 +730,47 @@ int gpxo_engine_create(const gpx_config* cfg, gpxo_engine** out) {
 }
 void gpxo_engine_destroy(gpxo_engine* e) { delete e; }
 
+/* what gpx_create_groups / gpx_load_rows check, for every record of a call before any is applied (a refused call
+ * changes nothing): gid and lane in range, 1..max_group_size members, none listed twice (PISM.groupMembers is a set,
+ * sorted by the ctor :205), and at most GPX_MAX_MSETS distinct member sets per engine.  -> every record's sorted member
+ * list */
+struct MemberRec {
+  u32 gid, lane;
+  i32 n_members;
+  const i32* members;
+};
+static int checkMembers(gpxo_engine* e, const std::vector<MemberRec>& recs, std::vector<std::vector<i32>>* sorted) {
+  std::set<std::vector<i32>> fresh;
+  sorted->resize(recs.size());
+  for (size_t k = 0; k < recs.size(); k++) {
+    const MemberRec& r = recs[k];
+    if (r.gid >= e->cfg.max_groups || r.lane >= e->L() || r.n_members <= 0 || r.n_members > (i32)e->cfg.max_group_size)
+      return GPX_ERANGE;
+    std::vector<i32>& m = (*sorted)[k];
+    m.assign(r.members, r.members + r.n_members);
+    std::sort(m.begin(), m.end());
+    if (std::adjacent_find(m.begin(), m.end()) != m.end()) return GPX_ERANGE;
+    if (!e->msets.count(m)) fresh.insert(m);
+  }
+  if (e->msets.size() + fresh.size() > GPX_MAX_MSETS) return GPX_ERANGE;
+  e->msets.insert(fresh.begin(), fresh.end());
+  return GPX_OK;
+}
+
 /* PaxosManager.createPaxosInstance(Map,Set) :664-691 -> HotRestoreInfo.createHRI :145-157 (GPX_INIT_BATCH)
  * or PISM.initiateRecovery :591-675 + putInitialState :692-699 (GPX_INIT_DEFAULT) */
 int gpxo_create_groups(gpxo_engine* e, uint32_t n, const gpx_group_desc* d) {
+  std::vector<MemberRec> recs(n);
+  for (u32 k = 0; k < n; k++) recs[k] = MemberRec{d[k].gid, 0, d[k].n_members, d[k].members};
+  std::vector<std::vector<i32>> sorted;
+  int rc = checkMembers(e, recs, &sorted);
+  if (rc) return rc;
   for (u32 k = 0; k < n; k++) {
-    if (d[k].gid >= e->cfg.max_groups || d[k].n_members <= 0 || d[k].n_members > GPX_MAX_GROUP_SIZE) return GPX_ERANGE;
     Group& g = e->groups[d[k].gid];
     g.live = true;
     g.version = d[k].version;
     g.name_hash = d[k].name_hash;
-    g.members.assign(d[k].members, d[k].members + d[k].n_members);
-    std::sort(g.members.begin(), g.members.end());
+    g.members = sorted[k];
     g.cpi = getCPI(e->cfg.checkpoint_interval, e->cfg.cpi_noise, g.name_hash);
     i32 coord0 = roundRobinCoordinator(g.name_hash, g.members.data(), (i32)g.members.size(), 0);
     for (u32 l = 0; l < e->L(); l++) {
@@ -822,17 +858,19 @@ int gpxo_dump_rows(gpxo_engine* e, uint32_t n, const uint32_t* gids, uint32_t la
 }
 
 int gpxo_load_rows(gpxo_engine* e, uint32_t n, const gpx_row* rows) {
+  std::vector<MemberRec> recs(n);
+  for (u32 k = 0; k < n; k++) recs[k] = MemberRec{rows[k].gid, rows[k].lane, rows[k].n_members, rows[k].members};
+  std::vector<std::vector<i32>> sorted;
+  int rc = checkMembers(e, recs, &sorted);
+  if (rc) return rc;
   for (u32 k = 0; k < n; k++) {
     const gpx_row& r = rows[k];
-    if (r.gid >= e->cfg.max_groups || r.lane >= e->L() || r.n_members <= 0 || r.n_members > GPX_MAX_GROUP_SIZE)
-      return GPX_ERANGE;
     Group& g = e->groups[r.gid];
     g.live = true;
     g.version = r.version;
     g.name_hash = r.name_hash; /* HotRestoreInfo carries the paxosID: getCPI :2694-2697 follows the name, not the gid */
     g.cpi = getCPI(e->cfg.checkpoint_interval, e->cfg.cpi_noise, g.name_hash);
-    g.members.assign(r.members, r.members + r.n_members);
-    std::sort(g.members.begin(), g.members.end());
+    g.members = sorted[k];
     Acceptor& A = e->lanes[r.lane].acc[r.gid];
     Coordinator& C = e->lanes[r.lane].coord[r.gid];
     A = Acceptor();
