@@ -60,6 +60,8 @@ req_meta_dtype = np.dtype([("client_ip", "u1", (4,)), ("client_port", "<u2"), ("
 assert req_meta_dtype.itemsize == 32
 # gpx_wire_member: one member of a JSON packet (gpx_wire_decode_json_device)
 wire_member_dtype = np.dtype([("pkt", "<u4"), ("off", "<u4"), ("len", "<u4"), ("status", "<i4")])
+# gpx_wire_encode_json_device: a wrapper's default and largest size, its head + tail, the largest member object
+GPX_JSON_WRAP_BYTES, GPX_JSON_WRAP_OVERHEAD, GPX_JSON_MAX_MEMBER = 4 << 20, 34, 65536
 accepted_pvalue_dtype = np.dtype([("slot", "<i4"), ("bnum", "<i4"), ("bcoord", "<i4"), ("frame_ref", "<u4"),
                                   ("req_id", "<i8"), ("payload_len", "<u4"), ("flags", "<u4")])
 prepare_reply_dtype = np.dtype([("gid", "<u4"), ("first_slot", "<i4"), ("bnum", "<i4"), ("bcoord", "<i4"), ("who", "<u4"),

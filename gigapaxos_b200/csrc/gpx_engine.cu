@@ -28,6 +28,7 @@
 #include "gpx_logfind.cuh"
 #include "gpx_wire_dev.cuh"
 #include "gpx_wire_json.cuh"
+#include "gpx_wire_json_enc.cuh"
 #include "gpx_wire_fwd.cuh"
 
 #include <cub/cub.cuh>
@@ -130,6 +131,10 @@ struct gpx_engine {
   size_t wire_io_bytes = 0;
   cudaEvent_t ev_wire = nullptr; /* the last wire call's work on its stream: the next call, on any stream, waits for it */
   bool wire_pending = false;
+  /* the JSON encoder's recipient sets (gpx_wire_encode_json_device), allocated by its first call */
+  JsonSetTable jsets;
+  JsonSets d_jsets{};
+  size_t jsets_up = 0; /* member sets the device copy covers */
 
   template <typename T>
   int dalloc(T** p, size_t n) {

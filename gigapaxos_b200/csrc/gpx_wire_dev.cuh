@@ -662,6 +662,16 @@ struct WireEncodeArgs {
   const uint32_t* n_ptr; /* decisions: records [*n_ptr, n) are not read and get no rstatus (device count); null = n */
 };
 
+/* where a reply that is neither void nor a NACK goes: GPX_WE_VOID (its group is gone, or a member index is out of
+ * range), GPX_WE_LOCAL (a local lane serves its destination: SHORT_CIRCUIT_LOCAL), GPX_WE_NO_NAME, else GPX_WE_SENT.
+ * The JSON encoder (gpx_wire_json_enc.cuh) routes a NACK by the same rule. */
+__device__ __forceinline__ uint8_t wire_reply_route(const DevState& S, const WireNames& W, const gpx_accept_reply_rec& x,
+                                                    const GroupCtx& g) {
+  if (!g.live || GPX_WHO_DST(x.who) >= g.R || GPX_WHO_ACC(x.who) >= g.R) return GPX_WE_VOID;
+  if (g.ms->lane_of_idx[GPX_WHO_DST(x.who)] != 0xffu) return GPX_WE_LOCAL;
+  if (W.slot == nullptr || W.slot[x.gid] == GPX_NAME_NONE) return GPX_WE_NO_NAME;
+  return GPX_WE_SENT;
+}
 /* one thread per record: what happens to it and its sort key */
 __global__ void k_wire_enc_keys_replies(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
                                         const __grid_constant__ WireEncodeArgs A) {
@@ -669,13 +679,11 @@ __global__ void k_wire_enc_keys_replies(const __grid_constant__ DevState S, cons
   if (i >= A.n) return;
   const gpx_accept_reply_rec x = reinterpret_cast<const gpx_accept_reply_rec*>(A.recs)[i];
   const uint32_t fl = GPX_WHO_FLAGS(x.who), lane = i % A.n_lanes;
-  uint8_t st = GPX_WE_SENT;
+  uint8_t st;
   const GroupCtx g = group_ctx(S, x.gid);
   if (fl & GPX_F_VOID) st = GPX_WE_VOID;
-  else if (fl & GPX_F_NACK) st = GPX_WE_NACK; /* allPositiveAcceptReplies :423-430: the host sends it alone */
-  else if (!g.live || GPX_WHO_DST(x.who) >= g.R || GPX_WHO_ACC(x.who) >= g.R) st = GPX_WE_VOID;
-  else if (g.ms->lane_of_idx[GPX_WHO_DST(x.who)] != 0xffu) st = GPX_WE_LOCAL; /* SHORT_CIRCUIT_LOCAL */
-  else if (W.slot == nullptr || W.slot[x.gid] == GPX_NAME_NONE) st = GPX_WE_NO_NAME;
+  else if (fl & GPX_F_NACK) st = GPX_WE_NACK; /* allPositiveAcceptReplies :423-430: never coalesced */
+  else st = wire_reply_route(S, W, x, g);
   A.rstatus[i] = st;
   A.key[i] = st == GPX_WE_SENT ? lane * S.G + x.gid : GPX_WIRE_NOKEY;
 }
@@ -744,10 +752,10 @@ __device__ __forceinline__ bool wire_run(const WireEncodeArgs& A, uint32_t p, ui
   return true;
 }
 
-/* the run's distinct slots in ascending signed order (TreeMap / TreeSet); `last` = sorted position of the entry that
- * wins a repeated slot (the last put).  Returns the number of distinct slots; with out != nullptr writes them. */
-template <typename T, bool WITH_REQ>
-__device__ __forceinline__ uint32_t wire_slots(const WireEncodeArgs& A, uint32_t p, uint32_t end, uint8_t* out) {
+/* the run's distinct slots in ascending signed order (TreeMap / TreeSet): each(k, slot, bi) for the k-th of them, bi =
+ * sorted position of the entry that wins a repeated slot (the last put).  Returns the number of distinct slots. */
+template <typename T, typename Each>
+__device__ __forceinline__ uint32_t wire_slots_each(const WireEncodeArgs& A, uint32_t p, uint32_t end, Each each) {
   const T* recs = reinterpret_cast<const T*>(A.recs);
   uint32_t n = 0;
   bool have = false;
@@ -766,16 +774,24 @@ __device__ __forceinline__ uint32_t wire_slots(const WireEncodeArgs& A, uint32_t
       }
     }
     if (!found) break;
-    if (out) {
-      uint8_t* o = out + (size_t)n * (WITH_REQ ? 12u : 4u);
-      ww_i32(o, best);
-      if (WITH_REQ) ww_i64(o + 4, reinterpret_cast<const gpx_accept_reply_rec*>(recs)[A.perm[bi]].req_id);
-    }
+    each(n, best, bi);
     n++;
     have = true;
     prev = best;
   }
   return n;
+}
+/* wire_slots_each writing the slots (and a reply's requestIDs) as big-endian words; out == nullptr only counts */
+template <typename T, bool WITH_REQ>
+__device__ __forceinline__ uint32_t wire_slots(const WireEncodeArgs& A, uint32_t p, uint32_t end, uint8_t* out) {
+  const T* recs = reinterpret_cast<const T*>(A.recs);
+  return wire_slots_each<T>(A, p, end, [&](uint32_t n, int32_t best, uint32_t bi) {
+    if (out) {
+      uint8_t* o = out + (size_t)n * (WITH_REQ ? 12u : 4u);
+      ww_i32(o, best);
+      if (WITH_REQ) ww_i64(o + 4, reinterpret_cast<const gpx_accept_reply_rec*>(recs)[A.perm[bi]].req_id);
+    }
+  });
 }
 
 /* one thread per sorted position; a position that starts a (lane, gid, ballot) run writes one BatchedAcceptReply
@@ -838,6 +854,17 @@ __device__ __forceinline__ void wire_refs_remote(const WireEncodeArgs& A, uint32
   }
 }
 
+/* the wrap-aware maximum medianCheckpointedSlot of the decision run [p, end) (BatchedCommit.addCommit :113-121) */
+__device__ __forceinline__ int32_t wire_run_median(const WireEncodeArgs& A, uint32_t p, uint32_t end) {
+  const gpx_decision_rec* recs = reinterpret_cast<const gpx_decision_rec*>(A.recs);
+  int32_t median = recs[A.perm[p]].median_cp;
+  for (uint32_t q = p + 1; q < end; q++) {
+    const int32_t m = recs[A.perm[q]].median_cp;
+    if (jsub(m, median) > 0) median = m;
+  }
+  return median;
+}
+
 /* one thread per sorted position; a position that starts a (gid, ballot) run writes one BatchedCommit
  * (PaxosPacketBatcher.fuseBatchedCommits :389-417, BatchedCommit.addCommit :113-121: medianCheckpointedSlot is the
  * wrap-aware maximum, gpx_wire_fuse_commits' rule), stored once and indexed once per member node that no local lane
@@ -864,11 +891,7 @@ __global__ void k_wire_enc_decisions(const __grid_constant__ DevState S, const _
   }
   if (!head) return;
   const gpx_decision_rec d = recs[A.perm[p]];
-  int32_t median = d.median_cp;
-  for (uint32_t q = p + 1; q < end; q++) {
-    const int32_t m = recs[A.perm[q]].median_cp;
-    if (jsub(m, median) > 0) median = m;
-  }
+  const int32_t median = wire_run_median(A, p, end);
   uint8_t* o = A.out + A.off[p];
   uint32_t b = ww_header(o, GPX_PT_BATCHED_COMMIT, W, d.gid);
   ww_i32(o + b, d.bnum);

@@ -430,6 +430,35 @@ def decode_json_device(engine, arena, refs, caps, stream=None) -> JsonOut:
     return JsonOut(status[:n], mem[: caps[0]], rep[: caps[1]], dec[: caps[2]], caps)
 
 
+JsonEncodeOut = namedtuple("JsonEncodeOut", "rstatus_replies rstatus_decisions out refs sizes")
+
+
+def encode_json_device(engine, replies, n_replies: int, decisions, n_dec_ptr: Optional[int], n_dec_max: int, caps,
+                       wrap_bytes: int = 0, stream=None) -> JsonEncodeOut:
+    """gpx_wire_encode_json_device: the first n_replies records of `replies` (gpx_accepts_device's layout) and the
+    decisions (count read on the device at address n_dec_ptr, at most n_dec_max; None = n_dec_max) as the JSON a loaded
+    Java node sends -- BATCHED_PAXOS_PACKET wrappers of at most wrap_bytes (0 = 4 MiB) per recipient set, each NACK a
+    bare ACCEPT_REPLY.  Either tensor may be None when its count is 0.  caps = (packet bytes, refs); GPX_ERANGE as in
+    decode_batch_device.  Returns both rstatus arrays (uint8), the packet arena, refs [k, 16] (a wrapper's gid column
+    is its sending lane) and the two host sizes."""
+    import torch
+    dev = (replies if replies is not None else decisions).device
+    L, st = engine.L, stream_handle(stream)
+    with _on(stream):
+        rr = torch.empty(max(n_replies, 1), dtype=torch.uint8, device=dev)
+        rd = torch.empty(max(n_dec_max, 1), dtype=torch.uint8, device=dev)
+        (out, refs), caps = _sized(
+            engine, caps, (C.c_uint64, C.c_uint32),
+            lambda c: (torch.empty(max(c[0], 1), dtype=torch.uint8, device=dev),
+                       torch.empty((max(c[1], 1), 16), dtype=torch.uint8, device=dev)),
+            lambda o, sz: L.fn("wire_encode_json_device")(engine.handle, C.c_uint32(n_replies), _dptr(replies),
+                                                          _dptr(decisions), C.c_void_p(n_dec_ptr) if n_dec_ptr else None,
+                                                          C.c_uint32(n_dec_max), _dptr(rr), _dptr(rd),
+                                                          C.c_uint64(wrap_bytes), _dptr(o[0]), sz[0], _dptr(o[1]),
+                                                          sz[1], st))
+    return JsonEncodeOut(rr[:n_replies], rd[:n_dec_max], out[: caps[0]], refs[: caps[1]], caps)
+
+
 # ---- the coordinator's side: REQUEST packets -> proposals -> ACCEPT packets, on the device ---------------------------
 RequestsOut = namedtuple("RequestsOut", "status reqs meta payload sizes")
 

@@ -1024,6 +1024,58 @@ int gpx_wire_decode_json_device(gpx_engine* e, uint32_t n, const uint8_t* bytes,
                                 uint32_t* n_members, gpx_accept_reply_rec* replies, uint32_t* n_replies,
                                 gpx_decision_rec* decisions, uint32_t* n_decisions, void* stream);
 
+/* The sending side: a node's replies and commits as a loaded Java node sends them.
+ *   GPX_JSON_WRAP_BYTES     a wrapper's default and largest size (4 MiB)
+ *   GPX_JSON_WRAP_OVERHEAD  the bytes of a wrapper that are not its members or the commas between them:
+ *                           {"type":90,"PT":37,"V":-1,"PP":[ and ]}
+ *   GPX_JSON_MAX_MEMBER     the largest member object the call writes; a BatchedAcceptReply of up to 1,800 distinct
+ *                           slots, or a BatchedCommit of up to 5,000, is always below it */
+#define GPX_JSON_WRAP_BYTES 4194304u
+#define GPX_JSON_WRAP_OVERHEAD 34u
+#define GPX_JSON_MAX_MEMBER 65536u
+
+/* Encode replies (gpx_handle_accepts' layout, record i * n_lanes + lane, n_replies a multiple of n_lanes) and
+ * decisions (n_dec_ptr: a device count, at most n_dec_max, as in gpx_wire_encode_decisions_device; NULL = n_dec_max)
+ * as the JSON a loaded Java node sends: BATCHED_PAXOS_PACKET wrappers (PaxosPacketBatcher.batch :280-303) of
+ * BatchedAcceptReply and BatchedCommit objects, and each NACK as a bare ACCEPT_REPLY.  Either input may be empty.
+ * The caller sends a sweep of at most MIN_PP_BATCH_SIZE (3) packets unwrapped (PaxosPacketBatcher.process :270-277),
+ * with gpx_wire_encode_replies_device and gpx_wire_encode_decisions_device; this call always wraps.
+ *   rstatus_replies[n_replies], rstatus_decisions[below the count]  the byte encoders' GPX_WE_* from the same rules,
+ *     except for a reply with GPX_F_NACK: GPX_WE_NACK when it is written here as a bare ACCEPT_REPLY (its destination
+ *     is a member no local lane serves, the group is live and named), else GPX_WE_LOCAL, GPX_WE_VOID or
+ *     GPX_WE_NO_NAME as a positive reply would be.  NACKs are never wrapped (PaxosPacketBatcher.coalesce :345-387).
+ *   Members: one BatchedAcceptReply per (lane, gid, ballot) run of GPX_WE_SENT replies, with the byte encoder's header
+ *     (the run's first reply) and SLOTS = [slot, requestID, ...] ascending, the last put of a slot winning; one
+ *     BatchedCommit per (gid, ballot) run of GPX_WE_SENT decisions with the wrap-aware maximum GC_S, GROUP = every
+ *     member node in the member-set order, SLOTS ascending and distinct.  Each object, and each bare ACCEPT_REPLY
+ *     (SNDR = the member node of WHO_ACC, S, CP_S and QID from the record), is byte-identical to packets_json's
+ *     batched_accept_reply_json / batched_commit_json / accept_reply_json: keys in their order, "," and ":" with no
+ *     spaces, strings escaped as json.dumps escapes them (\" \\ \b \f \n \r \t; every other byte below 0x20 and
+ *     every byte from 0x7f up as \u00xx, lowercase).
+ *   Sender and recipients: a reply is sent from lane i % n_lanes to the node of WHO_DST; a commit from the lane serving
+ *     its ballot coordinator (else the group's lowest local lane, lane 0 when it has none) to every member node no
+ *     local lane serves.  Recipient sets are compared as sets of node ids.
+ *   Wrappers: each lane, ascending, sweeps its reply members in (gid, run) order, then its commit members in gid
+ *     order (PaxosPacketBatcher.dequeueImpl :182-209).  Its members are grouped by recipient set in order of first
+ *     appearance (the LinkedHashMap of batch :281-296), sweep order within a group.  A group is cut in parallel: with
+ *     start_j the offset of member j in the group's comma-joined member stream and T = wrap_bytes -
+ *     GPX_JSON_WRAP_OVERHEAD - GPX_JSON_MAX_MEMBER, member j opens a new wrapper iff floor(start_j / T) differs from
+ *     its predecessor's, so no wrapper exceeds wrap_bytes.  A wrapper is {"type":90,"PT":37,"V":-1,"PP":[...]}.
+ *     wrap_bytes = 0 means GPX_JSON_WRAP_BYTES; a value above it or at most GPX_JSON_WRAP_OVERHEAD +
+ *     GPX_JSON_MAX_MEMBER is GPX_EINVAL.
+ *   out[*out_bytes]  every packet once: the bare ACCEPT_REPLYs in record order, then the wrappers in (lane, first-seen
+ *     recipient set, cut) order.
+ *   refs[*n_refs]  one {off, len, gid, node} per (packet, recipient node), nodes ascending within a packet, in the
+ *     order of out.  gid is the group for a bare ACCEPT_REPLY and the SENDING LANE for a wrapper.
+ * replies, decisions, n_dec_ptr, rstatus_*, out and refs are device pointers; *out_bytes and *n_refs are HOST pointers,
+ * capacities in / sizes out, and GPX_ERANGE reports the sizes and writes no packet.  A member larger than
+ * GPX_JSON_MAX_MEMBER makes the call GPX_EINVAL with no packet written.  Stream-ordered on `stream` (NULL = the
+ * engine's stream) with the other wire calls' scratch; one synchronisation reads the totals. */
+int gpx_wire_encode_json_device(gpx_engine* e, uint32_t n_replies, const gpx_accept_reply_rec* replies,
+                                const gpx_decision_rec* decisions, const uint32_t* n_dec_ptr, uint32_t n_dec_max,
+                                uint8_t* rstatus_replies, uint8_t* rstatus_decisions, uint64_t wrap_bytes,
+                                uint8_t* out, uint64_t* out_bytes, gpx_wire_ref* refs, uint32_t* n_refs, void* stream);
+
 /* ---- the coordinator's side: REQUEST packets in, ACCEPT packets out ---------------------------------------------
  * A RequestPacket reaches the coordinator as REQUEST bytes (PaxosPacket type 1), from a client or forwarded by another
  * replica (PISM.handleProposal :854-885), and leaves inside the coordinator's AcceptPacket, which carries the whole
