@@ -83,6 +83,7 @@ struct gpx_engine {
   int round_mode = 0;         /* gpx_set_round_mode: 0 / 1 device tail launch of k_round_slow, 2 host-launched pair;
                                * 3 / 4 the same two with the team kernel k_round in place of k_round_g */
   uint32_t rparity = 0;
+  bool ls_live = false; /* a k_round_g<L, true> launch may have left VALID lockstep records (ls_settle) */
   RoundCtl* h_ctl = nullptr; /* pinned */
   void* d_misc = nullptr;    /* group-management staging */
   size_t misc_bytes = 0;
@@ -248,7 +249,9 @@ int gpx_engine_create(const gpx_config* cfg, gpx_engine** out) {
     gpx_engine_destroy(e);\
     return rc;            \
   }
-  TRY(e->dalloc(&S.acc_row, L * G));
+  /* k_round_g's lockstep records (gpx_dev.cuh) follow the acceptor rows, 32-byte aligned (cudaMalloc: 256) */
+  if (L <= GPX_GROUND_MAXL) S.ls_off = (uint32_t)((L * G + 1) & ~(size_t)1);
+  TRY(e->dalloc(&S.acc_row, S.ls_off ? S.ls_off + 2 * G : L * G));
   TRY(e->dalloc(&S.acc_aux, L * G));
   TRY(e->dalloc(&S.acc_win, 2 * L * W * G));
   TRY(e->dalloc(&S.acc_dirty, L * G));
@@ -286,6 +289,7 @@ int gpx_engine_create(const gpx_config* cfg, gpx_engine** out) {
     cudaMemset(S.com_win, 0, 2 * L * W * G * sizeof(int4));
     cudaMemset(S.prop_win, 0, L * W * G * sizeof(int4));
     cudaMemset(S.ns_u, 0, L * G * 4); /* compact, 0: what group creation writes */
+    if (S.ls_off) cudaMemset(S.acc_row + S.ls_off, 0, 2 * G * sizeof(int4));
   }
   for (size_t l = 0; l < GPX_MAX_LANES; l++) S.lane_node[l] = l < L ? cfg->lane_node[l] : INT32_MIN;
   S.cpi_const = cfg->checkpoint_interval;
@@ -371,6 +375,7 @@ void gpx_engine_destroy(gpx_engine* e) {
 
 /* ---- groups ----------------------------------------------------------------------- */
 static int names_drop(gpx_engine* e, uint32_t n, const uint32_t* gids, const uint8_t* only); /* gpx_wire_host.inc */
+static void ls_settle(gpx_engine* e, cudaStream_t st); /* lockstep records back into the planes, below */
 
 static int intern_mset(gpx_engine* e, const std::vector<int32_t>& m, uint32_t* id) { /* m sorted */
   auto it = e->mset_ids.find(m);
@@ -462,6 +467,7 @@ int gpx_create_groups(gpx_engine* e, uint32_t n, const gpx_group_desc* d) {
   rc = e->ensure_misc(n * sizeof(InitRec));
   if (rc) return rc;
   CK(cudaMemcpyAsync(e->d_misc, recs.data(), n * sizeof(InitRec), cudaMemcpyHostToDevice, e->stream));
+  ls_settle(e, e->stream);
   k_init_groups<<<cdiv(n, 256), 256, 0, e->stream>>>(e->S, (const InitRec*)e->d_misc, n);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(e->stream));
@@ -481,6 +487,7 @@ int gpx_destroy_groups(gpx_engine* e, uint32_t n, const uint32_t* gids) {
   for (uint32_t k = 0; k < n; k++)
     if (gids[k] < e->cfg.max_groups) e->h_name_hash[gids[k]] = e->h_version[gids[k]] = 0;
   CK(cudaMemcpyAsync(e->d_misc, gids, n * 4ull, cudaMemcpyHostToDevice, e->stream));
+  ls_settle(e, e->stream);
   k_destroy_groups<<<cdiv(n, 256), 256, 0, e->stream>>>(e->S, (const uint32_t*)e->d_misc, n);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(e->stream));
@@ -496,6 +503,7 @@ int gpx_dump_rows(gpx_engine* e, uint32_t n, const uint32_t* gids, uint32_t lane
   if (rc) return rc;
   uint32_t* d_g = (uint32_t*)((uint8_t*)e->d_misc + goff);
   CK(cudaMemcpyAsync(d_g, gids, n * 4ull, cudaMemcpyHostToDevice, e->stream));
+  ls_settle(e, e->stream);
   k_dump_rows<<<cdiv(n, 128), 128, 0, e->stream>>>(e->S, d_g, n, lane, (gpx_row*)e->d_misc);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out, e->d_misc, n * sizeof(gpx_row), cudaMemcpyDeviceToHost, e->stream));
@@ -542,6 +550,7 @@ int gpx_load_rows(gpx_engine* e, uint32_t n, const gpx_row* rows) {
   rc = e->ensure_misc(n * sizeof(LoadRec));
   if (rc) return rc;
   CK(cudaMemcpyAsync(e->d_misc, recs.data(), n * sizeof(LoadRec), cudaMemcpyHostToDevice, e->stream));
+  ls_settle(e, e->stream);
   k_load_rows<<<cdiv(n, 128), 128, 0, e->stream>>>(e->S, (const LoadRec*)e->d_misc, n);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(e->stream));
@@ -580,6 +589,7 @@ int gpx_patch(gpx_engine* e, uint32_t n, const gpx_patch_rec* p) {
     }
     CK(cudaMemcpyAsync(e->d_misc, wave.data(), wave.size() * sizeof(gpx_patch_rec), cudaMemcpyHostToDevice,
                        e->stream));
+    ls_settle(e, e->stream);
     k_patch<<<cdiv(wave.size(), 128), 128, 0, e->stream>>>(e->S, (const gpx_patch_rec*)e->d_misc,
                                                             (uint32_t)wave.size());
     CK(cudaGetLastError());
@@ -596,10 +606,32 @@ static uint64_t round_blob1(const gpx_engine* e, uint32_t n, uint64_t pal) {
 /* every launch that appends to the log reads log_pos[lp] and writes log_pos[lp ^ 1]: flip after the launch */
 static inline void log_flip(gpx_engine* e) { e->S.lp ^= 1u; }
 
+/* ---- lockstep records (ls_rec, gpx_dev.cuh) ------------------------------------------------------------------
+ * k_round_g<L, true> keeps a group whose lanes advance in lockstep as one record and leaves the group's acc_row,
+ * coord_row[cl] and ns_u[cl] words stale.  Every other launch that reads or writes group state is preceded by
+ * ls_settle on its own stream, which writes the VALID records back once after the last such round.  These settle:
+ *   - the launch helpers below (propose, accept / act, tally, commit) and a round that does not run
+ *     k_round_g<L, true> (launch_round; round_on_stream settles ahead of its timing events);
+ *   - prepares and prepare replies, create, destroy, patch, dump / load rows, get / select / clear group flags,
+ *     missing decisions, pause, unpause and spread rounds.
+ * Calls that touch only the log rings, counters, group names or wire bytes do not. */
+static bool def_config(const DevState& S) { /* the reference's default configuration: k_round*<..., DEF = true> */
+  return S.journaling && S.gc_majority_executed && S.log_meta && !S.cpi_per_group;
+}
+static bool round_uses_ls(const gpx_engine* e) {
+  return e->S.ls_off && e->round_mode < 3 && def_config(e->S);
+}
+static void ls_settle(gpx_engine* e, cudaStream_t st) {
+  if (!e->ls_live) return;
+  e->ls_live = false;
+  k_ls_settle<<<cdiv(e->S.G, 256), 256, 0, st>>>(e->S); /* a launch error surfaces at the caller's next check */
+}
+
 /* ---- kernel launch helpers (device pointers) ------------------------------------- */
 static int launch_propose(gpx_engine* e, const gpx_request_rec* d_reqs, const uint8_t* d_payload,
                           uint64_t payload_al, uint32_t n, int32_t* d_status, cudaStream_t st,
                           uint32_t* d_head = nullptr) {
+  ls_settle(e, st);
   ProposeArgs A;
   A.reqs = d_reqs;
   A.n = n;
@@ -633,6 +665,7 @@ static int launch_accept(gpx_engine* e, bool fused, const gpx_accept_rec* d_recs
                          uint64_t blob1_bytes, const unsigned long long* blob1_used_ptr,
                          gpx_accept_reply_rec* d_replies, gpx_decision_rec* d_dec, gpx_exec_rec* d_exec,
                          cudaStream_t st) {
+  ls_settle(e, st);
   AcceptArgs A;
   A.recs = d_recs;
   A.n_ptr = n_ptr;
@@ -665,6 +698,7 @@ static int launch_accept(gpx_engine* e, bool fused, const gpx_accept_rec* d_recs
 
 static int launch_tally(gpx_engine* e, const gpx_accept_reply_rec* d_replies, const uint32_t* n_ptr, uint32_t mult,
                         uint32_t n_max, gpx_decision_rec* d_dec, cudaStream_t st) {
+  ls_settle(e, st);
   TallyArgs A;
   A.replies = d_replies;
   A.n_ptr = n_ptr;
@@ -682,6 +716,7 @@ static int launch_tally(gpx_engine* e, const gpx_accept_reply_rec* d_replies, co
 
 static int launch_commit(gpx_engine* e, const gpx_decision_rec* d_dec, const uint32_t* n_ptr, uint32_t n_max,
                          gpx_exec_rec* d_exec, cudaStream_t st) {
+  ls_settle(e, st);
   CommitArgs A;
   A.decisions = d_dec;
   A.n_ptr = n_ptr;
@@ -702,7 +737,7 @@ static int launch_commit(gpx_engine* e, const gpx_decision_rec* d_dec, const uin
 extern "C++" {
 template <int L, int LP>
 static void launch_round_t(uint32_t n, bool team, cudaStream_t st, const DevState& S, const RoundArgs& RA) {
-  const bool def = S.journaling && S.gc_majority_executed && S.log_meta && !S.cpi_per_group;
+  const bool def = def_config(S);
   bool done = false;
   if constexpr (L <= GPX_GROUND_MAXL) {
     if (!team) {
@@ -788,6 +823,10 @@ static int launch_round(gpx_engine* e, const gpx_request_rec* d_reqs, const uint
   RA.res_a = GPX_SEG_ACC_BYTES(n, RA.pay_bytes);
   RA.res_d = GPX_SEG_DEC_BYTES(n);
   log_advance(e, RA.res_a + RA.res_d, true);
+  if (round_uses_ls(e))
+    e->ls_live = true;
+  else
+    ls_settle(e, st);
   const uint32_t L = e->cfg.n_lanes;
   const uint32_t teams_per_block = (GPX_RBLOCK / 32u) * (32u / L); /* teams of L adjacent lanes */
   const uint32_t grid = cdiv((uint64_t)n, teams_per_block);
@@ -1006,6 +1045,7 @@ int gpx_handle_prepares(gpx_engine* e, uint32_t n, const gpx_pvalue_hdr* prepare
   A.n = n;
   A.replies = (gpx_prepare_reply_rec*)e->d_misc;
   log_advance(e, GPX_SEG_DEC_BYTES(n), true);
+  ls_settle(e, st);
   GPX_DISPATCH_L(L, k_prepare, cdiv(n, GPX_BLOCK), st, e->S, A);
   log_flip(e);
   CK(cudaGetLastError());
@@ -1045,6 +1085,7 @@ int gpx_handle_prepare_replies(gpx_engine* e, uint32_t n, const gpx_election_rec
   A.n = n;
   A.replies = (const gpx_prepare_reply_rec*)(base + el_bytes);
   A.out = (gpx_election_out*)(base + el_bytes + rep_bytes);
+  ls_settle(e, st);
   k_prepare_tally<<<cdiv(n, GPX_P1B_BLOCK), GPX_P1B_BLOCK, 0, st>>>(e->S, A);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out, A.out, out_bytes, cudaMemcpyDeviceToHost, st));
@@ -1115,6 +1156,7 @@ static int round_on_stream(gpx_engine* e, bool fused, const gpx_request_rec* d_r
   const uint64_t pal = (payload_bytes + 15) & ~15ull;
   const uint32_t L = e->cfg.n_lanes;
   const bool tm = e->timing;
+  if (!fused || !round_uses_ls(e)) ls_settle(e, st); /* outside the timed window */
   if (!fused) CK(cudaMemsetAsync(e->d_ctl, 0, sizeof(RoundCtl), st)); /* the fused kernels keep their own block zero */
   if (tm) cudaEventRecord(e->ev[0], st);
   if (fused) { /* the whole round is ONE kernel */
@@ -1751,6 +1793,7 @@ int gpx_get_group_flags(gpx_engine* e, uint32_t lane, uint32_t n, const uint32_t
   if (rc) return rc;
   uint32_t* d_g = (uint32_t*)((uint8_t*)e->d_misc + goff);
   CK(cudaMemcpyAsync(d_g, gids, n * 4ull, cudaMemcpyHostToDevice, e->stream));
+  ls_settle(e, e->stream);
   k_get_flags<<<cdiv(n, 256), 256, 0, e->stream>>>(e->S, lane, d_g, n, (uint8_t*)e->d_misc);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out, e->d_misc, n, cudaMemcpyDeviceToHost, e->stream));
@@ -1775,6 +1818,7 @@ int gpx_select_groups(gpx_engine* e, uint32_t lane, uint32_t mask, uint32_t valu
   A.n_found = (unsigned long long*)base;
   A.gids = (uint32_t*)(base + 16);
   CK(cudaMemsetAsync(base, 0, 16, st));
+  ls_settle(e, st);
   k_select_groups<<<cdiv(e->cfg.max_groups, GPX_PAUSE_BLOCK), GPX_PAUSE_BLOCK, 0, st>>>(e->S, A);
   CK(cudaGetLastError());
   unsigned long long found = 0;
@@ -1809,6 +1853,7 @@ int gpx_missing_decisions(gpx_engine* e, uint32_t lane, uint32_t n, const uint32
   A.size_limit = size_limit;
   A.too_much_gap = too_much_gap;
   A.out = (gpx_missing_rec*)(base + gid_bytes);
+  ls_settle(e, st);
   k_missing_decisions<<<cdiv(n, GPX_PAUSE_BLOCK), GPX_PAUSE_BLOCK, 0, st>>>(e->S, A);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out, A.out, (size_t)n * sizeof(gpx_missing_rec), cudaMemcpyDeviceToHost, st));
@@ -1828,6 +1873,7 @@ int gpx_clear_group_flags(gpx_engine* e, uint32_t lane, uint32_t n, const uint32
   int rc = e->ensure_misc((size_t)n * 4);
   if (rc) return rc;
   CK(cudaMemcpyAsync(e->d_misc, gids, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  ls_settle(e, e->stream);
   k_clear_flags<<<cdiv(n, 128), 128, 0, e->stream>>>(e->S, lane, (const uint32_t*)e->d_misc, n, mask);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(e->stream));
@@ -1858,6 +1904,7 @@ int gpx_pause_groups(gpx_engine* e, uint32_t n, const uint32_t* gids, gpx_row* o
   A.n = n;
   A.rows = (gpx_row*)(base + gid_bytes);
   A.paused = base + flag_off;
+  ls_settle(e, st);
   k_pause_groups<<<cdiv(n, GPX_PAUSE_BLOCK), GPX_PAUSE_BLOCK, 0, st>>>(e->S, A);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out_paused, A.paused, n, cudaMemcpyDeviceToHost, st));

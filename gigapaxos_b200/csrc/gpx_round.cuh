@@ -555,6 +555,26 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
                            * spill-free but made the R = 5 workload slower on an H100) */
 #endif
 
+/* The planes a VALID lockstep record {row, aux, ns_cl, cl} stands for (gpx_dev.cuh); the caller clears VALID. */
+__device__ __forceinline__ void ls_write_planes(const DevState& S, uint32_t gid, uint32_t L, int4 row, uint32_t cl,
+                                                int ns_cl) {
+  for (uint32_t l = 0; l < L; l++) S.acc_row[l * S.G + gid] = row;
+  S.coord_row[cl * S.G + gid] = make_int4(row.y, row.z, row.x, (int)(GPX_CF_EXISTS | GPX_CF_ACTIVE));
+  S.ns_u[cl * S.G + gid] = ns_cl;
+}
+
+/* Every VALID lockstep record back into the planes, VALID cleared: the host runs it before any launch other than
+ * k_round_g<L, true> that reads or writes group state.  One thread per gid. */
+__global__ void k_ls_settle(const __grid_constant__ DevState S) {
+  const uint32_t gid = blockIdx.x * blockDim.x + threadIdx.x;
+  if (gid >= S.G) return;
+  int4 r0, r1;
+  ld256(ls_rec(S, gid), r0, r1);
+  if (!((uint32_t)r1.z & GPX_LS_VALID)) return;
+  ls_write_planes(S, gid, S.L, r0, (uint32_t)r1.z >> 8, r1.y);
+  ls_rec(S, gid)[1] = make_int4(r1.x, r1.y, 0, 0);
+}
+
 /*
  * The fast kernel with one THREAD per group: the thread owns request i and all L lanes of its group.  Same inputs,
  * load levels, in-order predicate and durable outputs as k_round; the team vote is an AND over the lanes held in
@@ -562,6 +582,7 @@ __global__ void __launch_bounds__(GPX_RBLOCK, GPX_ROUND_MINB * (256 / GPX_RBLOCK
  * serves 32 adjacent groups, so every per-lane plane access (acc_row, acc_aux, coord_row, ns_u, the frame
  * records) is 32 x 4..16 B contiguous: whole lines per instruction.  The log images are staged per warp as in
  * k_round; a warp whose 32 groups all took the fast path stages its EXEC rows too and stores them as 16-byte pieces.
+ * With DEF, a group whose lanes are in lockstep is read and written as its 32-byte lockstep record (ls_rec).
  */
 template <int L, bool DEF>
 __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const __grid_constant__ DevState S,
@@ -617,8 +638,10 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
   const bool head = valid && (i == 0 || gprev != gid);
   const bool cand = head && gnext != gid && gid < G && entry < (uint32_t)L && !(rflags & GPX_F_STOP);
 
-  /* ---- level B: group meta and, for every lane, its acceptor row, aux word, coordinator row and the compact
-   * nodeSlotNumbers of the lane as coordinator; the first payload chunk ---- */
+  /* ---- level B: group meta and the group's lockstep record (DEF only); unless the record is VALID, for every lane
+   * its acceptor row, aux word, coordinator row and the compact nodeSlotNumbers of the lane as coordinator (one more
+   * dependent level, on the first round after a settle only); the first payload chunk ---- */
+  const bool LS = DEF && S.ls_off != 0u; /* the lockstep record (gpx_dev.cuh) */
   uint32_t meta = 0, aux[L], dirty[L];
   int4 arow[L], crw[L];
   int nsu[L]; /* ns_u[c]: the value every member's nodeSlotNumbers entry holds at coordinator lane c */
@@ -632,22 +655,39 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
   int4 pv = make_int4(0, 0, 0, 0);
   const uint8_t* const psrc = A.blob0 + poff;
   const bool pal = ((poff | (uint32_t)(uintptr_t)A.blob0) & 15u) == 0;
+  int4 ls0 = make_int4(0, 0, 0, 0), ls1 = ls0;
+  if (LS && head && gid < G) ld256(ls_rec(S, gid), ls0, ls1); /* every head: a VALID one is settled below */
+  const uint32_t ls_ctl = (uint32_t)ls1.z; /* GPX_LS_VALID | cl << 8, or 0 */
   if (cand) {
     meta = S.grp_meta[gid];
-#pragma unroll
-    for (int l = 0; l < L; l++) {
-      const uint32_t ri = (uint32_t)l * G + gid;
-      aux[l] = S.acc_aux[ri];
-      arow[l] = S.acc_row[ri];
-      crw[l] = S.coord_row[ri];
-      if (cf_journaling) dirty[l] = S.acc_dirty[ri];
-      nsu[l] = S.ns_u[ri];
-    }
     if (plen) {
       if (pal)
         pv = ld_stream4(psrc);
       else
         pv.x = psrc[0];
+    }
+    if (!(ls_ctl & GPX_LS_VALID)) {
+#pragma unroll
+      for (int l = 0; l < L; l++) {
+        const uint32_t ri = (uint32_t)l * G + gid;
+        aux[l] = S.acc_aux[ri];
+        arow[l] = S.acc_row[ri];
+        crw[l] = S.coord_row[ri];
+        if (cf_journaling) dirty[l] = S.acc_dirty[ri];
+        nsu[l] = S.ns_u[ri];
+      }
+    }
+  }
+  if (ls_ctl & GPX_LS_VALID) { /* the planes the record stands for; nsu[c] of a lane c other than cl is never used:
+                                * with c as coordinator crw[c] has no EXISTS and the group leaves the fast path */
+#pragma unroll
+    for (int l = 0; l < L; l++) {
+      arow[l] = ls0;
+      aux[l] = (uint32_t)ls1.x;
+      dirty[l] = 0;
+      crw[l] = (ls_ctl >> 8) == (uint32_t)l ? make_int4(ls0.y, ls0.z, ls0.x, (int)(GPX_CF_EXISTS | GPX_CF_ACTIVE))
+                                            : make_int4(0, 0, 0, 0);
+      nsu[l] = ls1.y;
     }
   }
   bool sf = cand && ((meta & (GPX_META_LIVE | GPX_META_IDENT)) == (GPX_META_LIVE | GPX_META_IDENT)) &&
@@ -719,6 +759,15 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
     const int4 q0 = make_int4((int)gid, slot, crow.x, crow.y);
     const bool metaf = cf_logmeta;
     int4* const img = &s_img[warp][lane_id * 2];
+    /* the group leaves this round in lockstep (equal rows, aux words and dirty bytes 0, no coordinator row but cl's):
+     * one record instead of the acc_row, coord_row[cl] and ns_u[cl] stores; the round keeps them equal */
+    bool lsc = LS;
+#pragma unroll
+    for (int l = 0; l < L; l++)
+      lsc = lsc && arow[l].x == arow[0].x && arow[l].y == arow[0].y && arow[l].z == arow[0].z &&
+            arow[l].w == arow[0].w && aux[l] == aux[0] && dirty[l] == 0u &&
+            ((uint32_t)l == cl || !((unsigned)crw[l].w & GPX_CF_EXISTS));
+    int4 lrow;
 #pragma unroll
     for (int l = 0; l < L; l++) {
       uint8_t* const seg_p = ring_ptr(S, l, seg[l]);
@@ -742,7 +791,8 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
       gc_step(row, dmed);
       row.x = (int)((unsigned)row.x + 1u); /* executed(): _slot++ */
       gc_step(row, dmed);                  /* second EEC iteration; nothing is queued (checked above) */
-      S.acc_row[(uint32_t)l * G + gid] = row;
+      if (!lsc) S.acc_row[(uint32_t)l * G + gid] = row;
+      lrow = row;
       const uint32_t wi = 2u * (((uint32_t)l * S.W + ((uint32_t)slot & Wm)) * G + gid);
       if (cf_journaling) {
         if ((evalid >> l) & 1u)
@@ -752,7 +802,7 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
         st256(&S.acc_win[wi], make_int4(slot, crow.x, crow.y, (int)frame_ref),
               make_int4(rq0.z, rq0.w, (int)plen, (int)(GPX_ENT_VALID | (1u << 16))));
     }
-    if (mine != u) S.ns_u[cl * G + gid] = mine; /* nodeSlotNumbers[cl][*] */
+    if (!lsc && mine != u) S.ns_u[cl * G + gid] = mine; /* nodeSlotNumbers[cl][*] */
     if (plen > 1 && !pal) { /* unaligned body: byte by byte, every lane */
 #pragma unroll 1
       for (uint32_t b = 1; b < plen; b++) {
@@ -766,8 +816,15 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
     else
       RA.P.status[i] = slot;
     crow.z = (int)((unsigned)crow.z + 1u); /* PCS.propose: nextProposalSlotNumber++ */
-    S.coord_row[cl * G + gid] = crow;
+    if (lsc) /* crow is {row.y, row.z, row.x, EXISTS | ACTIVE} again */
+      st256(ls_rec(S, gid), lrow, make_int4((int)aux[0], mine, (int)(GPX_LS_VALID | (cl << 8)), 0));
+    else
+      S.coord_row[cl * G + gid] = crow;
   } else if (head) {
+    if (ls_ctl & GPX_LS_VALID) { /* settled before anything else sees the group's planes */
+      ls_write_planes(S, gid, L, ls0, ls_ctl >> 8, ls1.y);
+      ls_rec(S, gid)[1] = make_int4(ls1.x, ls1.y, 0, 0);
+    }
     round_hand_off<L, L>(S, RA, i);
   }
   const uint32_t sfm = __ballot_sync(FULL, sf); /* bit g: group g of the warp took the fast path */
