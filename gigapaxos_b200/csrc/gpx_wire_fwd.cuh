@@ -4,7 +4,8 @@
  * and that node forwards them to the coordinator (PISM.handleProposal :854-885):
  *   k_wire_fwd    the sending side (gpx_wire_encode_forwards_device): the requests gpx_propose_device gave
  *                 GPX_RS_FORWARD become REQUEST packets addressed to the ballot's coordinator, cut as the RequestBatcher
- *                 cuts them.  One thread per run of a gid's requests, as in k_propose.
+ *                 cuts them.  One thread per run of a gid's requests, as in k_propose.  The walk of a run (fwd_run) is
+ *                 shared with the JSON sweep (gpx_wire_json_enc.cuh, k_json_enc_fwd), which sends the same cuts.
  *   k_json_req    the receiving side for a Java peer (gpx_wire_decode_json_requests_device): under load a Java node
  *                 sends its forwards as JSON members of BATCHED_PAXOS_PACKETs (PaxosPacketBatcher.process :270-277),
  *                 which gpx_wire_decode_json_device lists as GPX_WS_UNHANDLED; the REQUEST members among them become
@@ -36,16 +37,27 @@ __device__ __forceinline__ bool fwd_request(const WireFwdArgs& A, uint32_t q) {
   return A.status[q] == GPX_RS_FORWARD && !(A.meta[q].flags & GPX_RM_BROADCASTED);
 }
 
-/* one thread per request; the first request of a gid's run handles the run.  The run is routed as propose_run routes
- * it, from its first request's entry lane; its forwarded requests are cut with batch_end, each cut one REQUEST packet:
- * the outer request is the cut's first with forwardCount + 1 (setForwarderID :437-441), the others its `batched`.
- * Pass 0 writes rstatus and the packet sizes, pass 1 the packets and their refs at the scanned offsets. */
-__global__ void k_wire_fwd(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
-                           const __grid_constant__ WireFwdArgs A) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= A.n) return;
+/* request k heads a cut: its end, the consecutive forwarded requests after it that batch_end lets into its packet */
+__device__ __forceinline__ uint32_t fwd_cut_end(const DevState& S, const WireFwdArgs& A, uint32_t k, uint32_t gid) {
+  const uint32_t b = batch_end(S, A.reqs, A.n, k, gid);
+  uint32_t e = k + 1;
+  while (e < b && fwd_request(A, e)) e++;
+  return e;
+}
+
+/* the forward count the outer request of a cut headed by k carries: forwardCount++ (setForwarderID :437-441, Java int) */
+__device__ __forceinline__ int32_t fwd_count(const WireFwdArgs& A, uint32_t k) {
+  return (int32_t)((uint32_t)A.meta[k].forward_count + 1u);
+}
+
+/* the run of gid's requests that starts at request i, walked as PISM.handleProposal forwards it.  The run is routed as
+ * propose_run routes it, from its first request's entry lane; its forwarded requests are cut with batch_end.
+ * skip(k) is called for every request that is not forwarded, cut(k, b, st, dst, di) once per cut [k, b) with its
+ * status and its destination node dst, member index di of the group's member set (valid when st is GPX_WE_SENT). */
+template <typename Skip, typename Cut>
+__device__ __forceinline__ void fwd_run(const DevState& S, const WireNames& W, const WireFwdArgs& A, uint32_t i,
+                                        Skip&& skip, Cut&& cut) {
   const uint32_t gid = A.reqs[i].gid;
-  if (i > 0 && A.reqs[i - 1].gid == gid) return;
   uint32_t run_end = i + 1;
   while (run_end < A.n && A.reqs[run_end].gid == gid) run_end++;
   uint32_t meta = 0;
@@ -57,10 +69,11 @@ __global__ void k_wire_fwd(const __grid_constant__ DevState S, const __grid_cons
    * coordinator is not a member */
   uint8_t run_st = GPX_WE_SENT;
   int32_t dst = bcoord;
+  uint32_t di = 0xffu;
   if (routed) {
     const MsetInfo* ms = &S.msets[meta & 0xffffu];
     const uint32_t R = (meta >> 16) & 0xffu;
-    uint32_t di = wire_member_idx(ms, R, bcoord);
+    di = wire_member_idx(ms, R, bcoord);
     if (di == 0xffu) {
       run_st = GPX_WE_ELECT;
     } else {
@@ -74,51 +87,72 @@ __global__ void k_wire_fwd(const __grid_constant__ DevState S, const __grid_cons
     }
   }
   const bool named = routed && W.slot != nullptr && W.slot[gid] != GPX_NAME_NONE;
+  uint32_t k = i;
+  while (k < run_end) {
+    if (!routed || !fwd_request(A, k)) {
+      skip(k);
+      k++;
+      continue;
+    }
+    const uint32_t b = fwd_cut_end(S, A, k, gid);
+    uint8_t st = run_st;
+    if (st == GPX_WE_SENT && fwd_count(A, k) > 3) st = GPX_WE_ELECT; /* isPingPonging :508 */
+    if (st == GPX_WE_SENT && !named) st = GPX_WE_NO_NAME;
+    cut(k, b, st, dst, di);
+    k = b;
+  }
+}
+
+/* the REQUEST packet of the cut [k, b) at o, byte-identical to gpx_wire_encode_request: the outer request is the
+ * cut's first with forwardCount + 1, the others its `batched`.  Returns its bytes. */
+__device__ __forceinline__ uint32_t fwd_packet(uint8_t* o, const WireNames& W, const WireFwdArgs& A, uint32_t gid,
+                                               uint32_t k, uint32_t b) {
   WireAccArgs X;
   X.head = nullptr;
   X.reqs = A.reqs;
   X.meta = A.meta;
   X.n_reqs = A.n;
   X.payload = A.payload;
-  uint32_t k = i;
-  while (k < run_end) {
-    if (!routed || !fwd_request(A, k)) {
-      if (!A.emit) {
-        A.rstatus[k] = GPX_WE_VOID;
-        A.cnt[k] = A.cnt[A.n + k] = 0;
-      }
-      k++;
-      continue;
-    }
-    uint32_t b = batch_end(S, A.reqs, A.n, k, gid), e = k + 1; /* the cut of the consecutive forwarded requests */
-    while (e < b && fwd_request(A, e)) e++;
-    b = e;
-    uint8_t st = run_st;
-    const int32_t fc = (int32_t)((uint32_t)A.meta[k].forward_count + 1u); /* forwardCount++ (Java int) */
-    if (st == GPX_WE_SENT && fc > 3) st = GPX_WE_ELECT; /* isPingPonging :508 */
-    if (st == GPX_WE_SENT && !named) st = GPX_WE_NO_NAME;
-    if (!A.emit) {
-      for (uint32_t q = k; q < b; q++) {
-        A.rstatus[q] = st;
-        A.cnt[q] = A.cnt[A.n + q] = 0;
-      }
-      if (st == GPX_WE_SENT) {
-        A.cnt[k] = wire_requests_bytes(W, gid, A.reqs, k, b - k);
-        A.cnt[A.n + k] = 1;
-      }
-    } else if (st == GPX_WE_SENT) {
-      uint8_t* o = A.out + A.off[k];
-      const uint32_t len = ww_requests(o, GPX_PT_REQUEST, W, gid, X, k, b - k);
-      ww_i32(o + 13u + W.name[(size_t)gid * GPX_NAME_BYTES] + 34u, fc); /* the outer request's forwardCount */
-      gpx_wire_ref r;
-      r.off = A.off[k];
-      r.len = len;
-      r.gid = gid;
-      r.node = dst;
-      A.refs[A.off[A.n + k]] = r;
-    }
-    k = b;
-  }
+  const uint32_t len = ww_requests(o, GPX_PT_REQUEST, W, gid, X, k, b - k);
+  ww_i32(o + 13u + W.name[(size_t)gid * GPX_NAME_BYTES] + 34u, fwd_count(A, k)); /* the outer request's forwardCount */
+  return len;
+}
+
+/* one thread per request; the first request of a gid's run walks the run (fwd_run), each cut one REQUEST packet.
+ * Pass 0 writes rstatus and the packet sizes, pass 1 the packets and their refs at the scanned offsets. */
+__global__ void k_wire_fwd(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                           const __grid_constant__ WireFwdArgs A) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= A.n) return;
+  const uint32_t gid = A.reqs[i].gid;
+  if (i > 0 && A.reqs[i - 1].gid == gid) return;
+  fwd_run(
+      S, W, A, i,
+      [&](uint32_t k) {
+        if (!A.emit) {
+          A.rstatus[k] = GPX_WE_VOID;
+          A.cnt[k] = A.cnt[A.n + k] = 0;
+        }
+      },
+      [&](uint32_t k, uint32_t b, uint8_t st, int32_t dst, uint32_t) {
+        if (!A.emit) {
+          for (uint32_t q = k; q < b; q++) {
+            A.rstatus[q] = st;
+            A.cnt[q] = A.cnt[A.n + q] = 0;
+          }
+          if (st == GPX_WE_SENT) {
+            A.cnt[k] = wire_requests_bytes(W, gid, A.reqs, k, b - k);
+            A.cnt[A.n + k] = 1;
+          }
+        } else if (st == GPX_WE_SENT) {
+          gpx_wire_ref r;
+          r.off = A.off[k];
+          r.len = fwd_packet(A.out + A.off[k], W, A, gid, k, b);
+          r.gid = gid;
+          r.node = dst;
+          A.refs[A.off[A.n + k]] = r;
+        }
+      });
 }
 
 /* ---- REQUEST members of a Java peer's BATCHED_PAXOS_PACKETs (gpx_wire_decode_json_requests_device) ---------------- */

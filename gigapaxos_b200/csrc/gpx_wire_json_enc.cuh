@@ -1,29 +1,35 @@
 /*
- * gpx_wire_json_enc.cuh -- the sending side of the JSON form (gpx_wire_encode_json_device): a node's reply and decision
- * records become what a loaded Java node sends, BATCHED_PAXOS_PACKET wrappers (type 37) of BatchedAcceptReply (34) and
- * BatchedCommit (35) objects, one wrapper per recipient set and cut, and every NACK as a bare ACCEPT_REPLY (8).  The
- * rules are in include/gpx.h; the objects are byte-identical to gigapaxos_b200/packets_json.py's.
+ * gpx_wire_json_enc.cuh -- the sending side of the JSON form (gpx_wire_encode_json_sweep_device, and
+ * gpx_wire_encode_json_device, the sweep without forwards): a node's reply and decision records, and the requests it
+ * forwards, become what a loaded Java node sends, BATCHED_PAXOS_PACKET wrappers (type 37) of BatchedAcceptReply (34),
+ * BatchedCommit (35) and REQUEST (1) objects, one wrapper per recipient set and cut, every NACK as a bare ACCEPT_REPLY
+ * (8) and every forward of several requests as a lone REQUEST packet in the byte form.  The rules are in
+ * include/gpx.h; the objects are byte-identical to gigapaxos_b200/packets_json.py's.
  *
  * The records are classified and sorted as the byte encoders do it (k_wire_enc_keys_*, then a stable sort of the keys),
  * so a member is a run of wire_run, with wire_slots_each's slots.  Then:
  *   k_json_enc_nacks    one thread per reply: routes a NACK as wire_reply_route routes a positive reply, sizes its
  *                       bare packet.
- *   k_json_enc_members  one thread per member candidate (sorted reply positions, then sorted decision positions): the
- *                       run it starts, its sending lane, its recipient set and its object's size (nothing written);
- *                       the first candidate of each (lane, recipient set) by atomicMin.
+ *   k_json_enc_fwd      one thread per run of a gid's requests (gpx_wire_fwd.cuh's fwd_run, as k_wire_fwd walks it):
+ *                       each request's status; a cut of one request becomes a member, any other cut (and a member too
+ *                       large to wrap) a lone REQUEST packet, sized here.
+ *   k_json_enc_members  one thread per member candidate (sorted reply positions, then sorted decision positions, then
+ *                       requests): the run or forward it starts, its sending lane, its recipient set and its object's
+ *                       size (nothing written); the first candidate of each (lane, recipient set) by atomicMin.
  *   k_json_enc_keys     the wrapper sort key (lane, first candidate of the member's set) per candidate.
  *   (a stable radix sort by that key; candidates are in sweep order already, so the order is (lane, first, position))
  *   k_json_enc_vals     the member sizes + 1 in sorted order, for a scan by key: each member's start in its group's
  *                       comma-joined stream.
  *   k_json_enc_cut      one thread per sorted member: does it open or close a wrapper (the cut rule), its bytes in the
  *                       output (object, separator or wrapper head, wrapper tail) and its wrapper's refs.
- *   k_json_enc_emit_nacks, k_json_enc_emit   write the packets at the scanned offsets; the member that opens a wrapper
- *                       writes its head and notes where it starts, the one that closes it writes its tail.
+ *   k_json_enc_emit_nacks, k_json_enc_emit_fwd, k_json_enc_emit   write the packets at the scanned offsets (bare
+ *                       NACKs, then lone REQUEST packets, then wrappers); the member that opens a wrapper writes its
+ *                       head and notes where it starts, the one that closes it writes its tail.
  *   k_json_enc_refs     the member that closes a wrapper indexes it once per recipient node.
  * Every kernel is scalar and byte-addressed, so tests/emu compiles this file for the host.
  */
 #pragma once
-#include "gpx_wire_dev.cuh"
+#include "gpx_wire_fwd.cuh" /* fwd_run: the forwards are k_wire_fwd's */
 
 #include <algorithm>
 #include <map>
@@ -83,7 +89,8 @@ enum { JE_BYTES = 0, JE_REFS = 1, JE_OPENS = 2, JE_BIG = 3, JE_NCNT = 4 };
 struct WireJsonEncArgs {
   WireEncodeArgs R, D; /* replies and decisions: records, rstatus, keys and their stable order (perm, skey) */
   JsonSets Z;
-  uint32_t n;          /* member candidates: the R.n sorted reply positions, then the D.n sorted decision positions */
+  uint32_t n;          /* member candidates: the R.n sorted reply positions, the D.n sorted decision positions, then
+                        * the F.n requests */
   uint32_t L;
   uint32_t T;          /* cut width: wrap_bytes - GPX_JSON_WRAP_OVERHEAD - GPX_JSON_MAX_MEMBER */
   uint32_t* first;     /* [L][Z.n] the lowest candidate of each (lane, recipient set) */
@@ -99,10 +106,17 @@ struct WireJsonEncArgs {
   const uint32_t* off; /* [JE_NCNT][n] their exclusive prefix sums */
   uint32_t* ncnt;      /* [2][R.n] per reply: bare NACK bytes, NACK packets */
   const uint32_t* noff;
-  uint32_t nack_bytes, n_nacks; /* the totals of ncnt: the wrappers follow the bare NACKs */
+  uint32_t nack_bytes, n_nacks; /* the totals of ncnt: the lone REQUEST packets follow the bare NACKs */
   uint2* wbeg;         /* [n] per wrapper: its offset in out, its first ref */
   uint8_t* out;
   gpx_wire_ref* refs;
+  /* the forwards (F.n == 0, as a zeroed struct has it: none).  Candidate R.n + D.n + q is request q.  F.rstatus gets
+   * the statuses; F.cnt / F.off are [2][F.n] rows per request that heads a lone packet: its bytes, 1 */
+  WireFwdArgs F;
+  uint8_t* fmem;       /* [F.n] request q heads a cut of one request that is written as a member */
+  uint8_t* flane;      /* [F.n] at the head of a GPX_WE_SENT cut: its sending lane (the run's entry lane) */
+  uint8_t* fdi;        /* [F.n] and its destination's member index */
+  uint32_t lone_bytes, n_lone; /* the totals of F.cnt: the wrappers follow the lone REQUEST packets */
 };
 
 /* ---- JSON text, or only its length (p == nullptr) ------------------------------------------------------------------- */
@@ -127,13 +141,12 @@ __device__ __forceinline__ void jw_i64(JsonW& w, int64_t v) {
     for (uint32_t k = d; k-- > 0; u /= 10u) w.p[w.n + k] = (uint8_t)('0' + u % 10u);
   w.n += d;
 }
-/* a group's paxosID (ISO-8859-1 bytes) as json.dumps writes the string: \" \\ \b \f \n \r \t, every other byte below
- * 0x20 or from 0x7f up as \u00xx (lowercase hex), the rest as it is */
-__device__ __forceinline__ void jw_name(JsonW& w, const WireNames& W, uint32_t gid) {
-  const uint8_t* m = W.name + (size_t)gid * GPX_NAME_BYTES;
+/* n ISO-8859-1 bytes as json.dumps writes the string: \" \\ \b \f \n \r \t, every other byte below 0x20 or from
+ * 0x7f up as \u00xx (lowercase hex), the rest as it is */
+__device__ __forceinline__ void jw_str(JsonW& w, const uint8_t* m, uint32_t n) {
   jw_c(w, '"');
-  for (uint32_t i = 0; i < m[0]; i++) {
-    const uint32_t c = m[1 + i];
+  for (uint32_t i = 0; i < n; i++) {
+    const uint32_t c = m[i];
     const uint32_t e = c == '"' ? '"' : c == '\\' ? '\\' : c == 8 ? 'b' : c == 12 ? 'f' : c == 10 ? 'n'
                      : c == 13 ? 'r' : c == 9 ? 't' : 0u;
     if (e) {
@@ -148,6 +161,11 @@ __device__ __forceinline__ void jw_name(JsonW& w, const WireNames& W, uint32_t g
     }
   }
   jw_c(w, '"');
+}
+/* a group's paxosID */
+__device__ __forceinline__ void jw_name(JsonW& w, const WireNames& W, uint32_t gid) {
+  const uint8_t* m = W.name + (size_t)gid * GPX_NAME_BYTES;
+  jw_str(w, m + 1, m[0]);
 }
 /* PaxosPacket.toJSONObject :478-494: {"type":90,"PT":pt,"ID":name,"V":version */
 __device__ __forceinline__ void jw_head(JsonW& w, const WireNames& W, int32_t pt, uint32_t gid) {
@@ -180,11 +198,60 @@ __device__ __forceinline__ void jw_reply(JsonW& w, const DevState& S, const Wire
   jw_i64(w, x.req_id);
 }
 
-/* the member object of candidate c, which starts a run: a BatchedAcceptReply (batched_accept_reply_json) or a
- * BatchedCommit (batched_commit_json) */
+/* ,"CA":"/a.b.c.d:port" -- InetSocketAddress.toString() of a literal address */
+__device__ __forceinline__ void jw_addr(JsonW& w, const char* key, const uint8_t* ip, uint16_t port) {
+  jw_s(w, key);
+  for (int j = 0; j < 4; j++) {
+    jw_c(w, j ? '.' : '/');
+    jw_i64(w, ip[j]);
+  }
+  jw_c(w, ':');
+  jw_i64(w, port);
+  jw_c(w, '"');
+}
+/* request q forwarded alone as a JSON member: request_json (RequestPacket.toJSONSmartImpl :697-742) with forwardCount +
+ * 1.  A forwarded request carries no response, no digest and no batched requests, and is not broadcasted. */
+__device__ __forceinline__ void jw_request(JsonW& w, const WireNames& W, const WireFwdArgs& F, uint32_t q) {
+  const gpx_request_rec rq = F.reqs[q];
+  const gpx_wire_req_meta m = F.meta[q];
+  jw_head(w, W, GPX_PT_REQUEST, rq.gid);
+  jw_s(w, ",\"QID\":");
+  jw_i64(w, rq.req_id);
+  jw_s(w, ",\"QV\":");
+  jw_str(w, F.payload + rq.payload_off, rq.payload_len);
+  jw_s(w, ",\"ET\":");
+  jw_i64(w, m.entry_time);
+  const int32_t fc = fwd_count(F, q);
+  if (fc > 0) {
+    jw_s(w, ",\"NFWDS\":");
+    jw_i64(w, fc);
+  }
+  if (rq.flags & GPX_F_STOP) jw_s(w, ",\"STOP\":true");
+  jw_s(w, ",\"E\":");
+  jw_i64(w, rq.entry_node);
+  if (m.client_port) jw_addr(w, ",\"CA\":\"", m.client_ip, m.client_port);
+  if (m.listen_port) jw_addr(w, ",\"LA\":\"", m.listen_ip, m.listen_port);
+  if (m.flags & GPX_RM_RETURN_VALUE) jw_s(w, ",\"QF\":true");
+  jw_c(w, '}');
+}
+/* request q fits in a member: at most 6 bytes per value byte and 2 KiB for the rest (a name of at most 127 bytes,
+ * escaped, the keys, numbers and addresses) -- else its exact size */
+__device__ __forceinline__ bool jw_request_fits(const WireNames& W, const WireFwdArgs& F, uint32_t q) {
+  if (6ull * F.reqs[q].payload_len + 2048u <= GPX_JSON_MAX_MEMBER) return true;
+  JsonW w = {nullptr, 0};
+  jw_request(w, W, F, q);
+  return w.n <= GPX_JSON_MAX_MEMBER;
+}
+
+/* the member object of candidate c, which starts a run or a forward: a BatchedAcceptReply
+ * (batched_accept_reply_json), a BatchedCommit (batched_commit_json) or a REQUEST (request_json) */
 __device__ __forceinline__ void jw_member(JsonW& w, const DevState& S, const WireNames& W, const WireJsonEncArgs& A,
                                           uint32_t c) {
   uint32_t end = 0;
+  if (c >= A.R.n + A.D.n) {
+    jw_request(w, W, A.F, c - A.R.n - A.D.n);
+    return;
+  }
   if (c < A.R.n) {
     wire_run<gpx_accept_reply_rec>(A.R, c, end);
     const gpx_accept_reply_rec* recs = reinterpret_cast<const gpx_accept_reply_rec*>(A.R.recs);
@@ -253,7 +320,43 @@ __device__ __forceinline__ uint32_t json_commit_lane(const GroupCtx& g, int32_t 
   return 0;
 }
 
-/* one thread per member candidate: the run it starts (if any), its lane, recipient set and size */
+/* one thread per request; the first of a gid's run walks it as k_wire_fwd does, with its statuses.  A GPX_WE_SENT cut
+ * of one request whose object fits GPX_JSON_MAX_MEMBER is a member sent from the run's entry lane; every other
+ * GPX_WE_SENT cut is a lone REQUEST packet, sized in F.cnt as k_wire_fwd sizes it. */
+__global__ void k_json_enc_fwd(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                               const __grid_constant__ WireJsonEncArgs A) {
+  const WireFwdArgs& F = A.F;
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= F.n) return;
+  const uint32_t gid = F.reqs[i].gid;
+  if (i > 0 && F.reqs[i - 1].gid == gid) return;
+  const uint8_t lane = (uint8_t)((F.reqs[i].flags >> 8) & 0xfu);
+  fwd_run(
+      S, W, F, i,
+      [&](uint32_t k) {
+        F.rstatus[k] = GPX_WE_VOID;
+        A.fmem[k] = 0;
+        F.cnt[k] = F.cnt[F.n + k] = 0;
+      },
+      [&](uint32_t k, uint32_t b, uint8_t st, int32_t, uint32_t di) {
+        for (uint32_t q = k; q < b; q++) {
+          F.rstatus[q] = st;
+          A.fmem[q] = 0;
+          F.cnt[q] = F.cnt[F.n + q] = 0;
+        }
+        if (st != GPX_WE_SENT) return;
+        A.flane[k] = lane;
+        A.fdi[k] = (uint8_t)di;
+        if (b - k == 1 && jw_request_fits(W, F, k)) {
+          A.fmem[k] = 1;
+        } else {
+          F.cnt[k] = wire_requests_bytes(W, gid, F.reqs, k, b - k);
+          F.cnt[F.n + k] = 1;
+        }
+      });
+}
+
+/* one thread per member candidate: the run or forward it starts (if any), its lane, recipient set and size */
 __global__ void k_json_enc_members(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
                                    const __grid_constant__ WireJsonEncArgs A) {
   const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
@@ -266,10 +369,16 @@ __global__ void k_json_enc_members(const __grid_constant__ DevState S, const __g
       lane = i % A.R.n_lanes;
       set = A.Z.one[(S.grp_meta[x.gid] & 0xffffu) * GPX_MAX_GROUP_SIZE + GPX_WHO_DST(x.who)];
     }
-  } else if (wire_run<gpx_decision_rec>(A.D, c - A.R.n, end)) {
-    const gpx_decision_rec d = reinterpret_cast<const gpx_decision_rec*>(A.D.recs)[A.D.perm[c - A.R.n]];
-    lane = json_commit_lane(group_ctx(S, d.gid), d.bcoord);
-    set = A.Z.of_mset[S.grp_meta[d.gid] & 0xffffu];
+  } else if (c < A.R.n + A.D.n) {
+    if (wire_run<gpx_decision_rec>(A.D, c - A.R.n, end)) {
+      const gpx_decision_rec d = reinterpret_cast<const gpx_decision_rec*>(A.D.recs)[A.D.perm[c - A.R.n]];
+      lane = json_commit_lane(group_ctx(S, d.gid), d.bcoord);
+      set = A.Z.of_mset[S.grp_meta[d.gid] & 0xffffu];
+    }
+  } else if (A.fmem[c - A.R.n - A.D.n]) {
+    const uint32_t q = c - A.R.n - A.D.n;
+    lane = A.flane[q];
+    set = A.Z.one[(S.grp_meta[A.F.reqs[q].gid] & 0xffffu) * GPX_MAX_GROUP_SIZE + A.fdi[q]];
   }
   A.mset[c] = set;
   A.mlane[c] = (uint8_t)lane;
@@ -343,6 +452,22 @@ __global__ void k_json_enc_emit_nacks(const __grid_constant__ DevState S, const 
   A.refs[A.noff[A.R.n + i]] = r;
 }
 
+/* one thread per request: the lone REQUEST packet it heads (fwd_packet), after the bare NACKs, in request order; its ref
+ * as k_wire_fwd writes it */
+__global__ void k_json_enc_emit_fwd(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                                    const __grid_constant__ WireJsonEncArgs A) {
+  const WireFwdArgs& F = A.F;
+  const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= F.n || !F.cnt[F.n + q]) return;
+  const uint32_t gid = F.reqs[q].gid, at = A.nack_bytes + F.off[q];
+  gpx_wire_ref r;
+  r.off = at;
+  r.len = fwd_packet(A.out + at, W, F, gid, q, fwd_cut_end(S, F, q, gid));
+  r.gid = gid;
+  r.node = S.msets[S.grp_meta[gid] & 0xffffu].nodes[A.fdi[q]];
+  A.refs[A.n_nacks + F.off[F.n + q]] = r;
+}
+
 /* one thread per sorted position: the member's separator (or its wrapper's head), object and its wrapper's tail */
 __global__ void k_json_enc_emit(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
                                 const __grid_constant__ WireJsonEncArgs A) {
@@ -350,11 +475,12 @@ __global__ void k_json_enc_emit(const __grid_constant__ DevState S, const __grid
   if (j >= A.n) return;
   bool opens = false, closes = false;
   if (!json_cut(A, j, opens, closes)) return;
-  const uint32_t at = A.nack_bytes + A.off[(size_t)JE_BYTES * A.n + j];
+  const uint32_t at = A.nack_bytes + A.lone_bytes + A.off[(size_t)JE_BYTES * A.n + j];
   JsonW w = {A.out + at, 0};
   if (opens) {
     jw_s(w, GPX_JSON_WRAP_HEAD);
-    A.wbeg[A.off[(size_t)JE_OPENS * A.n + j]] = make_uint2(at, A.n_nacks + A.off[(size_t)JE_REFS * A.n + j]);
+    A.wbeg[A.off[(size_t)JE_OPENS * A.n + j]] =
+        make_uint2(at, A.n_nacks + A.n_lone + A.off[(size_t)JE_REFS * A.n + j]);
   } else {
     jw_c(w, ',');
   }
@@ -371,7 +497,8 @@ __global__ void k_json_enc_refs(const __grid_constant__ WireJsonEncArgs A) {
   if (!json_cut(A, j, opens, closes) || !closes) return;
   const uint32_t wi = A.off[(size_t)JE_OPENS * A.n + j] + (opens ? 1u : 0u) - 1u;
   const uint2 b = A.wbeg[wi];
-  const uint32_t end = A.nack_bytes + A.off[(size_t)JE_BYTES * A.n + j] + A.cnt[(size_t)JE_BYTES * A.n + j];
+  const uint32_t end =
+      A.nack_bytes + A.lone_bytes + A.off[(size_t)JE_BYTES * A.n + j] + A.cnt[(size_t)JE_BYTES * A.n + j];
   const uint32_t c = A.order[j], set = A.mset[c];
   for (uint32_t k = 0; k < A.Z.count[set]; k++) {
     gpx_wire_ref r;

@@ -459,6 +459,39 @@ def encode_json_device(engine, replies, n_replies: int, decisions, n_dec_ptr: Op
     return JsonEncodeOut(rr[:n_replies], rd[:n_dec_max], out[: caps[0]], refs[: caps[1]], caps)
 
 
+JsonSweepOut = namedtuple("JsonSweepOut", "rstatus_replies rstatus_decisions rstatus_reqs out refs sizes")
+
+
+def encode_json_sweep_device(engine, replies, n_replies: int, decisions, n_dec_ptr: Optional[int], n_dec_max: int,
+                             reqs, meta, n_reqs: int, status, payload, down_nodes: Sequence[int], caps,
+                             wrap_bytes: int = 0, stream=None) -> JsonSweepOut:
+    """gpx_wire_encode_json_sweep_device: encode_json_device's replies and decisions, and the forwarded requests among
+    the first n_reqs of reqs / meta (encode_forwards_device's inputs), as one sweep -- a forward of one request is a
+    REQUEST member of the wrapper to its coordinator, any other forward a lone REQUEST packet.  Any tensor may be None
+    when its count is 0.  caps = (packet bytes, refs); GPX_ERANGE as in decode_batch_device.  Returns the three rstatus
+    arrays (uint8; rstatus_reqs is encode_forwards_device's), the packet arena, refs [k, 16] (bare NACKs, lone
+    REQUEST packets, wrappers) and the two host sizes."""
+    import torch
+    dev = next(t for t in (replies, decisions, reqs) if t is not None).device
+    down = np.ascontiguousarray(list(down_nodes) or [0], dtype=np.int32)
+    L, st = engine.L, stream_handle(stream)
+    with _on(stream):
+        rr = torch.empty(max(n_replies, 1), dtype=torch.uint8, device=dev)
+        rd = torch.empty(max(n_dec_max, 1), dtype=torch.uint8, device=dev)
+        rq = torch.empty(max(n_reqs, 1), dtype=torch.uint8, device=dev)
+        (out, refs), caps = _sized(
+            engine, caps, (C.c_uint64, C.c_uint32),
+            lambda c: (torch.empty(max(c[0], 1), dtype=torch.uint8, device=dev),
+                       torch.empty((max(c[1], 1), 16), dtype=torch.uint8, device=dev)),
+            lambda o, sz: L.fn("wire_encode_json_sweep_device")(
+                engine.handle, C.c_uint32(n_replies), _dptr(replies), _dptr(decisions),
+                C.c_void_p(n_dec_ptr) if n_dec_ptr else None, C.c_uint32(n_dec_max), _dptr(reqs), _dptr(meta),
+                C.c_uint32(n_reqs), _dptr(status), _dptr(payload), C.c_uint32(len(down_nodes)),
+                down.ctypes.data_as(C.c_void_p), _dptr(rr), _dptr(rd), _dptr(rq), C.c_uint64(wrap_bytes),
+                _dptr(o[0]), sz[0], _dptr(o[1]), sz[1], st))
+    return JsonSweepOut(rr[:n_replies], rd[:n_dec_max], rq[:n_reqs], out[: caps[0]], refs[: caps[1]], caps)
+
+
 # ---- the coordinator's side: REQUEST packets -> proposals -> ACCEPT packets, on the device ---------------------------
 RequestsOut = namedtuple("RequestsOut", "status reqs meta payload sizes")
 

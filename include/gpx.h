@@ -1204,6 +1204,45 @@ int gpx_wire_decode_json_requests_device(gpx_engine* e, uint32_t n_members, cons
                                          gpx_wire_req_meta* meta, uint32_t* n_reqs, uint8_t* payload,
                                          uint64_t* payload_bytes, void* stream);
 
+/* Encode a node's whole non-digest sweep as a loaded Java node sends it: gpx_wire_encode_json_device's replies and
+ * decisions, and the requests gpx_wire_encode_forwards_device forwards, as REQUEST members of the same
+ * BATCHED_PAXOS_PACKET wrappers (BATCHED_REQUESTS and BATCH_ACROSS_GROUPS, both on by default: PaxosPacketBatcher
+ * coalesces a forwarded RequestPacket without batched requests, allCoalescableRequests :447-454).  The replies'
+ * and decisions' arguments are gpx_wire_encode_json_device's; reqs, meta, n_reqs, status, payload, n_down and
+ * down_nodes are gpx_wire_encode_forwards_device's, with the same conditions.  With n_reqs == 0 every output, size and
+ * return code is gpx_wire_encode_json_device's.
+ *   rstatus_reqs[n_reqs]  byte for byte gpx_wire_encode_forwards_device's rstatus for the same inputs (GPX_WE_SENT,
+ *     GPX_WE_VOID, GPX_WE_ELECT, GPX_WE_NO_NAME): the same routing, cuts, destinations and rules.
+ *   Wrapped or alone: a GPX_WE_SENT cut of exactly one request is a REQUEST member, byte-identical to packets_json's
+ *     request_json of that request with forwardCount + 1: "type", "PT", "ID", "V", "QID", "QV", "ET", "NFWDS" (when
+ *     forwardCount + 1 > 0), "STOP" (when true), "E", "CA" and "LA" ("/a.b.c.d:port", when the port is nonzero), "QF"
+ *     (when true), strings escaped as for gpx_wire_encode_json_device's names.  A cut of two or more requests -- a
+ *     RequestPacket with batched requests, which the reference does not coalesce but sends byteified
+ *     (PaxosMessenger.toJSONSmartObject :126-132) -- is written alone, byte-identical to the REQUEST packet
+ *     gpx_wire_encode_forwards_device writes for it.  So is a one-request member larger than GPX_JSON_MAX_MEMBER: a
+ *     deliberate difference, where a Java node would wrap it, so that a very large client value does not fail the
+ *     whole sweep.  Both are GPX_WE_SENT.  An oversized reply or commit member stays GPX_EINVAL.
+ *   Sender and recipients: a forward member is sent from the entry lane of its run's first request ((flags >> 8) &
+ *     0xf, the lane propose_route routes from) to the singleton {destination}.  So a forward to node X shares a wrapper
+ *     with that lane's replies to X and its commits whose only remote member is X.
+ *   Sweep: each lane sweeps its replies, then its commits, then its forward members in request order
+ *     (PaxosPacketBatcher.dequeueImpl :182-209); grouping by recipient set and the cut rule are
+ *     gpx_wire_encode_json_device's.
+ *   out[*out_bytes]  the bare ACCEPT_REPLYs in record order, then the lone REQUEST packets in request order, then the
+ *     wrappers.  refs[*n_refs] in that order: a lone packet's ref is {off, len, gid, node = destination}, as
+ *     gpx_wire_encode_forwards_device writes it; a wrapper's gid is the sending lane.
+ * n_replies + n_dec_max + n_reqs above 2^31 - 1 is GPX_ERANGE.  Pointers, capacities, GPX_ERANGE, GPX_EINVAL, the
+ * stream and the one synchronisation are gpx_wire_encode_json_device's; down_nodes is a HOST pointer.  As there, the
+ * caller decides whether a sweep of at most MIN_PP_BATCH_SIZE packets goes unwrapped. */
+int gpx_wire_encode_json_sweep_device(gpx_engine* e, uint32_t n_replies, const gpx_accept_reply_rec* replies,
+                                      const gpx_decision_rec* decisions, const uint32_t* n_dec_ptr, uint32_t n_dec_max,
+                                      const gpx_request_rec* reqs, const gpx_wire_req_meta* meta, uint32_t n_reqs,
+                                      const int32_t* status, const uint8_t* payload, uint32_t n_down,
+                                      const int32_t* down_nodes, uint8_t* rstatus_replies,
+                                      uint8_t* rstatus_decisions, uint8_t* rstatus_reqs, uint64_t wrap_bytes,
+                                      uint8_t* out, uint64_t* out_bytes, gpx_wire_ref* refs, uint32_t* n_refs,
+                                      void* stream);
+
 /* ---- helpers shared with the reference semantics ---------------------------------- */
 int32_t gpx_java_string_hash(const char* s, size_t len); /* String.hashCode() */
 /* PISM.roundRobinCoordinator :2251-2256 on sorted members */
