@@ -58,6 +58,10 @@ req_meta_dtype = np.dtype([("client_ip", "u1", (4,)), ("client_port", "<u2"), ("
                            ("listen_ip", "u1", (4,)), ("forward_count", "<i4"), ("entry_time", "<i8"),
                            ("flags", "<u4"), ("pad", "<u4")])
 assert req_meta_dtype.itemsize == 32
+# gpx_rc_key: one executed client request for the response cache (gpx_response_cache_put_device)
+rc_key_dtype = np.dtype([("gid", "<u4"), ("handle", "<i4"), ("req_id", "<i8"), ("client_ip", "u1", (4,)),
+                         ("client_port", "<u2"), ("pad", "<u2")])
+assert rc_key_dtype.itemsize == 24
 # gpx_wire_member: one member of a JSON packet (gpx_wire_decode_json_device)
 wire_member_dtype = np.dtype([("pkt", "<u4"), ("off", "<u4"), ("len", "<u4"), ("status", "<i4")])
 # gpx_wire_encode_json_device: a wrapper's default and largest size, its head + tail, the largest member object
@@ -363,6 +367,29 @@ class Engine:
         self.L.check(self.L.fn("get_group_flags")(self._h, C.c_uint32(lane), C.c_uint32(len(gids)), _ptr(gids),
                                                   _ptr(out)))
         return out
+
+    # ---- response cache: device buffers (torch CUDA tensors), on `stream` (None: torch's current stream) ----------
+    def response_cache_init(self, n_buckets: int, timeout_ms: int):
+        """gpx_response_cache_init: an empty table of n_buckets buckets whose entries expire after timeout_ms"""
+        self.L.check(self.L.fn("response_cache_init")(self._h, C.c_uint32(n_buckets), C.c_int64(timeout_ms)))
+
+    def response_cache_put(self, keys, n: int, now_ms: int, stream=None):
+        """gpx_response_cache_put_device: the first n rows of keys (rc_key_dtype records, [k, 24] uint8) at now_ms"""
+        from .wire import _dptr, stream_handle
+        self.L.check(self.L.fn("response_cache_put_device")(self._h, C.c_uint32(n), _dptr(keys), C.c_int64(now_ms),
+                                                             stream_handle(stream)))
+
+    def response_cache_match(self, reqs, meta, n: int, now_ms: int, hit, out_reqs, out_meta, stream=None) -> int:
+        """gpx_response_cache_match_device over the first n rows of reqs / meta ([k, 32] uint8, a request decoder's
+        output): hit int32 [n] receives each request's handle or -1, out_reqs / out_meta the misses in input order.
+        -> the count of misses"""
+        from .wire import _dptr, stream_handle
+        n_out = C.c_uint32(0)
+        self.L.check(self.L.fn("response_cache_match_device")(self._h, C.c_uint32(n), _dptr(reqs), _dptr(meta),
+                                                               C.c_int64(now_ms), _dptr(hit), _dptr(out_reqs),
+                                                               _dptr(out_meta), C.byref(n_out),
+                                                               stream_handle(stream)))
+        return n_out.value
 
     # ---- data path ------------------------------------------------------------------
     def propose(self, reqs: np.ndarray, payload: np.ndarray):

@@ -30,6 +30,7 @@
 #include "gpx_wire_json.cuh"
 #include "gpx_wire_json_enc.cuh"
 #include "gpx_wire_fwd.cuh"
+#include "gpx_respcache.cuh"
 
 #include <cub/cub.cuh>
 
@@ -136,6 +137,12 @@ struct gpx_engine {
   JsonSetTable jsets;
   JsonSets d_jsets{};
   size_t jsets_up = 0; /* member sets the device copy covers */
+  /* the response cache's key table (gpx_respcache_host.inc), allocated by gpx_response_cache_init; the generations
+   * live in the name state */
+  RcCell* rc_cell = nullptr;
+  uint32_t rc_mask = 0;
+  int64_t rc_timeout = 0;
+  uint32_t* rc_gen = nullptr; /* [G] the times gpx_set_group_names has named each gid */
 
   template <typename T>
   int dalloc(T** p, size_t n) {
@@ -354,6 +361,7 @@ void gpx_engine_destroy(gpx_engine* e) {
   if (e->d_misc) cudaFree(e->d_misc);
   if (e->d_wire) cudaFree(e->d_wire);
   if (e->d_wire_io) cudaFree(e->d_wire_io);
+  if (e->rc_cell) cudaFree(e->rc_cell);
   if (e->ev_wire) cudaEventDestroy(e->ev_wire);
   if (e->h_ctl) cudaFreeHost(e->h_ctl);
   for (auto& ps : e->pipe) {
@@ -1935,5 +1943,6 @@ int gpx_pause_groups(gpx_engine* e, uint32_t n, const uint32_t* gids, gpx_row* o
 
 #include "gpx_spread_host.inc"
 #include "gpx_wire_host.inc"
+#include "gpx_respcache_host.inc"
 
 } /* extern "C" */

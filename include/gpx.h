@@ -36,6 +36,8 @@
  *   gpx_wire_*               <- paxospackets byte codecs (RequestPacket.java:819-1024,
  *                               AcceptPacket.java:95-138, BatchedAcceptReply.java:103-173,
  *                               BatchedCommit.java:184-252, PaxosPacket.java:443-476)
+ *   gpx_response_cache_*     <- PaxosManager.handleIncomingPacket :1084, retransmittedRequest :332-349,
+ *                               executed :311-330 (ENABLE_RESPONSE_CACHING)
  *
  * Conventions (mirror the reference, SURVEY.md 8b): int return codes are for API
  * misuse only; protocol-level rejects (stopped group, stale ballot, unknown
@@ -1242,6 +1244,61 @@ int gpx_wire_encode_json_sweep_device(gpx_engine* e, uint32_t n_replies, const g
                                       uint8_t* rstatus_decisions, uint8_t* rstatus_reqs, uint64_t wrap_bytes,
                                       uint8_t* out, uint64_t* out_bytes, gpx_wire_ref* refs, uint32_t* n_refs,
                                       void* stream);
+
+/* ---- response cache: a client's retransmitted request is answered from the cache, not proposed again -------------
+ * PaxosManager.handleIncomingPacket :1084 checks every incoming REQUEST against the response cache before it is
+ * batched (ENABLE_RESPONSE_CACHING, on by default); retransmittedRequest :332-349 answers a hit from the cached
+ * response and drops the request; executed :311-330 puts every executed ClientRequest's response at every replica;
+ * entries expire REQUEST_TIMEOUT after they are put.  On the device path the requests are decoded on the device, so
+ * the check runs there: the engine keeps a key table in HBM, and the responses stay with the host app, which names
+ * each one by a `handle` of its choosing.  A Java adapter calls gpx_response_cache_put after Replicable.execute and
+ * gpx_response_cache_match between the request decoders and gpx_propose_device.
+ *
+ * Key identity: (gid, generation, req_id, client address) -- RequestPacket.equals :1489-1510 within one group.  The
+ * generation of a gid starts at 0 and rises by one each time gpx_set_group_names names it (0 for every gid of an
+ * engine that has no name state).  So an entry stops matching once its group is destroyed, paused, re-created or
+ * loaded and then named again, where the reference would answer from it until it expires: a deliberate difference, a
+ * response belongs to the group state that produced it.  client_port 0 means "no address" and equals only another
+ * port 0 (Java's null == null); client_ip is then not read.
+ *
+ * Table: n_buckets buckets of 8 cells; a key's bucket is the low bits of
+ *   splitmix64(req_id ^ splitmix64((uint64)gid << 32 | generation) ^ splitmix64((uint64)ip_be32 << 16 | port))
+ * and a key never moves to another bucket.  A cell is expired when now_ms - put_ms >= timeout_ms.  A full bucket
+ * costs only missed hits: a miss is proposed as it would be without the cache. */
+typedef struct gpx_rc_key { /* 24 B: one executed client request */
+  uint32_t gid;
+  int32_t handle;         /* >= 0: the host's name for the cached response */
+  int64_t req_id;
+  uint8_t client_ip[4];   /* as gpx_wire_req_meta */
+  uint16_t client_port;   /* 0 = no client address */
+  uint16_t pad;
+} gpx_rc_key;
+
+/* Allocate the table: n_buckets (a power of two, at most 2^24; anything else is GPX_EINVAL) and timeout_ms (>= 0, the
+ * host's REQUEST_TIMEOUT * 1000).  Calling it again clears the table.  gpx_response_cache_put and _match before it are
+ * GPX_EINVAL. */
+int gpx_response_cache_init(gpx_engine* e, uint32_t n_buckets, int64_t timeout_ms);
+
+/* outstanding.responses.put of executed :318-322 for keys[n] (device), at now_ms.  Keys apply in input order; in its
+ * bucket a key replaces the lowest live cell with the same key, else takes the lowest free or expired cell, else
+ * evicts the cell with the smallest put time (the lowest such cell).  A negative handle or a gid >= max_groups is
+ * GPX_EINVAL, and nothing is written.  Stream-ordered on `stream` (NULL = the engine's stream) with the wire calls;
+ * one synchronisation reads the check. */
+int gpx_response_cache_put_device(gpx_engine* e, uint32_t n, const gpx_rc_key* keys, int64_t now_ms, void* stream);
+
+/* handleIncomingPacket :1084 + retransmittedRequest :332 for reqs[n] and meta[n] (device; a request decoder's output).
+ * reqs[q] is a hit when no other request of the call has the same `client` value (the request decoders set it to the
+ * packet or member index, so a request unrolled from a batched RequestPacket is never a hit), its gid has a name or
+ * the engine has no name state, and a live cell holds its key, the address read from meta[q].
+ *   hit[n] (device): the cell's handle for a hit, -1 for a miss.
+ *   out_reqs, out_meta (device, room for n each): the misses in input order, so gpx_propose_device can take them as
+ *     they are; *n_out (a HOST pointer) receives their count.
+ * The table is read as it was before the call (a retransmission in the batch of its original is a miss); match never
+ * inserts.  Stream-ordered as put; one synchronisation reads *n_out. */
+int gpx_response_cache_match_device(gpx_engine* e, uint32_t n, const gpx_request_rec* reqs,
+                                    const gpx_wire_req_meta* meta, int64_t now_ms, int32_t* hit,
+                                    gpx_request_rec* out_reqs, gpx_wire_req_meta* out_meta, uint32_t* n_out,
+                                    void* stream);
 
 /* ---- helpers shared with the reference semantics ---------------------------------- */
 int32_t gpx_java_string_hash(const char* s, size_t len); /* String.hashCode() */
