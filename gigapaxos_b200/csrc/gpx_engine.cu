@@ -48,6 +48,8 @@ static int fail(int code, const std::string& msg) {
 
 static inline uint32_t cdiv(uint64_t a, uint32_t b) { return (uint32_t)((a + b - 1) / b); }
 
+#include "gpx_wire_seq.h"
+
 struct gpx_engine {
   gpx_config cfg;
   DevState S;

@@ -11,8 +11,8 @@
  * leaves its bucket.  A cell is live while its handle is >= 0 and now_ms - put_ms < timeout_ms.
  *
  * Every kernel here is scalar -- one thread per key, per request or per bucket run, plain loads and stores -- so
- * tests/emu compiles this file for the host.  The stable sorts and the scan between the launches are CUB's on the
- * device (gpx_respcache_host.inc) and the standard library's in the emulation.
+ * tests/emu compiles this file for the host.  The stable sorts and the scan between the launches are gpx_wire_seq.h's
+ * rc_put and rc_match, run with CUB on the device and with the standard library in the emulation.
  */
 #pragma once
 #include "gpx_wire_dev.cuh"

@@ -11,7 +11,8 @@
  *
  * Every kernel here is scalar -- one thread per packet, per record or per coalesced run, plain loads and stores over
  * gpx_dev.cuh's state -- so tests/emu compiles this file for the host.  The scans that size the outputs and the stable
- * sorts by gid run between the launches (CUB on the device, the standard library in the emulation).
+ * sorts by gid run between the launches, in the sequences of gpx_wire_seq.h (CUB on the device, the standard library
+ * in the emulation).
  */
 #pragma once
 #include "gpx_dev.cuh"

@@ -20,8 +20,8 @@
  *                  member (so the PP array is validated in parallel), looks the name up, writes its status and record
  *                  counts; pass 1 writes its records.
  *   k_json_fix     drops the members of packets a member found malformed.
- * The scans between the launches, the stable radix sort by gid and the gather (k_wire_gather) run on the host side
- * (gpx_wire_host.inc with CUB, the standard library in tests/emu/wire_json_emu.cpp).  Every kernel is scalar, with byte
+ * The scans between the launches, the stable radix sort by gid and the gather (k_wire_gather) are gpx_wire_seq.h's
+ * wire_decode_json, run with CUB on the device and with the standard library in tests/emu.  Every kernel is scalar, with byte
  * loads only, so the emulation compiles this file for the host with any chunk size.
  */
 #pragma once

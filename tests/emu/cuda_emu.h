@@ -7,7 +7,7 @@
  * <cuda_runtime.h> is host-compilable (g++): it brings int4 / make_int4 / uint3 and defines __device__, __global__,
  * __forceinline__ ... away.  What is left: the built-in index variables (declared `extern const` there, so they are
  * renamed to mutable globals), the few device-only names gpx_dev.cuh mentions in functions the emulated kernels never
- * call, and atomicAdd.
+ * call, and the atomics (atomicAdd, atomicMax, atomicMin, atomicCAS).
  */
 #pragma once
 #include <cuda_runtime.h>
@@ -48,6 +48,20 @@ template <class T>
 static inline T atomicMax(T* p, T v) {
   T old = *p;
   if (v > old) *p = v;
+  return old;
+}
+
+template <class T>
+static inline T atomicMin(T* p, T v) {
+  T old = *p;
+  if (v < old) *p = v;
+  return old;
+}
+
+template <class T>
+static inline T atomicCAS(T* p, T cmp, T v) {
+  T old = *p;
+  if (old == cmp) *p = v;
   return old;
 }
 

@@ -1,22 +1,11 @@
 /*
- * wire_emu.cpp -- k_names_*, k_wire_decode, k_wire_req_decode and the k_wire_enc_* kernels
- * (gigapaxos_b200/csrc/gpx_wire_dev.cuh, the source the GPU runs) compiled for the host over cuda_emu.h; see
- * p1b_emu.cpp.  The scans and the stable sorts by gid that gpx_wire_host.inc does with CUB are done here with the
- * standard library.  Test infrastructure only.
+ * wire_emu.cpp -- the wire calls' kernels (gigapaxos_b200/csrc/gpx_wire_*.cuh, the source the GPU runs) compiled for the
+ * host over cuda_emu.h, and driven by the product's own host sequences (gpx_wire_seq.h) on the CPU executor of
+ * wire_exec.h.  This file holds the world the kernels read (engine state, member sets, the name table) and the byte
+ * codec's calls; wire_json_emu.cpp, wire_fwd_emu.cpp, wire_json_out_emu.cpp and wire_json_sweep_emu.cpp add the
+ * others over the same world.  Test infrastructure only.
  */
-#include "cuda_emu.h"
-
-template <class T>
-static inline T atomicCAS(T* p, T cmp, T v) { /* one thread at a time */
-  T old = *p;
-  if (old == cmp) *p = v;
-  return old;
-}
-
-#include "gpx_wire_dev.cuh"
-
-#include <numeric>
-#include <vector>
+#include "wire_exec.h"
 
 struct EmuWire {
   DevState S;
@@ -110,170 +99,87 @@ extern "C" void emu_wire_names_rehash(void* p) {
   emu_launch(k_names_rehash, (x->S.G + 63) / 64, 64, x->W, x->S.G);
 }
 
-static std::vector<uint32_t> stable_order(const std::vector<uint32_t>& key) {
-  std::vector<uint32_t> perm(key.size());
-  std::iota(perm.begin(), perm.end(), 0u);
-  std::stable_sort(perm.begin(), perm.end(), [&](uint32_t a, uint32_t b) { return key[a] < key[b]; });
-  return perm;
-}
-/* records into a stable order: dst[i] = src[perm[i]] */
-template <class T>
-static void gather(const std::vector<uint32_t>& perm, const std::vector<T>& src, T* dst) {
-  for (size_t i = 0; i < perm.size(); i++) dst[i] = src[perm[i]];
-}
-static void exclusive_rows(const std::vector<uint32_t>& cnt, std::vector<uint32_t>& off, uint32_t n, uint32_t rows,
-                           uint64_t* tot) {
-  for (uint32_t j = 0; j < rows; j++) {
-    uint64_t s = 0;
-    for (uint32_t i = 0; i < n; i++) {
-      off[(size_t)j * n + i] = (uint32_t)s;
-      s += cnt[(size_t)j * n + i];
-    }
-    tot[j] = s;
+/* live groups gids[0..n) with one member set m[0..R) (sorted ascending), interned once as gpx_create_groups interns
+ * it: worlds of more groups than there are member-set slots */
+extern "C" int emu_wire_groups_alike(void* p, uint32_t n, const uint32_t* gids, uint32_t R, const int32_t* m) {
+  EmuWire* x = static_cast<EmuWire*>(p);
+  if (n == 0) return 0;
+  if (emu_wire_group(p, gids[0], R, m)) return -1;
+  for (uint32_t k = 1; k < n; k++) {
+    if (gids[k] >= x->S.G) return -1;
+    x->meta[gids[k]] = x->meta[gids[0]];
   }
+  return 0;
 }
 
-/* gpx_wire_decode_batch without the copies; sizes[4] = {accepts, blob bytes, replies, decisions} are capacities in,
- * sizes out; returns -5 (GPX_ERANGE) when an output is too small */
+/* the rows propose_route reads, [L][G] each (the caller keeps them alive), and RequestBatcher's settings */
+extern "C" void emu_fwd_state(void* p, int4* acc_row, uint32_t* acc_aux, int4* coord_row, int32_t batching,
+                              int32_t max_batch_size, int32_t size_est, long long max_batch_bytes) {
+  EmuWire* x = static_cast<EmuWire*>(p);
+  x->S.acc_row = acc_row;
+  x->S.acc_aux = acc_aux;
+  x->S.coord_row = coord_row;
+  x->S.batching = batching;
+  x->S.max_batch_size = max_batch_size;
+  x->S.size_est = size_est;
+  x->S.max_batch_bytes = max_batch_bytes;
+}
+
+/* gpx_wire_decode_batch_device; sizes[4] = {accepts, blob bytes, replies, decisions} are capacities in, sizes out */
 extern "C" int emu_wire_decode(void* p, uint32_t n, const uint8_t* bytes, uint64_t n_bytes, const gpx_wire_ref* pkts,
                                int32_t* status, gpx_accept_rec* acc, uint8_t* blob, gpx_accept_reply_rec* rep,
                                gpx_decision_rec* dec, uint64_t* sizes, uint32_t block) {
   EmuWire* x = static_cast<EmuWire*>(p);
-  std::vector<uint32_t> cnt((size_t)WD_NCNT * n + 1), off((size_t)WD_NCNT * n + 1);
-  WireDecodeArgs A;
-  memset(&A, 0, sizeof A);
-  A.bytes = bytes;
-  A.pkts = pkts;
-  A.n_bytes = n_bytes;
-  A.n = n;
-  A.cnt = cnt.data();
-  A.off = off.data();
-  A.status = status;
-  emu_launch(k_wire_decode, (n + block - 1) / block, block, x->S, x->W, A);
-  uint64_t tot[WD_NCNT];
-  exclusive_rows(cnt, off, n, WD_NCNT, tot);
-  bool small = false;
-  for (int j = 0; j < WD_NCNT; j++) {
-    small = small || tot[j] > sizes[j];
-    sizes[j] = tot[j];
-  }
-  if (small) return GPX_ERANGE;
-  std::vector<gpx_accept_rec> sa(tot[WD_ACC] + 1);
-  std::vector<gpx_accept_reply_rec> sr(tot[WD_REP] + 1);
-  std::vector<gpx_decision_rec> sd(tot[WD_DEC] + 1);
-  std::vector<uint32_t> ka(tot[WD_ACC]), kr(tot[WD_REP]), kd(tot[WD_DEC]);
-  A.acc = sa.data();
-  A.blob = blob;
-  A.rep = sr.data();
-  A.dec = sd.data();
-  A.acc_key = ka.data();
-  A.rep_key = kr.data();
-  A.dec_key = kd.data();
-  A.emit = 1;
-  emu_launch(k_wire_decode, (n + block - 1) / block, block, x->S, x->W, A);
-  gather(stable_order(ka), sa, acc);
-  gather(stable_order(kr), sr, rep);
-  gather(stable_order(kd), sd, dec);
-  return 0;
+  EmuExec ex{block};
+  EmuCall call;
+  uint32_t na = cap32(sizes[0]), nr = cap32(sizes[2]), nd = cap32(sizes[3]);
+  const int rc = wire_decode(ex, call, ex.env(x->S, x->W), n, bytes, n_bytes, pkts, status, acc, &na, blob, &sizes[1],
+                             rep, &nr, dec, &nd);
+  sizes[0] = na;
+  sizes[2] = nr;
+  sizes[3] = nd;
+  return rc;
 }
 
-/* gpx_wire_decode_requests_device without the copies; sizes[2] = {requests, payload bytes} in / out; GPX_ERANGE when
- * an output is too small (nothing but status written then) */
+/* gpx_wire_decode_requests_device; sizes[2] = {requests, payload bytes} in / out */
 extern "C" int emu_wire_decode_requests(void* p, uint32_t n, const uint8_t* bytes, uint64_t n_bytes,
                                         const gpx_wire_ref* pkts, int64_t now_ms, int32_t* status,
                                         gpx_request_rec* reqs, gpx_wire_req_meta* meta, uint8_t* payload,
                                         uint64_t* sizes, uint32_t block) {
   EmuWire* x = static_cast<EmuWire*>(p);
-  std::vector<uint32_t> cnt((size_t)WQ_NCNT * n + 1), off((size_t)WQ_NCNT * n + 1);
-  WireReqDecodeArgs A;
-  memset(&A, 0, sizeof A);
-  A.bytes = bytes;
-  A.pkts = pkts;
-  A.n_bytes = n_bytes;
-  A.n = n;
-  A.now_ms = now_ms;
-  A.cnt = cnt.data();
-  A.off = off.data();
-  A.status = status;
-  emu_launch(k_wire_req_decode, (n + block - 1) / block, block, x->S, x->W, A);
-  uint64_t tot[WQ_NCNT];
-  exclusive_rows(cnt, off, n, WQ_NCNT, tot);
-  const bool small = tot[WQ_REQ] > sizes[0] || tot[WQ_PAY] > sizes[1];
-  sizes[0] = tot[WQ_REQ];
-  sizes[1] = tot[WQ_PAY];
-  if (small) return GPX_ERANGE;
-  const size_t nq = tot[WQ_REQ];
-  std::vector<gpx_request_rec> sq(nq + 1);
-  std::vector<gpx_wire_req_meta> sm(nq + 1);
-  std::vector<uint32_t> key(nq);
-  A.req = sq.data();
-  A.meta = sm.data();
-  A.key = key.data();
-  A.payload = payload;
-  A.emit = 1;
-  emu_launch(k_wire_req_decode, (n + block - 1) / block, block, x->S, x->W, A);
-  const std::vector<uint32_t> perm = stable_order(key);
-  gather(perm, sq, reqs);
-  gather(perm, sm, meta);
-  return 0;
+  EmuExec ex{block};
+  EmuCall call;
+  uint32_t nq = cap32(sizes[0]);
+  const int rc = wire_decode_requests(ex, call, ex.env(x->S, x->W), n, bytes, n_bytes, pkts, now_ms, status, reqs, meta,
+                                      &nq, payload, &sizes[1]);
+  sizes[0] = nq;
+  return rc;
 }
 
-enum { EMU_ENC_REPLIES = 0, EMU_ENC_DECISIONS = 1, EMU_ENC_ACCEPTS = 2 };
-
-/* gpx_wire_encode_replies (kind 0: n records of n_lanes), gpx_wire_encode_decisions (1) or
- * gpx_wire_encode_accepts_device (2, the ACCEPTs' requests at heads .. payload) without the copies.  The keys, the sort
- * and the passes run over n records; n_ptr, when not null, is the record count as the device reads it.  sizes[2] =
- * {bytes, refs} in / out. */
+/* gpx_wire_encode_replies_device (kind 0: n records of n_lanes), gpx_wire_encode_decisions_device (1) or
+ * gpx_wire_encode_accepts_device (2, the ACCEPTs' requests at heads .. payload); n_ptr, when not null, is the record
+ * count as the device reads it.  sizes[2] = {bytes, refs} in / out. */
 extern "C" int emu_wire_encode(void* p, int kind, const uint32_t* n_ptr, uint32_t n, const void* recs,
                                const uint32_t* heads, const gpx_request_rec* reqs, const gpx_wire_req_meta* meta,
                                uint32_t n_reqs, const uint8_t* payload, uint8_t* rstatus, uint8_t* out,
                                gpx_wire_ref* refs, uint64_t* sizes, uint32_t block) {
   EmuWire* x = static_cast<EmuWire*>(p);
-  std::vector<uint32_t> key(n + 1), perm, skey(n + 1), cnt(2 * (size_t)n + 1), off(2 * (size_t)n + 1);
-  WireEncodeArgs A;
-  memset(&A, 0, sizeof A);
-  A.recs = recs;
-  A.n = n;
-  A.n_lanes = x->S.L;
-  A.rstatus = rstatus;
-  A.key = key.data();
-  A.n_ptr = n_ptr;
-  WireAccArgs X;
-  X.head = heads;
-  X.reqs = reqs;
-  X.meta = meta;
-  X.n_reqs = n_reqs;
-  X.payload = payload;
-  const uint32_t grid = (n + block - 1) / block;
-  const auto launch = [&](bool keys) {
-    if (kind == EMU_ENC_REPLIES)
-      keys ? emu_launch(k_wire_enc_keys_replies, grid, block, x->S, x->W, A)
-           : emu_launch(k_wire_enc_replies, grid, block, x->S, x->W, A);
-    else if (kind == EMU_ENC_DECISIONS)
-      keys ? emu_launch(k_wire_enc_keys_decisions, grid, block, x->S, x->W, A)
-           : emu_launch(k_wire_enc_decisions, grid, block, x->S, x->W, A);
-    else
-      keys ? emu_launch(k_wire_enc_keys_accepts, grid, block, x->S, x->W, A, X)
-           : emu_launch(k_wire_enc_accepts, grid, block, x->S, x->W, A, X);
-  };
-  launch(true);
-  key.resize(n);
-  perm = stable_order(key);
-  for (uint32_t i = 0; i < n; i++) skey[i] = key[perm[i]];
-  A.perm = perm.data();
-  A.skey = skey.data();
-  A.cnt = cnt.data();
-  A.off = off.data();
-  launch(false);
-  uint64_t tot[2];
-  exclusive_rows(cnt, off, n, 2, tot);
-  const bool small = tot[0] > sizes[0] || tot[1] > sizes[1];
-  sizes[0] = tot[0];
-  sizes[1] = tot[1];
-  if (small) return GPX_ERANGE;
-  A.out = out;
-  A.refs = refs;
-  A.emit = 1;
-  launch(false);
-  return 0;
+  EmuExec ex{block};
+  EmuCall call;
+  /* with a device count of 0 a test may hand in no records and no heads at all; the entry point wants buffers there,
+   * so empty ones stand in, and AddressSanitizer traps any read of them */
+  const std::unique_ptr<uint32_t[]> none(new uint32_t[0]);
+  if (!recs) recs = none.get();
+  if (!heads) heads = none.get();
+  WireAccArgs Q;
+  Q.head = heads;
+  Q.reqs = reqs;
+  Q.meta = meta;
+  Q.n_reqs = n_reqs;
+  Q.payload = payload;
+  uint32_t nr = cap32(sizes[1]);
+  const int rc = wire_encode(ex, call, ex.env(x->S, x->W), (WireEnc)kind, n, n_ptr, recs, Q, rstatus, out, &sizes[0],
+                             refs, &nr);
+  sizes[1] = nr;
+  return rc;
 }

@@ -1,119 +1,38 @@
 /*
- * wire_json_out_emu.cpp -- the kernels of gigapaxos_b200/csrc/gpx_wire_json_enc.cuh (the source the GPU runs) compiled
- * for the host over cuda_emu.h, beside the byte codec (wire_emu.cpp) and the JSON decoder (wire_json_emu.cpp) on the
- * same engine state, so one world serves all three.  The stable radix sorts, the scans and the scan by key that
- * gpx_wire_host.inc does with CUB are done here with the standard library.  Test infrastructure only.
+ * wire_json_out_emu.cpp -- gpx_wire_encode_json_sweep_device's sequence over the kernels of
+ * gigapaxos_b200/csrc/gpx_wire_json_enc.cuh on the CPU executor, beside the byte codec (wire_emu.cpp) and the JSON
+ * decoder (wire_json_emu.cpp) on the same world.  emu_wire_encode_json is the sweep without requests, as
+ * gpx_wire_encode_json_device is.  Test infrastructure only.
  */
 #include "wire_json_emu.cpp"
 
-template <class T>
-static inline T atomicMin(T* p, T v) { /* one thread at a time */
-  T old = *p;
-  if (v < old) *p = v;
-  return old;
+/* sizes[2] = {bytes, refs} capacities in, sizes out.  Returns 0, GPX_ERANGE (sizes reported, no packet written) or
+ * GPX_EINVAL (wrap_bytes out of range, n_replies not a multiple of n_lanes, an oversized reply or commit member). */
+extern "C" int emu_wire_encode_json_sweep(void* p, uint32_t nr, const gpx_accept_reply_rec* rep,
+                                          const gpx_decision_rec* dec, const uint32_t* n_dec_ptr, uint32_t nd,
+                                          const gpx_request_rec* reqs, const gpx_wire_req_meta* meta, uint32_t nq,
+                                          const int32_t* status, const uint8_t* payload, uint32_t n_down,
+                                          const int32_t* down, uint8_t* rst_r, uint8_t* rst_d, uint8_t* rst_q,
+                                          uint64_t wrap_bytes, uint8_t* out, gpx_wire_ref* refs, uint64_t* sizes,
+                                          uint32_t block) {
+  EmuWire* x = static_cast<EmuWire*>(p);
+  EmuExec ex{block};
+  EmuCall call;
+  JsonSetTable T; /* the recipient sets of the world's member sets, as gpx_wire_host.inc's json_sets builds them */
+  T.grow(x->msets.data(), x->msets.size());
+  const JsonSets Z = {T.of_mset.data(), T.one.data(), T.nodes.data(), T.count.data(), (uint32_t)T.count.size()};
+  uint32_t n_refs = cap32(sizes[1]);
+  const int rc = wire_encode_json_sweep(ex, call, ex.env(x->S, x->W), Z, nr, rep, dec, n_dec_ptr, nd, reqs, meta, nq,
+                                        status, payload, n_down, down, rst_r, rst_d, rst_q, wrap_bytes, out, &sizes[0],
+                                        refs, &n_refs);
+  sizes[1] = n_refs;
+  return rc;
 }
 
-#include "gpx_wire_json_enc.cuh"
-
-/* gpx_wire_encode_json_device without the copies: sizes[2] = {bytes, refs} capacities in, sizes out.  Returns 0,
- * -5 (GPX_ERANGE: sizes reported, no packet written) or -1 (GPX_EINVAL: wrap_bytes out of range, an oversized
- * member).  n_dec_ptr, when not null, is the decision count as the device reads it. */
 extern "C" int emu_wire_encode_json(void* p, uint32_t nr, const gpx_accept_reply_rec* rep, const gpx_decision_rec* dec,
                                     const uint32_t* n_dec_ptr, uint32_t nd, uint8_t* rst_r, uint8_t* rst_d,
                                     uint64_t wrap_bytes, uint8_t* out, gpx_wire_ref* refs, uint64_t* sizes,
                                     uint32_t block) {
-  EmuWire* x = static_cast<EmuWire*>(p);
-  if (wrap_bytes == 0) wrap_bytes = GPX_JSON_WRAP_BYTES;
-  if (wrap_bytes > GPX_JSON_WRAP_BYTES || wrap_bytes <= GPX_JSON_WRAP_OVERHEAD + GPX_JSON_MAX_MEMBER) return GPX_EINVAL;
-  const uint32_t n = nr + nd, L = x->S.L;
-  if (n == 0) {
-    sizes[0] = sizes[1] = 0;
-    return 0;
-  }
-  JsonSetTable T;
-  T.grow(x->msets.data(), x->msets.size());
-  std::vector<uint32_t> rkey(nr + 1), rperm, rskey(nr + 1), dkey(nd + 1), dperm, dskey(nd + 1),
-      first((size_t)L * T.count.size(), GPX_JSON_ENC_NONE), mset(n), msize(n), order, val(n), start(n),
-      cnt((size_t)JE_NCNT * n), off((size_t)JE_NCNT * n), ncnt(2ull * nr + 1), noff(2ull * nr + 1);
-  std::vector<uint8_t> mlane(n);
-  std::vector<unsigned long long> key(n), skey(n);
-  std::vector<uint2> wbeg(n);
-  WireJsonEncArgs A;
-  memset(&A, 0, sizeof A);
-  for (int k = 0; k < 2; k++) {
-    WireEncodeArgs& X = k ? A.D : A.R;
-    X.recs = k ? (const void*)dec : (const void*)rep;
-    X.n = k ? nd : nr;
-    X.n_lanes = L;
-    X.rstatus = k ? rst_d : rst_r;
-    X.n_ptr = k ? n_dec_ptr : nullptr;
-    X.key = (k ? dkey : rkey).data();
-  }
-  A.Z = {T.of_mset.data(), T.one.data(), T.nodes.data(), T.count.data(), (uint32_t)T.count.size()};
-  A.n = n;
-  A.L = L;
-  A.T = (uint32_t)(wrap_bytes - GPX_JSON_WRAP_OVERHEAD - GPX_JSON_MAX_MEMBER);
-  A.first = first.data();
-  A.mset = mset.data();
-  A.mlane = mlane.data();
-  A.msize = msize.data();
-  A.key = key.data();
-  A.val = val.data();
-  A.cnt = cnt.data();
-  A.ncnt = ncnt.data();
-  A.wbeg = wbeg.data();
-  const auto grid = [&](uint32_t k) { return (k + block - 1) / block; };
-  /* the byte encoders' keys and stable sorts */
-  if (nr) {
-    emu_launch(k_wire_enc_keys_replies, grid(nr), block, x->S, x->W, A.R);
-    rkey.resize(nr);
-    rperm = stable_order(rkey);
-    for (uint32_t i = 0; i < nr; i++) rskey[i] = rkey[rperm[i]];
-    A.R.perm = rperm.data();
-    A.R.skey = rskey.data();
-  }
-  if (nd) {
-    emu_launch(k_wire_enc_keys_decisions, grid(nd), block, x->S, x->W, A.D);
-    dkey.resize(nd);
-    dperm = stable_order(dkey);
-    for (uint32_t i = 0; i < nd; i++) dskey[i] = dkey[dperm[i]];
-    A.D.perm = dperm.data();
-    A.D.skey = dskey.data();
-  }
-  if (nr) emu_launch(k_json_enc_nacks, grid(nr), block, x->S, x->W, A);
-  emu_launch(k_json_enc_members, grid(n), block, x->S, x->W, A);
-  emu_launch(k_json_enc_keys, grid(n), block, A);
-  order.resize(n);
-  std::iota(order.begin(), order.end(), 0u);
-  std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return key[a] < key[b]; });
-  for (uint32_t j = 0; j < n; j++) skey[j] = key[order[j]];
-  A.skey = skey.data();
-  A.order = order.data();
-  emu_launch(k_json_enc_vals, grid(n), block, A);
-  for (uint32_t j = 0, s = 0; j < n; j++) { /* exclusive sum by key */
-    if (j == 0 || skey[j] != skey[j - 1]) s = 0;
-    start[j] = s;
-    s += val[j];
-  }
-  A.start = start.data();
-  emu_launch(k_json_enc_cut, grid(n), block, A);
-  uint64_t tot[JE_NCNT], ntot[2] = {0, 0};
-  exclusive_rows(cnt, off, n, JE_NCNT, tot);
-  if (nr) exclusive_rows(ncnt, noff, nr, 2, ntot);
-  A.off = off.data();
-  A.noff = noff.data();
-  if (tot[JE_BIG]) return GPX_EINVAL;
-  const uint64_t bytes = tot[JE_BYTES] + ntot[0], n_refs = tot[JE_REFS] + ntot[1];
-  const bool small = bytes > sizes[0] || n_refs > sizes[1];
-  sizes[0] = bytes;
-  sizes[1] = n_refs;
-  if (small) return GPX_ERANGE;
-  A.nack_bytes = (uint32_t)ntot[0];
-  A.n_nacks = (uint32_t)ntot[1];
-  A.out = out;
-  A.refs = refs;
-  if (A.n_nacks) emu_launch(k_json_enc_emit_nacks, grid(nr), block, x->S, x->W, A);
-  emu_launch(k_json_enc_emit, grid(n), block, x->S, x->W, A);
-  emu_launch(k_json_enc_refs, grid(n), block, A);
-  return 0;
+  return emu_wire_encode_json_sweep(p, nr, rep, dec, n_dec_ptr, nd, nullptr, nullptr, 0, nullptr, nullptr, 0, nullptr,
+                                    rst_r, rst_d, nullptr, wrap_bytes, out, refs, sizes, block);
 }
