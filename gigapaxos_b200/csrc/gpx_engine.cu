@@ -624,7 +624,10 @@ static inline void log_flip(gpx_engine* e) { e->S.lp ^= 1u; }
  *     k_round_g<L, true> (launch_round; round_on_stream settles ahead of its timing events);
  *   - prepares and prepare replies, create, destroy, patch, dump / load rows, get / select / clear group flags,
  *     missing decisions, pause, unpause and spread rounds.
- * Calls that touch only the log rings, counters, group names or wire bytes do not. */
+ * Calls that touch only the log rings, counters, group names or wire bytes do not.  Nor do the forwards encoders
+ * (gpx_wire_encode_forwards_device, gpx_wire_encode_json_sweep_device: k_wire_fwd, k_json_enc_fwd), although they
+ * read the planes: their propose_route reads only the ballots and the EXISTS bit of acc_row and coord_row, which a
+ * VALID record never changes.  tests/test_lockstep_audit.py lists every kernel that reaches the planes and why. */
 static bool def_config(const DevState& S) { /* the reference's default configuration: k_round*<..., DEF = true> */
   return S.journaling && S.gc_majority_executed && S.log_meta && !S.cpi_per_group;
 }
