@@ -111,7 +111,7 @@ struct DevState {
    * launch), so nobody needs to know when the other blocks have read -- no ticket, no fence, no trailing kernel */
   unsigned long long* log_pos;   /* [2][GPX_MAX_LANES][2] */
   uint32_t lp;                   /* which copy this launch reads */
-  uint32_t ls_off; /* the lockstep records (ls_rec below) start at acc_row + ls_off; 0: the engine keeps none.  It
+  uint32_t ls_off; /* the lockstep records (ls_rec, ls_hot below) start at acc_row + ls_off; 0: the engine keeps none. It
                     * fills the padding in front of cur_seg: no other field and no kernel parameter moves */
   unsigned long long* cur_seg;   /* [L] segment bases of the round in flight (k_round -> k_round_slow) */
   unsigned long long* ctr;       /* [GPX_CTR_STRIPES][C_NCTR] */
@@ -206,21 +206,31 @@ __device__ __forceinline__ void ns_put(const DevState& S, uint32_t c, uint32_t g
 }
 
 /*
- * Lockstep record of a group, ls_rec(S, gid)[0..1]: {acc_slot, bnum, bcoord, gc_slot}, {aux, ns_cl, ctl, 0} with
- * ctl = GPX_LS_VALID | cl << 8.  Only k_round_g<L, true> reads and writes it, so that a group whose co-located lanes
- * advance in lockstep moves one 32-byte sector per round instead of its per-lane planes.  While VALID is set:
- *   - every lane's acc_row is the record's row, coord_row[cl] is {bnum, bcoord, acc_slot, EXISTS | ACTIVE} and
- *     ns_u[cl] is ns_cl (never GPX_NS_MIXED, so node_slots[cl] is stale as the ns_u rule says); those acc_row,
- *     coord_row[cl] and ns_u[cl] words of the gid are STALE;
+ * Lockstep record of a group, in two parts: the cold record ls_rec(S, gid) = {bnum, bcoord, aux, ctl} with
+ * ctl = GPX_LS_VALID | cl << 8, and three hot planes of one word per gid, ls_hot(S, GPX_LS_SLOT / GPX_LS_GC /
+ * GPX_LS_NS)[gid] = acc_slot, gc_slot and ns_cl.  Only k_round_g<L, true> reads and writes them, so that a group whose
+ * co-located lanes advance in lockstep moves 28 bytes per round instead of its per-lane planes.  An in-order round
+ * changes only the hot words: a record that stays VALID has its cold part read and never written back, and the hot
+ * words sit in arrays of their own so that their stores fill whole sectors.  While VALID is set:
+ *   - every lane's acc_row is {acc_slot, bnum, bcoord, gc_slot}, coord_row[cl] is {bnum, bcoord, acc_slot,
+ *     EXISTS | ACTIVE} and ns_u[cl] is ns_cl (never GPX_NS_MIXED, so node_slots[cl] is stale as the ns_u rule says);
+ *     those acc_row, coord_row[cl] and ns_u[cl] words of the gid are STALE;
  *   - every lane's acc_aux equals aux, every acc_dirty is 0 and no lane other than cl has a coordinator row with
  *     EXISTS: these words are current, the record caches them.
- * The cache is sound because nothing else writes those words without settling first: k_round_g writes the planes
- * back and clears VALID before it leaves such a group to k_round_slow, and the host runs k_ls_settle (every VALID
- * record -> planes) before any other launch that reads or writes group state.
+ * While VALID is clear the hot words mean nothing.  The cache is sound because nothing else writes those words without
+ * settling first: k_round_g writes the planes back and clears VALID before it leaves such a group to k_round_slow,
+ * and the host runs k_ls_settle (every VALID record -> planes) before any other launch that reads or writes group
+ * state.
  */
 #define GPX_LS_VALID 1u
-/* one 32-byte sector per gid behind the acceptor rows, in their allocation (ls_off is even) */
-__device__ __forceinline__ int4* ls_rec(const DevState& S, uint32_t gid) { return S.acc_row + S.ls_off + 2u * gid; }
+enum { GPX_LS_SLOT = 0, GPX_LS_GC = 1, GPX_LS_NS = 2 };
+/* Behind the acceptor rows, in their allocation: G cold records of 16 B at acc_row + ls_off (ls_off is even, so they
+ * start 32-byte aligned), then the three hot planes of G words each.  ls_int4s is the allocation's size in int4. */
+__host__ __device__ __forceinline__ size_t ls_int4s(size_t G) { return G + (3 * G + 3) / 4; }
+__device__ __forceinline__ int4* ls_rec(const DevState& S, uint32_t gid) { return S.acc_row + S.ls_off + gid; }
+__device__ __forceinline__ int* ls_hot(const DevState& S, uint32_t plane) {
+  return reinterpret_cast<int*>(S.acc_row + S.ls_off + S.G) + (size_t)plane * S.G;
+}
 
 /* PISM :456-460: only an ACTIVE acceptor handles packets */
 __device__ __forceinline__ bool st_usable(uint32_t aux) {

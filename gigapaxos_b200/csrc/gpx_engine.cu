@@ -260,7 +260,7 @@ int gpx_engine_create(const gpx_config* cfg, gpx_engine** out) {
   }
   /* k_round_g's lockstep records (gpx_dev.cuh) follow the acceptor rows, 32-byte aligned (cudaMalloc: 256) */
   if (L <= GPX_GROUND_MAXL) S.ls_off = (uint32_t)((L * G + 1) & ~(size_t)1);
-  TRY(e->dalloc(&S.acc_row, S.ls_off ? S.ls_off + 2 * G : L * G));
+  TRY(e->dalloc(&S.acc_row, S.ls_off ? S.ls_off + ls_int4s(G) : L * G));
   TRY(e->dalloc(&S.acc_aux, L * G));
   TRY(e->dalloc(&S.acc_win, 2 * L * W * G));
   TRY(e->dalloc(&S.acc_dirty, L * G));
@@ -298,7 +298,7 @@ int gpx_engine_create(const gpx_config* cfg, gpx_engine** out) {
     cudaMemset(S.com_win, 0, 2 * L * W * G * sizeof(int4));
     cudaMemset(S.prop_win, 0, L * W * G * sizeof(int4));
     cudaMemset(S.ns_u, 0, L * G * 4); /* compact, 0: what group creation writes */
-    if (S.ls_off) cudaMemset(S.acc_row + S.ls_off, 0, 2 * G * sizeof(int4));
+    if (S.ls_off) cudaMemset(S.acc_row + S.ls_off, 0, ls_int4s(G) * sizeof(int4));
   }
   for (size_t l = 0; l < GPX_MAX_LANES; l++) S.lane_node[l] = l < L ? cfg->lane_node[l] : INT32_MIN;
   S.cpi_const = cfg->checkpoint_interval;

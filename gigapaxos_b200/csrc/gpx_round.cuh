@@ -568,11 +568,11 @@ __device__ __forceinline__ void ls_write_planes(const DevState& S, uint32_t gid,
 __global__ void k_ls_settle(const __grid_constant__ DevState S) {
   const uint32_t gid = blockIdx.x * blockDim.x + threadIdx.x;
   if (gid >= S.G) return;
-  int4 r0, r1;
-  ld256(ls_rec(S, gid), r0, r1);
-  if (!((uint32_t)r1.z & GPX_LS_VALID)) return;
-  ls_write_planes(S, gid, S.L, r0, (uint32_t)r1.z >> 8, r1.y);
-  ls_rec(S, gid)[1] = make_int4(r1.x, r1.y, 0, 0);
+  const int4 c = *ls_rec(S, gid);
+  const int slot = ls_hot(S, GPX_LS_SLOT)[gid], gc = ls_hot(S, GPX_LS_GC)[gid], ns = ls_hot(S, GPX_LS_NS)[gid];
+  if (!((uint32_t)c.w & GPX_LS_VALID)) return;
+  ls_write_planes(S, gid, S.L, make_int4(slot, c.x, c.y, gc), (uint32_t)c.w >> 8, ns);
+  *ls_rec(S, gid) = make_int4(c.x, c.y, c.z, 0);
 }
 
 /*
@@ -582,7 +582,8 @@ __global__ void k_ls_settle(const __grid_constant__ DevState S) {
  * serves 32 adjacent groups, so every per-lane plane access (acc_row, acc_aux, coord_row, ns_u, the frame
  * records) is 32 x 4..16 B contiguous: whole lines per instruction.  The log images are staged per warp as in
  * k_round; a warp whose 32 groups all took the fast path stages its EXEC rows too and stores them as 16-byte pieces.
- * With DEF, a group whose lanes are in lockstep is read and written as its 32-byte lockstep record (ls_rec).
+ * With DEF, a group whose lanes are in lockstep is read as its lockstep record (ls_rec and the ls_hot words), and
+ * only the hot words are written while it stays in lockstep.
  */
 template <int L, bool DEF>
 __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const __grid_constant__ DevState S,
@@ -655,9 +656,18 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
   int4 pv = make_int4(0, 0, 0, 0);
   const uint8_t* const psrc = A.blob0 + poff;
   const bool pal = ((poff | (uint32_t)(uintptr_t)A.blob0) & 15u) == 0;
-  int4 ls0 = make_int4(0, 0, 0, 0), ls1 = ls0;
-  if (LS && head && gid < G) ld256(ls_rec(S, gid), ls0, ls1); /* every head: a VALID one is settled below */
-  const uint32_t ls_ctl = (uint32_t)ls1.z; /* GPX_LS_VALID | cl << 8, or 0 */
+  /* the record's row {acc_slot, bnum, bcoord, gc_slot}, its cold part {bnum, bcoord, aux, ctl} and ns_cl */
+  int4 ls0 = make_int4(0, 0, 0, 0), lcold = ls0;
+  int ls_ns = 0;
+  if (LS && head && gid < G) { /* every head: a VALID one is settled below */
+    lcold = *ls_rec(S, gid);
+    ls0.x = ls_hot(S, GPX_LS_SLOT)[gid];
+    ls0.w = ls_hot(S, GPX_LS_GC)[gid];
+    ls_ns = ls_hot(S, GPX_LS_NS)[gid];
+    ls0.y = lcold.x;
+    ls0.z = lcold.y;
+  }
+  const uint32_t ls_ctl = (uint32_t)lcold.w; /* GPX_LS_VALID | cl << 8, or 0 */
   if (cand) {
     meta = S.grp_meta[gid];
     if (plen) {
@@ -683,11 +693,11 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
 #pragma unroll
     for (int l = 0; l < L; l++) {
       arow[l] = ls0;
-      aux[l] = (uint32_t)ls1.x;
+      aux[l] = (uint32_t)lcold.z;
       dirty[l] = 0;
       crw[l] = (ls_ctl >> 8) == (uint32_t)l ? make_int4(ls0.y, ls0.z, ls0.x, (int)(GPX_CF_EXISTS | GPX_CF_ACTIVE))
                                             : make_int4(0, 0, 0, 0);
-      nsu[l] = ls1.y;
+      nsu[l] = ls_ns;
     }
   }
   bool sf = cand && ((meta & (GPX_META_LIVE | GPX_META_IDENT)) == (GPX_META_LIVE | GPX_META_IDENT)) &&
@@ -816,14 +826,20 @@ __global__ void __launch_bounds__(GPX_GBLOCK, GPX_GROUND_MINB) k_round_g(const _
     else
       RA.P.status[i] = slot;
     crow.z = (int)((unsigned)crow.z + 1u); /* PCS.propose: nextProposalSlotNumber++ */
-    if (lsc) /* crow is {row.y, row.z, row.x, EXISTS | ACTIVE} again */
-      st256(ls_rec(S, gid), lrow, make_int4((int)aux[0], mine, (int)(GPX_LS_VALID | (cl << 8)), 0));
-    else
+    if (lsc) { /* crow is {row.y, row.z, row.x, EXISTS | ACTIVE} again */
+      ls_hot(S, GPX_LS_SLOT)[gid] = lrow.x;
+      ls_hot(S, GPX_LS_GC)[gid] = lrow.w;
+      ls_hot(S, GPX_LS_NS)[gid] = mine;
+      /* a VALID record keeps its cold part: the fast path moves neither the ballot nor aux, and cl is the lane whose
+       * coordinator row the record holds */
+      if (!(ls_ctl & GPX_LS_VALID))
+        *ls_rec(S, gid) = make_int4(lrow.y, lrow.z, (int)aux[0], (int)(GPX_LS_VALID | (cl << 8)));
+    } else
       S.coord_row[cl * G + gid] = crow;
   } else if (head) {
     if (ls_ctl & GPX_LS_VALID) { /* settled before anything else sees the group's planes */
-      ls_write_planes(S, gid, L, ls0, ls_ctl >> 8, ls1.y);
-      ls_rec(S, gid)[1] = make_int4(ls1.x, ls1.y, 0, 0);
+      ls_write_planes(S, gid, L, ls0, ls_ctl >> 8, ls_ns);
+      *ls_rec(S, gid) = make_int4(lcold.x, lcold.y, lcold.z, 0);
     }
     round_hand_off<L, L>(S, RA, i);
   }

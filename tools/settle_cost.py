@@ -46,7 +46,7 @@ def settle_us(G: int, reps: int) -> dict:
             times.append(ks[0].device_time_total)
     e.close()
     return dict(groups=G, lanes=L, settle_us_median=statistics.median(times), settle_us=times,
-                record_bytes_read=32 * G)
+                record_bytes_read=28 * G)
 
 
 def main() -> int:
