@@ -9,6 +9,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+from collections import namedtuple
 from typing import Optional
 
 import numpy as np
@@ -20,6 +21,7 @@ GPX_MAX_WINDOW = 8
 
 # return codes
 GPX_OK, GPX_EINVAL, GPX_ENOMEM, GPX_ECUDA, GPX_ENOGPU, GPX_ERANGE, GPX_EIO, GPX_EAGAIN = 0, -1, -2, -3, -4, -5, -6, -7
+GPX_ENOENT = -8  # gpx_log_frame_device: requests or names the frames need are missing (listed)
 # PaxosAcceptor.STATES ordinals
 ST_RECOVERY, ST_ACTIVE_1, ST_ACTIVE_2, ST_STOPPED, ST_FREE = 0, 1, 2, 3, 255
 # record flags
@@ -92,6 +94,10 @@ log_want_dtype = np.dtype([("gid", "<u4"), ("min_slot", "<i4"), ("n_slots", "<u4
 log_hit_dtype = np.dtype([("decision", decision_dtype), ("accept", accept_dtype), ("blob_pos", "<u8"), ("reserved", "<u8")])
 assert log_want_dtype.itemsize == 16 and log_hit_dtype.itemsize == 96
 log_range_dtype = np.dtype([("pos", "<u8"), ("len", "<u4"), ("dst_off", "<u4")])
+# gpx_log_frame_device: the caller's table of the RequestPacket fields the ring does not hold, and what a call lacks
+journal_req_dtype = np.dtype([("gid", "<u4"), ("entry_node", "<i4"), ("req_id", "<i8"), ("entry_time", "<i8")])
+journal_miss_dtype = np.dtype([("gid", "<u4"), ("kind", "<u4"), ("req_id", "<i8")])
+assert journal_req_dtype.itemsize == 24 and journal_miss_dtype.itemsize == 16
 missing_dtype = np.dtype([("gid", "<u4"), ("slot", "<i4"), ("max_decision_slot", "<i4"), ("n_missing", "<u2"),
                           ("missing_too_much", "u1"), ("flags", "u1"), ("missing", "<i4", (GPX_MAX_WINDOW,))])
 assert missing_dtype.itemsize == 48
@@ -251,6 +257,9 @@ class Library:
     def check(self, rc: int):
         if rc != 0:
             raise GpxError(rc, self.last_error())
+
+
+LogFrames = namedtuple("LogFrames", "rc from_ frames missing sizes")
 
 
 class Engine:
@@ -562,6 +571,31 @@ class Engine:
         self.L.check(self.L.fn("log_drain_async")(self._h, C.c_uint32(lane), C.c_void_p(dst_ptr), C.c_uint64(cap),
                                                   C.byref(f), C.byref(nb), C.c_void_p(after_stream) if after_stream else None))
         return f.value, nb.value
+
+    def log_frame_device(self, lane: int, from_: int, meta, n_meta: int, caps=(0, 0, 0), stream=None):
+        """gpx_log_frame_device: the journal frames of [from_, head) of `lane`'s ring.  meta: a CUDA tensor of n_meta
+        journal_req_dtype records ([n, 24] uint8, ascending by (gid, req_id)), or None.  caps = (frame bytes, frames,
+        misses); on GPX_ERANGE the outputs are allocated again at the sizes the call reports and the call is repeated.
+        -> LogFrames(rc, the new from, frames uint8 [bytes], missing [k, 16] (journal_miss_dtype rows), sizes); rc is
+        GPX_OK or GPX_ENOENT (no frame written, from unchanged), any other code raises."""
+        import torch
+        from .wire import _dptr, _on, stream_handle
+        dev = meta.device if meta is not None else torch.device("cuda", torch.cuda.current_device())
+        caps = [int(c) for c in caps]
+        with _on(stream):
+            for _ in range(2):
+                out = torch.empty(max(caps[0], 1), dtype=torch.uint8, device=dev)
+                miss = torch.empty((max(caps[2], 1), 16), dtype=torch.uint8, device=dev)
+                f, ob, nf, nm = C.c_uint64(from_), C.c_uint64(caps[0]), C.c_uint32(caps[1]), C.c_uint32(caps[2])
+                rc = self.L.fn("log_frame_device")(self._h, C.c_uint32(lane), C.byref(f), _dptr(meta),
+                                                   C.c_uint32(n_meta), _dptr(out), C.byref(ob), C.byref(nf),
+                                                   _dptr(miss), C.byref(nm), stream_handle(stream))
+                caps = [ob.value, nf.value, nm.value]
+                if rc != GPX_ERANGE:
+                    break
+        if rc not in (GPX_OK, GPX_ENOENT):
+            self.L.check(rc)
+        return LogFrames(rc, f.value, out[: caps[0]], miss[: caps[2]], tuple(caps))
 
     def log_drain_wait(self):
         self.L.check(self.L.fn("log_drain_wait")(self._h))

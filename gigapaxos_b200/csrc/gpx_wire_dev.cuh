@@ -936,11 +936,12 @@ __global__ void k_wire_enc_keys_accepts(const __grid_constant__ DevState S, cons
   A.key[i] = st == GPX_WE_SENT ? a.h.gid : GPX_WIRE_NOKEY;
 }
 
-/* RequestPacket.toBytes :819-949 of request q without batched requests (n_batched written by the caller's count) */
-__device__ __forceinline__ uint32_t ww_request(uint8_t* p, int32_t type, const WireNames& W, uint32_t gid,
-                                               const WireAccArgs& X, uint32_t q, uint32_t n_batched) {
-  const gpx_request_rec rq = X.reqs[q];
-  const gpx_wire_req_meta m = X.meta[q];
+/* RequestPacket.toBytes :819-949 of one request without batched requests (n_batched written by the caller's count):
+ * its record, its wire meta and the arena its value lies in (at rq.payload_off).  Shared with the journal frames
+ * (gpx_journal.cuh) */
+__device__ __forceinline__ uint32_t ww_request_rec(uint8_t* p, int32_t type, const WireNames& W, uint32_t gid,
+                                                   const gpx_request_rec rq, const gpx_wire_req_meta m,
+                                                   const uint8_t* payload, uint32_t n_batched) {
   uint32_t b = ww_header(p, type, W, gid);
   ww_i64(p + b, rq.req_id);
   p[b + 8] = (rq.flags & GPX_F_STOP) ? 1u : 0u;
@@ -960,11 +961,20 @@ __device__ __forceinline__ uint32_t ww_request(uint8_t* p, int32_t type, const W
   ww_i32(p + b + 18, 0); /* digest */
   ww_i32(p + b + 22, (int32_t)rq.payload_len);
   b += 26;
-  wire_copy(p + b, X.payload + rq.payload_off, rq.payload_len);
+  wire_copy(p + b, payload + rq.payload_off, rq.payload_len);
   b += rq.payload_len;
   ww_i32(p + b, 0); /* responseValue */
   ww_i32(p + b + 4, (int32_t)n_batched);
   return b + 8;
+}
+/* the bytes ww_request_rec writes for a value of val_len bytes */
+__device__ __forceinline__ uint32_t ww_request_bytes(const WireNames& W, uint32_t gid, uint32_t val_len) {
+  return 13u + W.name[(size_t)gid * GPX_NAME_BYTES] + 55u + val_len;
+}
+/* request q of the ACCEPTs' requests */
+__device__ __forceinline__ uint32_t ww_request(uint8_t* p, int32_t type, const WireNames& W, uint32_t gid,
+                                               const WireAccArgs& X, uint32_t q, uint32_t n_batched) {
+  return ww_request_rec(p, type, W, gid, X.reqs[q], X.meta[q], X.payload, n_batched);
 }
 /* requests q0 .. q0 + n - 1 as one packet: the first of type `type`, the others its latched REQUESTs
  * ({int length}{REQUEST packet} :929-936); returns the bytes written */

@@ -27,6 +27,7 @@
 #include <algorithm>
 #include <cstring>
 
+#include "gpx_journal.cuh"
 #include "gpx_respcache.cuh"
 #include "gpx_wire_dev.cuh"
 #include "gpx_wire_fwd.cuh"
@@ -870,5 +871,91 @@ static int rc_match(Ex& ex, C& call, void** buf, size_t* buf_bytes, const RcTabl
       (rc = ex.sync())) /* the one host read: the count of misses */
     return rc;
   *n_out = tot;
+  return call.end();
+}
+
+/* ---- journal frames (gpx_journal.cuh) --------------------------------------------------------------------------------
+ * gpx_log_frame_device over [*from, head), head being the engine's head of the lane.  Before the one synchronisation
+ * only the range is known on the host, so the directory and the counters are sized from it: an image takes at least 32
+ * ring bytes and a segment at least GPX_SEG_DEC_BYTES(1). */
+template <class Ex, class C>
+static int log_frame(Ex& ex, C& call, const WireEnv& E, uint32_t lane, uint64_t* from, uint64_t head,
+                     const gpx_journal_req* meta, uint32_t n_meta, uint8_t* out, uint64_t* out_bytes,
+                     uint32_t* n_frames, gpx_journal_miss* missing, uint32_t* n_missing) {
+  WireOut o[] = {{out_bytes, out != nullptr}, {n_frames, out != nullptr}, {n_missing, missing != nullptr}};
+  int rc = wire_args(from && (!n_meta || meta), 0, o);
+  if (rc) return rc;
+  if (*from & 31) return fail(GPX_EINVAL, "from is not a segment boundary");
+  if (*from > head) return fail(GPX_EINVAL, "from is beyond the head");
+  if (*from == head) return GPX_OK;
+  const uint64_t range = head - *from;
+  if (range > E.S.ring_cap) return fail(GPX_ERANGE, "bytes from `from` on were already overwritten");
+  if (range / 32 > 0xffffffffull) return fail(GPX_ERANGE, "range too long for one call");
+  if ((rc = call.begin())) return rc;
+  const uint32_t n = (uint32_t)(range / 32);
+  const uint32_t seg_cap = (uint32_t)std::min<uint64_t>(range / GPX_SEG_DEC_BYTES(1) + 2, 1ull << 20);
+  WireScan scan{ex.scan_bytes(n)};
+  JournalArgs A;
+  memset(&A, 0, sizeof A);
+  A.lane = lane;
+  A.n = n;
+  A.meta = meta;
+  A.n_meta = n_meta;
+  LogSeg* segs;
+  unsigned long long* ctl;
+  uint32_t* off;
+  if ((rc = wire_place(ex, E.buf, E.bytes, [&](Carve& c) {
+         segs = c.take<LogSeg>(seg_cap);
+         ctl = c.take<unsigned long long>(JF_NCTL);
+         A.cnt = c.take<uint32_t>((size_t)JF_NCNT * n);
+         off = c.take<uint32_t>((size_t)JF_NCNT * n);
+         scan.lay(c, JF_NCNT);
+         return (size_t)0;
+       })))
+    return rc;
+  A.segs = segs;
+  A.ctl = ctl;
+  LogFindArgs D;
+  memset(&D, 0, sizeof D);
+  D.lane = lane;
+  D.from = *from;
+  D.segs = segs;
+  D.seg_cap = seg_cap;
+  D.ctl = ctl;
+  /* pass 0: the directory, the table's order, each image's frame bytes, frame and misses, their scans */
+  if ((rc = ex.fill(ctl, 0, JF_NCTL * sizeof(unsigned long long))) || (rc = ex.launch(k_log_dir, 1, 32, E.S, D)) ||
+      (n_meta && (rc = ex.launch(k_journal_meta, n_meta, 256, A))) ||
+      (rc = ex.launch(k_journal, n, GPX_JOURNAL_BLOCK, E.S, E.W, A)) || (rc = ex.scan(A.cnt, off, n, JF_NCNT, scan)) ||
+      (rc = ex.totals(A.cnt, off, n, JF_NCNT, scan.tot)))
+    return rc;
+  A.off = off;
+  uint32_t tot[JF_NCNT];
+  unsigned long long c[JF_NCTL];
+  if ((rc = ex.launch(k_journal_fit, n, 256, A)) || (rc = ex.read(tot, scan.tot, sizeof tot)) ||
+      (rc = ex.read(c, ctl, sizeof c)) || (rc = ex.sync())) /* the one host read: the sizes and the flags */
+    return rc;
+  if (c[LOGF_ERR] == LOGF_OVERWRITTEN) return fail(GPX_ERANGE, "bytes from `from` on were already overwritten");
+  if (c[LOGF_ERR] == LOGF_CORRUPT) return fail(GPX_EINVAL, "`from` is not a segment boundary");
+  if (c[LOGF_ERR] == LOGF_TOO_MANY) return fail(GPX_ERANGE, "more log segments than the directory holds");
+  if (c[LOGF_HEAD] != head) return fail(GPX_EINVAL, "the head moved: order the calls that log before this one");
+  if (c[JF_UNSORTED]) return fail(GPX_EINVAL, "meta is not strictly ascending by (gid, req_id)");
+  if (c[JF_BAD_BLOB]) return fail(GPX_EINVAL, "an ACCEPT image's request blob lies outside its segment");
+  if (tot[JF_MISS]) { /* the misses, and no frame */
+    const uint32_t sizes[3] = {0, 0, tot[JF_MISS]};
+    if ((rc = wire_fit(o, sizes, "missing too small"))) return rc;
+    A.miss = missing;
+    A.emit = 1;
+    if ((rc = ex.launch(k_journal, n, GPX_JOURNAL_BLOCK, E.S, E.W, A)) || (rc = call.end())) return rc;
+    return fail(GPX_ENOENT, "requests or names the frames need are missing");
+  }
+  if (c[JF_OVER]) return fail(GPX_ERANGE, "the frames pass 4 GiB");
+  const uint32_t sizes[3] = {tot[JF_BYTES], tot[JF_FRAMES], 0};
+  if ((rc = wire_fit(o, sizes, "frame output too small"))) return rc;
+  if (tot[JF_FRAMES]) { /* pass 1: the frames at the scanned offsets, left in flight */
+    A.out = out;
+    A.emit = 2;
+    if ((rc = ex.launch(k_journal, n, GPX_JOURNAL_BLOCK, E.S, E.W, A))) return rc;
+  }
+  *from = head;
   return call.end();
 }

@@ -66,6 +66,11 @@ class Journaler:
         self.fos.write(frame)
         self.cur_size += len(frame)
 
+    def append_frames(self, frames):
+        """frames already in the {int32 BE len}{bytes} form (gpx_log_frame_device's output), in one write"""
+        self.fos.write(frames)
+        self.cur_size += len(frames)
+
     def end_batch(self):
         self.fos.flush()  # FLUSH=true, SYNC=false (PaxosConfig.java:720,725)
         if self.cur_size > self.max:
@@ -188,6 +193,80 @@ class LogDrainer:
                                entry_replica=entry, entry_time=int(etime), batched=tuple(subs))
         return wire.encode_accept(req, int(a["slot"]), int(a["bnum"]), int(a["bcoord"]), False, int(a["median_cp"]),
                                   int(a["sender"]))
+
+
+MetaSource = Callable[[np.ndarray], np.ndarray]
+"""journal_miss_dtype records -> journal_req_dtype records: {gid, entryReplica, req_id, entryTime} of the requests a
+frame call lacks (PaxosManager.outstanding is the Java node's source)."""
+
+
+class DeviceLogDrainer:
+    """LogDrainer's job with the frames written on the device (gpx_log_frame_device): one call frames every image of
+    the lane's undrained range in HBM, the frames come down to page-locked memory in one copy and go to the Journaler in
+    one write, then the range is released.  The caller's table of entryReplica / entryTime lives on the device; add()
+    puts requests in it ahead of the drain, and the requests a call reports missing (GPX_ENOENT) are asked of
+    meta_source before the call is repeated."""
+
+    def __init__(self, engine: Engine, lane: int, journaler: Journaler, meta_source: MetaSource, offset: int = 0):
+        self.engine, self.lane, self.j, self.meta_source = engine, lane, journaler, meta_source
+        self.offset = offset
+        self.frames_written = 0
+        self.meta = np.zeros(0, dtype=abi.journal_req_dtype)
+        self._dmeta = None
+        self._pinned = None
+        self.caps = (1 << 16, 1 << 10, 64)
+
+    def add(self, reqs: np.ndarray):
+        """enter journal_req_dtype records in the table (a request already in it keeps its entry)"""
+        reqs = np.asarray(reqs, dtype=abi.journal_req_dtype)
+        if len(reqs) == 0:
+            return
+        m = np.concatenate([self.meta, reqs])
+        m = m[np.lexsort((m["req_id"], m["gid"]))]  # stable: of equal keys the table's entry comes first
+        new = np.ones(len(m), dtype=bool)
+        new[1:] = (m["gid"][1:] != m["gid"][:-1]) | (m["req_id"][1:] != m["req_id"][:-1])
+        self.meta = m[new]
+        self._dmeta = None
+
+    def forget(self, keep: np.ndarray):
+        """keep only the table entries where keep (a bool mask over self.meta) is true"""
+        self.meta = self.meta[keep]
+        self._dmeta = None
+
+    def _device_meta(self):
+        import torch
+        if self._dmeta is None and len(self.meta):
+            self._dmeta = torch.from_numpy(self.meta.view(np.uint8).reshape(-1, 24).copy()).cuda()
+        return self._dmeta
+
+    def drain(self) -> int:
+        """frames [offset, head) into the journal; returns the number of frames"""
+        import torch
+        while True:
+            r = self.engine.log_frame_device(self.lane, self.offset, self._device_meta(), len(self.meta), self.caps)
+            self.caps = tuple(max(a, b) for a, b in zip(self.caps, r.sizes))
+            if r.rc == abi.GPX_OK:
+                break
+            torch.cuda.current_stream().synchronize()
+            miss = np.ascontiguousarray(r.missing.cpu().numpy()).reshape(-1).view(abi.journal_miss_dtype)
+            if np.any(miss["req_id"] == -1):
+                raise KeyError("gids without a name (gpx_set_group_names): %s" % sorted(set(miss["gid"].tolist())))
+            before = len(self.meta)
+            self.add(self.meta_source(miss))
+            if len(self.meta) == before:
+                raise KeyError("meta_source knows none of %d missing requests" % len(miss))
+        n = int(r.sizes[0])
+        if n:
+            if self._pinned is None or self._pinned.numel() < n:
+                self._pinned = torch.empty(max(n, 1 << 20), dtype=torch.uint8, pin_memory=True)
+            self._pinned[:n].copy_(r.frames[:n], non_blocking=True)
+            torch.cuda.current_stream().synchronize()
+            self.j.append_frames(memoryview(self._pinned[:n].numpy()))
+        self.j.end_batch()
+        self.frames_written += int(r.sizes[1])
+        self.offset = r.from_
+        self.engine.log_release(self.lane, self.offset)
+        return int(r.sizes[1])
 
 
 def read_journal(path: str) -> Iterator[bytes]:

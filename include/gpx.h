@@ -78,7 +78,8 @@ enum {
   GPX_ENOGPU = -4,
   GPX_ERANGE = -5,
   GPX_EIO = -6,
-  GPX_EAGAIN = -7 /* log ring full (log_backpressure): drain + release, then repeat the call; nothing was done */
+  GPX_EAGAIN = -7, /* log ring full (log_backpressure): drain + release, then repeat the call; nothing was done */
+  GPX_ENOENT = -8  /* gpx_log_frame_device: a logged request or group name is not known; the misses are listed */
 };
 
 /* PaxosAcceptor.STATES ordinals (PaxosAcceptor.java:87-92); FREE = no instance */
@@ -195,7 +196,7 @@ typedef struct gpx_exec_rec {
  * moves as one 32-byte plus one 16-byte aligned store; image.payload_off is relative to the
  * segment's payload area; unlogged records have GPX_F_VOID.  Segments are 32-byte multiples.
  * DECISION segment: images are gpx_decision_rec (32 B), no payload area.
- * (SQLPaxosLogger.journal frames {int32 len}{packet bytes}, :1000-1003; gpx_wire_*
+ * (SQLPaxosLogger.journal frames {int32 len}{packet bytes}, :1000-1003; gpx_log_frame_device
  * re-frames segments into that byte format.) */
 #define GPX_SEG_MAGIC 0x53585047u /* "GPXS" */
 typedef struct gpx_log_seg_hdr {
@@ -603,6 +604,64 @@ typedef struct gpx_log_hit { /* 96 B */
   uint64_t reserved;
 } gpx_log_hit;
 int gpx_log_find(gpx_engine* e, uint32_t lane, uint64_t from, uint32_t n, const gpx_log_want* wants, gpx_log_hit* out);
+
+/* ---- journal frames on the device: a drained range of the ring as Journaler bytes ------------------------------------
+ * SQLPaxosLogger.journal :965-1036 appends each logged packet to the journal file as {int32 BE length}{packet}, the
+ * packet as SQLPaxosLogger.toBytes :1084-1098 writes it: an ACCEPT byteified (AcceptPacket.toBytes), a DECISION or a
+ * PREPARE as the JSON string of the packet.  gpx_log_frame_device writes those frames for a range of one lane's ring in
+ * HBM, ready for one copy to the host and one write to the file.
+ *
+ * The ring does not hold two RequestPacket fields a frame needs, entryReplica and entryTime; the caller passes them
+ * per request in meta[n_meta] (device memory; PaxosManager.outstanding is the Java node's source), sorted ascending by
+ * (gid, req_id) without duplicates, else GPX_EINVAL and nothing is written.  Names and versions come from
+ * gpx_set_group_names' table.
+ *
+ *   Range     [*from, head) of `lane`, head being the engine's head of that lane at the call (as gpx_log_drain_async
+ *             reads it, after the calls that log are enqueued; a call on another stream must be ordered before this
+ *             one).  *from is a segment boundary: 0 before the ring has wrapped, else a position this call or
+ *             gpx_log_drain_async handed out.  Bytes already overwritten are GPX_ERANGE and a segment header that does
+ *             not parse is GPX_EINVAL, as in gpx_log_find.  An empty range returns GPX_OK at once with no frame.
+ *   Frames    out[*out_bytes] receives, segment by segment in ring order and image by image, one frame per image
+ *             that is not VOID, exactly as journal.LogDrainer appends them for the same range:
+ *               ACCEPT (48-byte image)   the AcceptPacket bytes of gpx_wire_encode_accept: recovery 0, median_cp and
+ *                 sender from the image, every RequestPacket field the ring does not hold at wire.Request's default
+ *                 (no client or listen address, forwardCount 0, no digest, no response).  nreq <= 1: the request is
+ *                 the image's req_id, STOP flag and blob.  nreq > 1: the blob's gpx_batch_ent list, the first entry
+ *                 the outer request (entryReplica and entryTime of the image's req_id), the others its `batched`
+ *                 REQUEST packets, each with its own req_id, STOP bit and table entry.
+ *               DECISION (32-byte image, no GPX_F_PREPARE)   journal.decision_json:
+ *                 {"type":90,"PT":6,"ID","V","B","GC_S","S","QID","ET","E"}, then "STOP":true only with GPX_F_STOP.
+ *               PREPARE (GPX_F_PREPARE)   journal.prepare_json: {"type":90,"PT":2,"ID","V","B","PREP_MIN"}; it
+ *                 needs no table entry.
+ *             The paxosID is escaped as json.dumps with ensure_ascii escapes it (gpx_wire_encode_json_device's rule).
+ *             *n_frames receives the number of frames.
+ *   Misses    an image whose gid has no name, or one of whose requests is not in meta, gets no frame.  Then no frame
+ *             at all is written, *from is unchanged, missing[*n_missing] lists one gpx_journal_miss per request the
+ *             table lacks (req_id -1 once for an image whose gid has no name), in image order, and the call returns
+ *             GPX_ENOENT.  The caller adds those requests to meta and calls again, so the order of frames is never
+ *             broken.
+ *   Sizes     *out_bytes, *n_frames and *n_missing are HOST pointers, capacities in / sizes out.  GPX_ERANGE reports the
+ *             sizes and writes nothing: the frames' when a frame output is too small, or the misses' (the frame sizes
+ *             0) when missing is.  Frames beyond 4 GiB in one call are GPX_ERANGE.
+ *   Success   *from becomes head, and the lane's drain position moves up to it, so that gpx_log_release(lane, *from)
+ *             is accepted; the caller releases once the frames are durable.
+ * meta, out and missing are device pointers.  Stream-ordered on `stream` (NULL = the engine's stream), with the wire
+ * calls' scratch and their ordering between streams; one synchronisation reads the totals (and, as in
+ * gpx_log_drain_async, one more when a call of unknown log size left the engine's head to be read back). */
+typedef struct gpx_journal_req { /* 24 B */
+  uint32_t gid;
+  int32_t entry_node; /* RequestPacket.entryReplica */
+  int64_t req_id;
+  int64_t entry_time; /* RequestPacket.entryTime, ms */
+} gpx_journal_req;
+typedef struct gpx_journal_miss { /* 16 B: a request the call could not frame */
+  uint32_t gid;
+  uint32_t kind;  /* GPX_F_ACCEPT, GPX_F_DECISION or GPX_F_PREPARE: the image that needs it */
+  int64_t req_id; /* the request that is missing, or -1 when the gid has no name */
+} gpx_journal_miss;
+int gpx_log_frame_device(gpx_engine* e, uint32_t lane, uint64_t* from, const gpx_journal_req* meta, uint32_t n_meta,
+                         uint8_t* out, uint64_t* out_bytes, uint32_t* n_frames, gpx_journal_miss* missing,
+                         uint32_t* n_missing, void* stream);
 
 /* Request bodies for a batch of gpx_log_find hits (blob_pos) or of carried-over pvalues (the latest log position
  * before the head that is congruent to frame_ref * 16 modulo log_ring_bytes) in ONE device->host copy:
