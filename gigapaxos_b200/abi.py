@@ -98,6 +98,10 @@ log_range_dtype = np.dtype([("pos", "<u8"), ("len", "<u4"), ("dst_off", "<u4")])
 journal_req_dtype = np.dtype([("gid", "<u4"), ("entry_node", "<i4"), ("req_id", "<i8"), ("entry_time", "<i8")])
 journal_miss_dtype = np.dtype([("gid", "<u4"), ("kind", "<u4"), ("req_id", "<i8")])
 assert journal_req_dtype.itemsize == 24 and journal_miss_dtype.itemsize == 16
+# gpx_journal_compact_device: what the call did to each file
+journal_file_dtype = np.dtype([("status", "<u4"), ("kept", "<u4"), ("dropped", "<u4"), ("unresolved", "<u4"),
+                               ("out_off", "<u4"), ("out_bytes", "<u4")])
+assert journal_file_dtype.itemsize == 24
 missing_dtype = np.dtype([("gid", "<u4"), ("slot", "<i4"), ("max_decision_slot", "<i4"), ("n_missing", "<u2"),
                           ("missing_too_much", "u1"), ("flags", "u1"), ("missing", "<i4", (GPX_MAX_WINDOW,))])
 assert missing_dtype.itemsize == 48
@@ -249,6 +253,15 @@ class Library:
     def build_info(self) -> str:
         return self.fn("build_info")().decode()
 
+    def journal_index(self, buf: bytes, base: int = 0) -> np.ndarray:
+        """gpx_journal_index: base + the offset of every whole frame of one journal file's bytes (uint32)"""
+        cap = len(buf) // 4 + 1
+        starts = np.zeros(cap, np.uint32)
+        n, end = C.c_uint32(0), C.c_uint64(0)
+        self.check(self.fn("journal_index")(C.c_char_p(bytes(buf)), C.c_uint64(len(buf)), C.c_uint32(base),
+                                            _ptr(starts), C.c_uint32(cap), C.byref(n), C.byref(end)))
+        return starts[: n.value]
+
     def config_defaults(self) -> Config:
         cfg = Config()
         self.fn("config_defaults")(C.byref(cfg))
@@ -260,6 +273,7 @@ class Library:
 
 
 LogFrames = namedtuple("LogFrames", "rc from_ frames missing sizes")
+JournalCompact = namedtuple("JournalCompact", "rc out files bad sizes")
 
 
 class Engine:
@@ -596,6 +610,36 @@ class Engine:
         if rc not in (GPX_OK, GPX_ENOENT):
             self.L.check(rc)
         return LogFrames(rc, f.value, out[: caps[0]], miss[: caps[2]], tuple(caps))
+
+    def journal_compact_device(self, data, n_bytes: int, file_off, starts, gc_slot, last_readonly: bool,
+                               caps=(0, 0), stream=None):
+        """gpx_journal_compact_device over CUDA tensors: data (uint8, the files concatenated), file_off (uint32 [k+1]),
+        starts (uint32 frame offsets), gc_slot (int32 per gid).  caps = (out bytes, bad frames); on GPX_ERANGE the
+        outputs are allocated again at the sizes the call reports and the call is repeated.  -> JournalCompact(rc, out
+        uint8 [bytes], files [k, 24] (journal_file_dtype rows), bad uint32 frame indices, sizes); rc is GPX_OK or
+        GPX_EINVAL with bad listed (nothing else written), any other code raises."""
+        import torch
+        from .wire import _dptr, _on, stream_handle
+        k = int(file_off.numel()) - 1
+        caps = [int(c) for c in caps]
+        with _on(stream):
+            for _ in range(2):
+                out = torch.empty(max(caps[0], 1), dtype=torch.uint8, device=data.device)
+                files = torch.empty((max(k, 1), 24), dtype=torch.uint8, device=data.device)
+                bad = torch.empty(max(caps[1], 1), dtype=torch.int32, device=data.device)
+                ob, nb = C.c_uint64(caps[0]), C.c_uint32(caps[1])
+                rc = self.L.fn("journal_compact_device")(
+                    self._h, _dptr(data), C.c_uint64(n_bytes), _dptr(file_off), C.c_uint32(k), _dptr(starts),
+                    C.c_uint32(int(starts.numel())), _dptr(gc_slot), C.c_uint32(int(gc_slot.numel())),
+                    C.c_uint32(1 if last_readonly else 0), _dptr(out), C.byref(ob), _dptr(files), _dptr(bad),
+                    C.byref(nb), stream_handle(stream))
+                caps = [ob.value, nb.value]
+                if rc != GPX_ERANGE:
+                    break
+        if rc == GPX_EINVAL and caps[1]:
+            return JournalCompact(rc, out[:0], files[:0], bad[: caps[1]], tuple(caps))
+        self.L.check(rc)
+        return JournalCompact(rc, out[: caps[0]], files[:k], bad[:0], tuple(caps))
 
     def log_drain_wait(self):
         self.L.check(self.L.fn("log_drain_wait")(self._h))

@@ -28,6 +28,7 @@
 #include <cstring>
 
 #include "gpx_journal.cuh"
+#include "gpx_journal_gc.cuh"
 #include "gpx_respcache.cuh"
 #include "gpx_wire_dev.cuh"
 #include "gpx_wire_fwd.cuh"
@@ -958,4 +959,107 @@ static int log_frame(Ex& ex, C& call, const WireEnv& E, uint32_t lane, uint64_t*
   }
   *from = head;
   return call.end();
+}
+
+/* ---- journal garbage collection (gpx_journal_gc.cuh) -----------------------------------------------------------------
+ * gpx_journal_compact_device.  Everything up to the one synchronisation is enqueued without a host read, malformed
+ * frames included (they are neither indexed nor kept), so that the totals of the counters, the bad count and the
+ * flag on file_off come back together. */
+template <class Ex, class C>
+static int journal_compact(Ex& ex, C& call, const WireEnv& E, const uint8_t* bytes, uint64_t n_bytes,
+                           const uint32_t* file_off, uint32_t n_files, const uint32_t* starts, uint32_t n,
+                           const int32_t* gc_slot, uint32_t n_gids, uint32_t last_readonly, uint8_t* out,
+                           uint64_t* out_bytes, gpx_journal_file* files, uint32_t* bad, uint32_t* n_bad) {
+  WireOut o[] = {{out_bytes, out != nullptr}, {n_bad, bad != nullptr}};
+  int rc = wire_args((!n_bytes || bytes) && (!n || starts) && (!n_files || (file_off && files && gc_slot)), n_bytes, o);
+  if (rc) return rc;
+  if (n_files == 0) return n ? fail(GPX_EINVAL, "frames without a file") : GPX_OK;
+  if (n_gids < E.S.G) return fail(GPX_EINVAL, "gc_slot needs one slot per group (n_gids < max_groups)");
+  if ((rc = call.begin())) return rc;
+  JournalGcArgs A;
+  memset(&A, 0, sizeof A);
+  A.bytes = bytes;
+  A.n_bytes = (uint32_t)n_bytes;
+  A.file_off = file_off;
+  A.n_files = n_files;
+  A.starts = starts;
+  A.n = n;
+  A.gc_slot = gc_slot;
+  A.last_readonly = last_readonly;
+  GidSort sort(ex, n, E.S.G); /* key G: not indexed */
+  WireScan scan{ex.scan_bytes(n)}, fscan{ex.scan_bytes(n_files)};
+  uint32_t *cnt, *off, *foff;
+  if ((rc = wire_place(ex, E.buf, E.bytes, [&](Carve& c) {
+         A.bad_off = c.take<uint32_t>(1);
+         A.rec = c.take<JgcRec>(n);
+         A.key = c.take<uint32_t>(n);
+         cnt = c.take<uint32_t>((size_t)JG_NCNT * n);
+         off = c.take<uint32_t>((size_t)JG_NCNT * n);
+         scan.lay(c, JG_NCNT);
+         sort.lay(c);
+         A.fs = c.take<JgcFile>(n_files);
+         A.fbytes = c.take<uint32_t>(n_files);
+         foff = c.take<uint32_t>(n_files);
+         fscan.lay(c, 1);
+         return (size_t)0;
+       })))
+    return rc;
+  A.cnt = cnt;
+  A.off = off;
+  A.tot = scan.tot;
+  A.foff = foff;
+  /* parse, sort the indexed frames by gid, keep, scan; then the files and the scan of their compacted bytes */
+  if ((rc = ex.fill(A.bad_off, 0, 4)) || (rc = ex.launch(k_jgc_offsets, n_files + 1, 256, A))) return rc;
+  if (n) {
+    if ((rc = ex.launch(k_jgc_parse, n, 128, E.S, E.W, A)) || (rc = sort.run(ex, A.key, n))) return rc;
+    A.perm = sort.perm;
+    A.skey = sort.skeys;
+    if ((rc = ex.launch(k_jgc_keep, n, 256, A)) || (rc = ex.scan(cnt, off, n, JG_NCNT, scan)) ||
+        (rc = ex.totals(cnt, off, n, JG_NCNT, scan.tot)))
+      return rc;
+  } else if ((rc = ex.fill(scan.tot, 0, JG_NCNT * sizeof(uint32_t)))) {
+    return rc;
+  }
+  uint32_t tot[JG_NCNT], ftot = 0, bad_off = 0;
+  if ((rc = ex.launch(k_jgc_file, n_files, 128, A)) || (rc = ex.scan(A.fbytes, foff, n_files, 1, fscan)) ||
+      (rc = ex.totals(A.fbytes, foff, n_files, 1, fscan.tot)) || (rc = ex.read(tot, scan.tot, sizeof tot)) ||
+      (rc = ex.read(&ftot, fscan.tot, 4)) || (rc = ex.read(&bad_off, A.bad_off, 4)) ||
+      (rc = ex.sync())) /* the one host read: the totals and the flag */
+    return rc;
+  if (bad_off) return fail(GPX_EINVAL, "file_off is not ascending from 0 to n_bytes");
+  if (tot[JG_BAD]) { /* the malformed frames' indices, and nothing else */
+    const uint32_t sizes[2] = {0, tot[JG_BAD]};
+    if ((rc = wire_fit(o, sizes, "bad too small"))) return rc;
+    A.bad = bad;
+    if ((rc = ex.launch(k_jgc_bad, n, 256, A)) || (rc = call.end())) return rc;
+    return fail(GPX_EINVAL, "frames that do not parse or do not chain");
+  }
+  const uint32_t sizes[2] = {ftot, 0};
+  if ((rc = wire_fit(o, sizes, "out too small"))) return rc;
+  A.out = out;
+  A.files = files;
+  if (ftot && (rc = ex.launch(k_jgc_copy, (uint32_t)std::min<uint64_t>((uint64_t)n * 32u, 32ull * GPX_JGC_COPY_WARPS),
+                              256, A)))
+    return rc;
+  if ((rc = ex.launch(k_jgc_files, n_files, 128, A))) return rc;
+  return call.end();
+}
+
+/* gpx_journal_index's walk (journal.read_journal's) */
+static int journal_index(const uint8_t* buf, uint64_t n_bytes, uint32_t base, uint32_t* starts, uint32_t cap,
+                         uint32_t* n_frames, uint64_t* end) {
+  if (!n_frames || !end || (n_bytes && !buf) || (cap && !starts)) return fail(GPX_EINVAL, "null argument");
+  if (base + n_bytes > 0xffffffffull) return fail(GPX_EINVAL, "base + n_bytes passes 4 GiB");
+  uint64_t p = 0;
+  uint32_t k = 0;
+  while (p + 4 <= n_bytes) {
+    const uint32_t l = ((uint32_t)buf[p] << 24) | ((uint32_t)buf[p + 1] << 16) | ((uint32_t)buf[p + 2] << 8) | buf[p + 3];
+    if (l >= 0x80000000u || p + 4 + l > n_bytes) break; /* torn tail */
+    if (k < cap) starts[k] = base + (uint32_t)p;
+    k++;
+    p += 4 + l;
+  }
+  *n_frames = k;
+  *end = p;
+  return k > cap ? fail(GPX_ERANGE, "more frames than cap") : GPX_OK;
 }

@@ -27,6 +27,7 @@ import numpy as np
 
 from . import abi, wire
 from .abi import Engine
+from .paxos_manager import _jsub
 
 MAX_LOG_FILE_SIZE = 64 * 1024 * 1024  # PC.MAX_LOG_FILE_SIZE PaxosConfig.java:314
 
@@ -306,3 +307,188 @@ def replay_decisions(files: List[str]) -> Dict[str, Dict[int, dict]]:
             if v["kind"] == "DECISION":
                 out.setdefault(v["paxos_id"], {})[v["slot"]] = v
     return out
+
+
+# ---- garbage collection (SQLPaxosLogger.garbageCollectJournal :3154, compactLogfiles :3282-3450, mergeLogfiles :3476)
+
+JGC_UNCHANGED, JGC_COMPACTED, JGC_EMPTY, JGC_TORN = 0, 1, 2, 3  # gpx_journal_file.status
+
+
+GcSlotOf = Callable[[str, int], "int | None"]
+"""(paxosID, version) -> the group's GC slot, or None when the pair names no live group (gpx_set_group_names' table)."""
+
+
+class CompactedFile:
+    """what compaction does to one journal file: status (JGC_*), the new bytes of a JGC_COMPACTED file, the frames it
+    holds afterwards and those removed, and how many of its frames named no live group"""
+
+    def __init__(self, status: int, data, kept: int, dropped: int, unresolved: int):
+        self.status, self.data, self.kept, self.dropped, self.unresolved = status, data, kept, dropped, unresolved
+
+    def __eq__(self, other):
+        return vars(self) == vars(other)
+
+    def __repr__(self):
+        return "CompactedFile(%r)" % {k: (len(v) if k == "data" and v is not None else v) for k, v in vars(self).items()}
+
+
+def _frames(data: bytes):
+    """(offset, packet) of every whole frame, and where read_journal's walk stops"""
+    out, p = [], 0
+    while p + 4 <= len(data):
+        (ln,) = struct.unpack(">i", data[p: p + 4])
+        if ln < 0 or p + 4 + ln > len(data):
+            break
+        out.append((p, data[p + 4: p + 4 + ln]))
+        p += 4 + ln
+    return out, p
+
+
+def _gc_fields(pkt: bytes):
+    """(paxosID, version, slot, bnum, bcoord, is_prepare) of a journaled packet, or ValueError"""
+    try:
+        v = parse_packet(pkt)
+    except Exception as e:  # noqa: BLE001 -- any failure to read the packet is a malformed frame
+        raise ValueError("frame does not parse: %s" % e) from None
+    slot = v["first_undecided_slot"] if v["kind"] == "PREPARE" else v["slot"]
+    ints = [v["version"], slot, v["bnum"], v["bcoord"]]
+    if not isinstance(v["paxos_id"], str) or any(type(x) is not int or not -(1 << 31) <= x < (1 << 31) for x in ints):
+        raise ValueError("frame fields out of range")
+    return v["paxos_id"], v["version"], slot, v["bnum"], v["bcoord"], v["kind"] == "PREPARE"
+
+
+def compact_files(files: List[str], gc_slot_of: GcSlotOf, last_readonly: bool = True) -> List[CompactedFile]:
+    """The host model of gpx_journal_compact_device (include/gpx.h): one lane's journal files in roll order -> what
+    compaction does to each.  A frame whose (paxosID, version) names no live group is kept; one at or below its
+    group's GC slot is dropped; a PREPARE is also dropped when an indexed frame of its group (any frame above the GC
+    slot, in any of the files) has a higher ballot, compared entry by entry as LogIndex.isLogMsgNeeded :331-345 does.
+    An ACCEPT's or DECISION's slot is its pvalue's slot (the index's, MessageLogDiskMap.add :412), not the ballot
+    number SQLPaxosLogger.getSlot :492-496 returns.  A torn file, and the last one when last_readonly, stay as they
+    are.  ValueError on a frame that is not an ACCEPT, a DECISION or a PREPARE."""
+    parsed = []  # per file: (data, [(offset, length, group key or None, indexed, fields)], torn)
+    index: Dict[tuple, List[Tuple[int, int]]] = {}
+    for path in files:
+        with open(path, "rb") as f:
+            data = f.read()
+        frames, end = _frames(data)
+        rows = []
+        for k, (off, pkt) in enumerate(frames):
+            try:
+                pid, ver, slot, bn, bc, prep = _gc_fields(pkt)
+            except ValueError as e:
+                raise ValueError("%s: frame %d: %s" % (path, k, e)) from None
+            gc = gc_slot_of(pid, ver)
+            key = None if gc is None else (pid, ver)
+            indexed = key is not None and _jsub(slot, gc) > 0
+            if indexed:
+                index.setdefault(key, []).append((bn, bc))
+            rows.append((off, 4 + len(pkt), key, indexed, prep, bn, bc))
+        parsed.append((data, rows, end != len(data)))
+    out = []
+    for i, (data, rows, torn) in enumerate(parsed):
+        keep = []
+        for off, ln, key, indexed, prep, bn, bc in rows:
+            if key is None:
+                k = True
+            elif not indexed:
+                k = False
+            elif prep:
+                k = not any(_jsub(en, bn) > 0 or (en == bn and _jsub(ec, bc) > 0) for en, ec in index[key])
+            else:
+                k = True
+            keep.append(k)
+        unresolved = sum(1 for r in rows if r[2] is None)
+        kept = sum(keep)
+        if torn or (last_readonly and i == len(parsed) - 1):
+            out.append(CompactedFile(JGC_TORN if torn else JGC_UNCHANGED, None, len(rows), 0, unresolved))
+        elif kept == 0:
+            out.append(CompactedFile(JGC_EMPTY, None, 0, len(rows), unresolved))
+        elif kept == len(rows):
+            out.append(CompactedFile(JGC_UNCHANGED, None, kept, 0, unresolved))
+        else:
+            body = b"".join(data[off: off + ln] for (off, ln, *_), k in zip(rows, keep) if k)
+            out.append(CompactedFile(JGC_COMPACTED, body, kept, len(rows) - kept, unresolved))
+    return out
+
+
+def _replace(path: str, data) -> None:
+    """path's contents become data: a .tmp file written, fsynced and renamed over it (modifyLogfileAndLogIndex)"""
+    tmp = path + ".tmp"
+    with open(tmp, "wb") as f:
+        f.write(data)
+        f.flush()
+        os.fsync(f.fileno())
+    os.replace(tmp, path)
+
+
+def apply_compaction(journaler: Journaler, files: List[str], results: List[CompactedFile]) -> None:
+    """Writes what compaction decided for each of files (journaler's, the current file never among them): a
+    compacted file replaced, an empty one deleted and dropped from journaler.files.  Then adjacent files whose sizes
+    sum to at most 2 x the journaler's file size limit are merged into the later one, the earlier deleted
+    (compactLogfiles :3305-3312 / mergeLogfiles).  A torn file is neither merged nor merged into: its tail would end
+    up inside the merged file."""
+    if journaler.cur in files:
+        raise ValueError("the current journal file is never rewritten")
+    left = []
+    for path, r in zip(files, results):
+        if r.status == JGC_COMPACTED:
+            _replace(path, r.data)
+        elif r.status == JGC_EMPTY:
+            os.remove(path)
+            journaler.files.remove(path)
+            continue
+        left.append((path, r.status == JGC_TORN))
+    prev = None
+    for path, torn in left:
+        if torn:
+            prev = None
+            continue
+        if prev is not None and os.path.getsize(prev) + os.path.getsize(path) <= 2 * journaler.max:
+            with open(prev, "rb") as a, open(path, "rb") as b:
+                _replace(path, a.read() + b.read())
+            os.remove(prev)
+            journaler.files.remove(prev)
+        prev = path
+
+
+class JournalCompactor:
+    """Garbage-collects a Journaler's files on the device (gpx_journal_compact_device): the files but the current one
+    are read, indexed on the host (gpx_journal_index), uploaded once together with the current file (read-only: its
+    frames still count for the PREPARE rule), compacted in one call, and written back by apply_compaction."""
+
+    def __init__(self, engine: Engine, journaler: Journaler):
+        self.engine, self.j = engine, journaler
+        self.caps = (1 << 20, 64)
+
+    def compact(self, gc_slot: np.ndarray) -> List[CompactedFile]:
+        """gc_slot: int32 per gid of the engine (PaxosManager.journal_gc_slots) -> what happened to each non-current
+        file, in the order of journaler.files before the call"""
+        import torch
+        files = [f for f in self.j.files if f != self.j.cur]
+        if not files:
+            return []
+        self.j.fos.flush()
+        blobs = []
+        for path in files + [self.j.cur]:
+            with open(path, "rb") as f:
+                blobs.append(f.read())
+        file_off = np.zeros(len(blobs) + 1, np.uint32)
+        file_off[1:] = np.cumsum([len(b) for b in blobs])
+        starts = np.concatenate([self.engine.L.journal_index(b, int(o)) for b, o in zip(blobs, file_off[:-1])])
+        dev = torch.device("cuda", torch.cuda.current_device())
+        data = torch.from_numpy(np.frombuffer(b"".join(blobs) or b"\0", np.uint8).copy()).to(dev)
+        gcs = torch.from_numpy(np.ascontiguousarray(gc_slot, np.int32)).to(dev)
+        r = self.engine.journal_compact_device(data, int(file_off[-1]), torch.from_numpy(file_off).to(dev),
+                                               torch.from_numpy(starts.astype(np.uint32)).to(dev), gcs, True,
+                                               self.caps)
+        self.caps = tuple(max(a, b) for a, b in zip(self.caps, r.sizes))
+        if r.rc != abi.GPX_OK:
+            raise ValueError("journal frames that do not parse: %s" % r.bad.cpu().numpy().tolist())
+        out = r.out.cpu().numpy()
+        fr = r.files.cpu().numpy().reshape(-1).view(abi.journal_file_dtype)[: len(files)]
+        results = [CompactedFile(int(x["status"]),
+                                 out[int(x["out_off"]): int(x["out_off"]) + int(x["out_bytes"])].tobytes()
+                                 if int(x["status"]) == JGC_COMPACTED else None,
+                                 int(x["kept"]), int(x["dropped"]), int(x["unresolved"])) for x in fr]
+        apply_compaction(self.j, files, results)
+        return results

@@ -1007,6 +1007,24 @@ class PaxosManager:
             executed += 1
         return executed
 
+    def journal_gc_slots(self, lane: int) -> np.ndarray:
+        """int32 per gid of the engine: the GC slot of lane's journal (gpx_journal_compact_device's gc_slot), gcSlot =
+        (cp - accGC < 0) ? cp : accGC (SQLPaxosLogger.deleteOutdatedMessages :1480-1482), cp the lane's last recorded
+        checkpoint slot of the group and accGC its acceptor's acc_gc_slot (gpx_dump_rows); -1 for a group without a
+        checkpoint (LogIndex.java:41) or without an instance"""
+        out = np.full(int(self.engine.cfg.max_groups), -1, np.int32)
+        cp: Dict[str, int] = {}
+        for name, l, slot, _ in self.checkpoints:
+            if l == lane:
+                cp[name] = slot
+        named = [(self.instances[n].gid, s) for n, s in cp.items() if n in self.instances]
+        if named:
+            gids = np.array([g for g, _ in named], np.uint32)
+            acc = self.engine.dump_rows(gids, lane)["acc_gc_slot"]
+            for (g, c), a in zip(named, acc.tolist()):
+                out[g] = c if _jsub(c, a) < 0 else a
+        return out
+
     def flush(self, max_rounds: int = 64) -> int:
         total = 0
         for _ in range(max_rounds):

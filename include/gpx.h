@@ -663,6 +663,68 @@ int gpx_log_frame_device(gpx_engine* e, uint32_t lane, uint64_t* from, const gpx
                          uint8_t* out, uint64_t* out_bytes, uint32_t* n_frames, gpx_journal_miss* missing,
                          uint32_t* n_missing, void* stream);
 
+/* ---- journal garbage collection on the device: compact journal files to the frames a checkpoint still needs ---------
+ * SQLPaxosLogger.compactLogfile :3350-3450 rewrites each journal file to the frames LogIndex.isLogMsgNeeded :331-345
+ * still wants, and deletes a file that keeps none.  gpx_journal_compact_device does that for k files of one lane's
+ * journal at once, in HBM.
+ *
+ *   Input     bytes[n_bytes]: the k = n_files files concatenated in roll order, file f at [file_off[f], file_off[f+1])
+ *             (file_off[0] = 0, ascending, file_off[k] = n_bytes); starts[n_frames]: the offset of every frame's
+ *             {int32 BE length} in bytes, ascending (gpx_journal_index writes them).  gc_slot[n_gids]: the GC slot of
+ *             each gid, n_gids >= max_groups; the caller computes gcSlot = (cp - accGC < 0) ? cp : accGC
+ *             (SQLPaxosLogger.deleteOutdatedMessages :1480-1482) from the group's last checkpoint slot cp and the
+ *             acceptor's acc_gc_slot (gpx_dump_rows), and -1 for a group without a checkpoint (LogIndex.java:41).
+ *   Parse     each frame's packet is an ACCEPT (AcceptPacket bytes), a DECISION or a PREPARE (the JSON of
+ *             journal.decision_json / prepare_json; other keys are allowed), read as (paxosID, version, slot, ballot);
+ *             a PREPARE's slot is PREP_MIN.  (paxosID, version) resolves to a gid as the wire decoders resolve it:
+ *             gpx_set_group_names' table, a live group at that version.
+ *   Keep      an unresolved frame is kept (a paused group, a stale version or a name not in the table: the call
+ *             cannot prove it unneeded).  A resolved one is dropped when slot - gc_slot[gid] <= 0 (int32 wrap
+ *             arithmetic).  A resolved PREPARE above the gc slot is also dropped when an indexed frame of its group --
+ *             a resolved frame of any type above the group's gc slot, in any of the k files -- has a higher ballot:
+ *             bnum - bnum' > 0, or equal bnums and bcoord - bcoord' > 0, tested entry by entry as the reference
+ *             does.  Every other frame is kept.
+ *             Deliberate divergence: SQLPaxosLogger.getSlot :492-496 returns an ACCEPT's or DECISION's ballot number
+ *             as its slot, so compactLogfile compares the ballot number with the GC slot.  The index built at journal
+ *             time uses the pvalue's slot (MessageLogDiskMap.add :412), and so does this call: an ACCEPT above the GC
+ *             slot whose ballot number is at or below it is kept.
+ *   Files     files[f] receives the file's gpx_journal_file.  A file whose last frame does not end at the file's end
+ *             (a torn tail: gpx_journal_index stops there) is GPX_JGC_TORN and left as it is, as is the last file
+ *             when last_readonly is set (GPX_JGC_UNCHANGED); their frames still count as indexed entries.  Of the
+ *             others, a file that keeps every frame is GPX_JGC_UNCHANGED, one that keeps none GPX_JGC_EMPTY (the
+ *             caller deletes it), any other GPX_JGC_COMPACTED: its kept frames, unchanged and in order, are at
+ *             out[out_off, out_off + out_bytes).  Only compacted files have bytes in out, in file order.
+ *   Errors    a frame whose length runs past its file or disagrees with the next start, the first frame of a file
+ *             not at the file's start, or a packet that does not parse: no file record and no byte is written,
+ *             bad[*n_bad] lists the frame indices in ascending order, and the call returns GPX_EINVAL.  A file_off
+ *             that is not ascending from 0 to n_bytes is GPX_EINVAL with no list.
+ *   Sizes     *out_bytes and *n_bad are HOST pointers, capacities in / sizes out; GPX_ERANGE reports the sizes and
+ *             writes nothing (out_bytes 0 when bad is the one too small).  n_bytes above 4 GiB - 1 is GPX_ERANGE.
+ * bytes, file_off, starts, gc_slot, out, files and bad are device pointers.  Stream-ordered on `stream` (NULL = the
+ * engine's stream), with the wire calls' scratch and ordering between streams; one synchronisation reads the totals.
+ * The call reads no group state but the groups' liveness. */
+enum { GPX_JGC_UNCHANGED = 0, GPX_JGC_COMPACTED = 1, GPX_JGC_EMPTY = 2, GPX_JGC_TORN = 3 };
+typedef struct gpx_journal_file { /* 24 B */
+  uint32_t status;     /* GPX_JGC_* */
+  uint32_t kept;       /* frames the file holds after the call */
+  uint32_t dropped;    /* frames removed */
+  uint32_t unresolved; /* of the frames, those whose name did not resolve (all kept) */
+  uint32_t out_off;    /* GPX_JGC_COMPACTED: the file's bytes in out */
+  uint32_t out_bytes;
+} gpx_journal_file;
+int gpx_journal_compact_device(gpx_engine* e, const uint8_t* bytes, uint64_t n_bytes, const uint32_t* file_off,
+                               uint32_t n_files, const uint32_t* starts, uint32_t n_frames, const int32_t* gc_slot,
+                               uint32_t n_gids, uint32_t last_readonly, uint8_t* out, uint64_t* out_bytes,
+                               gpx_journal_file* files, uint32_t* bad, uint32_t* n_bad, void* stream);
+/* The frame starts of a journal file in host memory, as journal.read_journal walks it: from offset 0, a frame is
+ * {int32 BE length}{length bytes}, and the walk stops at a negative length or at a frame that runs past n_bytes (a
+ * torn tail).  starts[k] = base + the offset of frame k, for up to cap frames; *n_frames receives the count and *end
+ * the offset where the walk stopped (n_bytes unless the tail is torn).  GPX_ERANGE when the count exceeds cap (the
+ * first cap are written), GPX_EINVAL on a null pointer or when base + n_bytes passes 4 GiB.  No engine is involved:
+ * the walk is a chain of dependent reads over bytes the caller has just read from the file. */
+int gpx_journal_index(const uint8_t* buf, uint64_t n_bytes, uint32_t base, uint32_t* starts, uint32_t cap,
+                      uint32_t* n_frames, uint64_t* end);
+
 /* Request bodies for a batch of gpx_log_find hits (blob_pos) or of carried-over pvalues (the latest log position
  * before the head that is congruent to frame_ref * 16 modulo log_ring_bytes) in ONE device->host copy:
  * ranges[i] = {absolute log position, length, offset in dst (a multiple of 16)}; range i lands at
