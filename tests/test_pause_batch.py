@@ -141,20 +141,12 @@ def emu_lib(tmp_path_factory):
     return C.CDLL(out)
 
 
-@pytest.mark.parametrize("journaling,R,seed,block", [(1, 3, 5, 128), (0, 3, 6, 1), (1, 5, 7, 33), (0, 2, 8, 128)])
-def test_kernel_source_on_the_host_equals_oracle(oracle_lib, emu_lib, journaling, R, seed, block):
-    """DevState's arrays are filled from the oracle engine's rows and group flags (committed / accepted windows are
-    synthesised so that every lane's caught-up answer is the oracle's), k_pause_groups runs thread by thread, and its
-    verdicts, rows and the state it leaves are the oracle's."""
-    G, W = 120, 8
-    nodes = [100, 101, 102, 103, 104][:R]
-    # (the oracle engine journals either way: with accepts kept in memory its last accepted pvalue never leaves and nothing
-    # pauses.  `journaling` here is the KERNEL's flag -- 0 makes it look through the synthesised accepted windows too)
-    eng = busy_engine(oracle_lib, G, seed, 1, R)
+def pause_state(eng, R, G, W, journaling, rng):
+    """DevState's arrays for k_pause_groups from the oracle engine's rows and group flags, with committed / accepted
+    windows synthesised so that every lane's caught-up answer is the oracle's"""
     all_g = np.arange(G, dtype=np.uint32)
     rows = [eng.dump_rows(all_g, l) for l in range(R)]
     flags = [eng.group_flags(all_g, l) for l in range(R)]
-    rng = np.random.default_rng(seed)
     live = (rows[0]["state"] != abi.ST_FREE).astype(np.uint8)
     acc_row = np.zeros((R, G, 4), dtype=np.int32)
     acc_aux = np.zeros((R, G), dtype=np.uint32)
@@ -182,6 +174,22 @@ def test_kernel_source_on_the_host_equals_oracle(oracle_lib, emu_lib, journaling
         acc_win[l, :, :, 7] = 1  # GPX_ENT_VALID
         livepv = busy & (why == 2)
         acc_win[l, w, :, 0] = np.where(livepv, r["acc_gc_slot"] + 1 + rng.integers(0, 4, size=G), acc_win[l, w, :, 0])
+    return live, acc_row, acc_aux, acc_win, coord_row, node_slots
+
+
+@pytest.mark.parametrize("journaling,R,seed,block", [(1, 3, 5, 128), (0, 3, 6, 1), (1, 5, 7, 33), (0, 2, 8, 128)])
+def test_kernel_source_on_the_host_equals_oracle(oracle_lib, emu_lib, journaling, R, seed, block):
+    """DevState's arrays are filled from the oracle engine's rows and group flags (committed / accepted windows are
+    synthesised so that every lane's caught-up answer is the oracle's), k_pause_groups runs thread by thread, and its
+    verdicts, rows and the state it leaves are the oracle's."""
+    G, W = 120, 8
+    nodes = [100, 101, 102, 103, 104][:R]
+    # (the oracle engine journals either way: with accepts kept in memory its last accepted pvalue never leaves and nothing
+    # pauses.  `journaling` here is the KERNEL's flag -- 0 makes it look through the synthesised accepted windows too)
+    eng = busy_engine(oracle_lib, G, seed, 1, R)
+    all_g = np.arange(G, dtype=np.uint32)
+    rng = np.random.default_rng(seed)
+    live, acc_row, acc_aux, acc_win, coord_row, node_slots = pause_state(eng, R, G, W, journaling, rng)
     gids = rng.permutation(G + 2).astype(np.uint32)
     want_rows, want_ok = eng.pause_groups(gids)
     got_rows = np.zeros((len(gids), R), dtype=abi.row_dtype)

@@ -6,8 +6,14 @@
   * the oracle's phase 1b against the host-language twin (two restatements of PaxosCoordinatorState.java:264-587).
 
 A run's sanity assertions ("some but not all groups paused", "every verdict occurred") can miss for an unlucky seed; only
-mismatches between the two sides count as failures.     python tools/soak_emu.py [iterations]
+mismatches between the two sides count as failures.
+
+    python tools/soak_emu.py [iterations] [--order asc|desc|shuffle]
+
+--order sets the order the emulated launches run their threads in (tests/emu/cuda_emu.h); shuffle draws a fresh
+permutation seed for every iteration and prints it with a failure.
 """
+import argparse
 import ctypes as C
 import os
 import subprocess
@@ -34,10 +40,12 @@ def build(src):
     subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", "-I", "/usr/local/cuda/include",
                            "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
                            "-x", "c++", os.path.join(ROOT, "tests", "emu", src), "-o", out])
-    return C.CDLL(out)
+    lib = C.CDLL(out)
+    lib.emu_set_order.argtypes = [C.c_char_p]
+    return lib
 
 
-def attempt(fn, *args):
+def attempt(spec, fn, *args):
     try:
         fn(*args)
         return 1
@@ -45,11 +53,11 @@ def attempt(fn, *args):
         lines = traceback.format_exc().splitlines()
         if any(k in " ".join(lines[-4:]) for k in SANITY):
             return 0
-        print(args, "\n".join(lines[-25:]))
+        print(f"order {spec}:", fn.__name__, args, "\n".join(lines[-25:]))
         raise
 
 
-def main(iters):
+def main(iters, order="asc"):
     lib = oracle_library()
     e1, e2, e3 = build("p1b_emu.cpp"), build("pause_emu.cpp"), build("logfind_emu.cpp")
     e3.emu_log_find.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
@@ -58,22 +66,29 @@ def main(iters):
     ok = 0
     t0 = time.time()
     for _ in range(iters):
+        spec = f"shuffle:{int(rng.integers(1 << 62))}" if order == "shuffle" else order
+        for e in (e1, e2, e3):  # also restarts the launch count: an iteration's orders follow from its seed alone
+            assert e.emu_set_order(spec.encode()) == 0, spec
         seed = int(rng.integers(100, 60000))
         R = int(rng.choice([1, 2, 3, 3, 4, 5]))
         wrap = bool(rng.integers(0, 2))
         ln = None
         if R >= 3 and rng.integers(0, 3) == 0:
             ln = [tp.NODES5[i] for i in rng.choice(R, size=int(rng.integers(1, R)), replace=False)]
-        ok += attempt(tp.test_kernel_source_on_the_host_equals_oracle, lib, e1, R, seed, wrap, int(rng.choice([1, 7, 33, 64])), ln)
-        ok += attempt(tp.test_oracle_phase1b_equals_the_host_twin, lib, R, seed, wrap, ln)
-        ok += attempt(tb.test_kernel_source_on_the_host_equals_oracle, lib, e2, int(rng.integers(0, 2)), int(rng.choice([2, 3, 5])),
+        ok += attempt(spec, tp.test_kernel_source_on_the_host_equals_oracle, lib, e1, R, seed, wrap, int(rng.choice([1, 7, 33, 64])), ln)
+        ok += attempt(spec, tp.test_oracle_phase1b_equals_the_host_twin, lib, R, seed, wrap, ln)
+        ok += attempt(spec, tb.test_kernel_source_on_the_host_equals_oracle, lib, e2, int(rng.integers(0, 2)), int(rng.choice([2, 3, 5])),
                       seed, int(rng.choice([1, 33, 128])))
-        ok += attempt(tl.test_kernel_source_on_the_host_equals_oracle, lib, e3, seed, int(rng.choice([1, 3, 7])),
+        ok += attempt(spec, tl.test_kernel_source_on_the_host_equals_oracle, lib, e3, seed, int(rng.choice([1, 3, 7])),
                       int(rng.choice([1, 64, 256])))
-        ok += attempt(tl.test_kernel_source_on_a_ring_that_wraps, lib, e3, seed)
-    print(f"{iters} iterations x 5 checks: {ok} complete, {5 * iters - ok} ended at a sanity assertion, 0 mismatches; "
+        ok += attempt(spec, tl.test_kernel_source_on_a_ring_that_wraps, lib, e3, seed)
+    print(f"{iters} iterations x 5 checks, order {order}: {ok} complete, {5 * iters - ok} ended at a sanity assertion, 0 mismatches; "
           f"{time.time() - t0:.0f} s")
 
 
 if __name__ == "__main__":
-    main(int(sys.argv[1]) if len(sys.argv) > 1 else 50)
+    ap = argparse.ArgumentParser()
+    ap.add_argument("iterations", type=int, nargs="?", default=50)
+    ap.add_argument("--order", choices=("asc", "desc", "shuffle"), default="asc")
+    a = ap.parse_args()
+    main(a.iterations, a.order)
