@@ -82,9 +82,9 @@ struct gpx_engine {
   RoundCtl* d_ctl = nullptr;
   RoundCtl* d_rctl = nullptr; /* [2] the round kernels' own control blocks: they alternate as the working block, each
                                * round zeroes the one the next round counts into */
-  const RoundCtl* last_ctl = nullptr; /* where the last round left its counters */
-  int round_mode = 0;         /* gpx_set_round_mode: 0 / 1 device tail launch of k_round_slow, 2 host-launched pair;
-                               * 3 / 4 the same two with the team kernel k_round in place of k_round_g */
+  /* gpx_set_round_mode, decoded by set_round_mode */
+  bool round_team = false;      /* the team kernel k_round in place of k_round_g */
+  bool round_slow_host = false; /* the host launches k_round_slow behind the round kernel, not the device */
   uint32_t rparity = 0;
   bool ls_live = false; /* a k_round_g<L, true> launch may have left VALID lockstep records (ls_settle) */
   RoundCtl* h_ctl = nullptr; /* pinned */
@@ -121,7 +121,6 @@ struct gpx_engine {
   /* timing */
   int n_sms = 132; /* H100 SXM; replaced by the device's own count at engine creation */
   bool timing = false;
-  bool compact_fused = false; /* round_on_stream(fused = false): k_propose + k_act instead of the four phase kernels */
   cudaEvent_t ev[5];
   gpx_kernel_times kt;
   /* phase-2 wire calls (gpx_wire_host.inc): group names, allocated by the first call that needs them */
@@ -168,6 +167,9 @@ struct gpx_engine {
     return GPX_OK;
   }
 };
+
+/* the stream of a call that takes one: the caller's, or the engine's when the caller passes none */
+static cudaStream_t call_stream(gpx_engine* e, void* stream) { return stream ? (cudaStream_t)stream : e->stream; }
 
 extern "C" {
 
@@ -218,6 +220,15 @@ int32_t gpx_get_cpi(int32_t cpi, double noise, int32_t name_hash) {
 }
 
 /* ---- lifecycle -------------------------------------------------------------------- */
+/* gpx_set_round_mode's modes: 0 / 1 device tail launch of k_round_slow, 2 host-launched pair; 3 / 4 the same two with
+ * the team kernel k_round in place of k_round_g.  false (nothing changed) when `mode` is none of them */
+static bool set_round_mode(gpx_engine* e, int mode) {
+  if (mode < 0 || mode > 4) return false;
+  e->round_team = mode >= 3;
+  e->round_slow_host = mode == 2 || mode == 4;
+  return true;
+}
+
 int gpx_engine_create(const gpx_config* cfg, gpx_engine** out) {
   if (!cfg || !out) return fail(GPX_EINVAL, "null argument");
   if (cfg->abi_version != GPX_ABI_VERSION) return fail(GPX_EINVAL, "abi_version mismatch");
@@ -344,7 +355,7 @@ int gpx_engine_create(const gpx_config* cfg, gpx_engine** out) {
   }
   cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking);
   for (int i = 0; i < 5; i++) cudaEventCreate(&e->ev[i]);
-  if (const char* rm = getenv("GPX_ROUND_MODE")) e->round_mode = atoi(rm) >= 0 && atoi(rm) <= 4 ? atoi(rm) : 0; /* tuning / tests */
+  if (const char* rm = getenv("GPX_ROUND_MODE")) set_round_mode(e, atoi(rm)); /* tuning / tests; out of range: mode 0 */
   e->h_version.assign(G, 0);
   e->h_name_hash.assign(G, 0);
   cudaError_t err = cudaDeviceSynchronize();
@@ -632,7 +643,7 @@ static bool def_config(const DevState& S) { /* the reference's default configura
   return S.journaling && S.gc_majority_executed && S.log_meta && !S.cpi_per_group;
 }
 static bool round_uses_ls(const gpx_engine* e) {
-  return e->S.ls_off && e->round_mode < 3 && def_config(e->S);
+  return e->S.ls_off && !e->round_team && def_config(e->S);
 }
 static void ls_settle(gpx_engine* e, cudaStream_t st) {
   if (!e->ls_live) return;
@@ -641,7 +652,18 @@ static void ls_settle(gpx_engine* e, cudaStream_t st) {
 }
 
 /* ---- kernel launch helpers (device pointers) ------------------------------------- */
-static int launch_propose(gpx_engine* e, const gpx_request_rec* d_reqs, const uint8_t* d_payload,
+/* what a phase launch counts into and appends to: the control block, the ACCEPT records k_propose writes, and the
+ * queue of EXEC rows beyond one per (record, lane) with its capacity.  The host-buffer calls use the engine's own
+ * (engine_out); the device forms pass the caller's. */
+struct PhaseOut {
+  RoundCtl* ctl;
+  gpx_accept_rec* accepts;
+  gpx_exec_rec* extra;
+  uint32_t extra_cap;
+};
+static PhaseOut engine_out(const gpx_engine* e) { return {e->d_ctl, e->d_accepts, e->d_extra, e->extra_cap}; }
+
+static int launch_propose(gpx_engine* e, const PhaseOut& o, const gpx_request_rec* d_reqs, const uint8_t* d_payload,
                           uint64_t payload_al, uint32_t n, int32_t* d_status, cudaStream_t st,
                           uint32_t* d_head = nullptr) {
   ls_settle(e, st);
@@ -649,11 +671,11 @@ static int launch_propose(gpx_engine* e, const gpx_request_rec* d_reqs, const ui
   A.reqs = d_reqs;
   A.n = n;
   A.payload_bytes_al = payload_al;
-  A.accepts = e->d_accepts;
+  A.accepts = o.accepts;
   A.status = d_status;
   A.copy_tab = e->d_copy_tab;
   A.copy_dst = e->d_copy_dst;
-  A.ctl = e->d_ctl;
+  A.ctl = o.ctl;
   k_propose<<<cdiv(n, GPX_BLOCK), GPX_BLOCK, 0, st>>>(e->S, A, e->d_mark, d_head);
   k_build_blobs<<<cdiv(n, GPX_BLOCK), GPX_BLOCK, 0, st>>>(A, d_payload, e->d_blob1, e->d_mark);
   CK(cudaGetLastError());
@@ -673,9 +695,9 @@ static int launch_propose(gpx_engine* e, const gpx_request_rec* d_reqs, const ui
     default: KERNEL<8><<<grid, GPX_BLOCK, 0, st>>>(__VA_ARGS__); break;                \
   }
 
-static int launch_accept(gpx_engine* e, bool fused, const gpx_accept_rec* d_recs, const uint32_t* n_ptr,
-                         uint32_t n_max, const uint8_t* blob0, uint64_t blob0_bytes, const uint8_t* blob1,
-                         uint64_t blob1_bytes, const unsigned long long* blob1_used_ptr,
+static int launch_accept(gpx_engine* e, const PhaseOut& o, bool fused, const gpx_accept_rec* d_recs,
+                         const uint32_t* n_ptr, uint32_t n_max, const uint8_t* blob0, uint64_t blob0_bytes,
+                         const uint8_t* blob1, uint64_t blob1_bytes, const unsigned long long* blob1_used_ptr,
                          gpx_accept_reply_rec* d_replies, gpx_decision_rec* d_dec, gpx_exec_rec* d_exec,
                          cudaStream_t st) {
   ls_settle(e, st);
@@ -692,9 +714,9 @@ static int launch_accept(gpx_engine* e, bool fused, const gpx_accept_rec* d_recs
   A.decisions = d_dec;
   A.out_mask = e->d_out_mask;
   A.exec = d_exec;
-  A.extra = e->d_extra;
-  A.extra_cap = e->extra_cap;
-  A.n_extra = &e->d_ctl->n_extra;
+  A.extra = o.extra;
+  A.extra_cap = o.extra_cap;
+  A.n_extra = &o.ctl->n_extra;
   const uint32_t grid = cdiv(n_max, GPX_BLOCK);
   /* host mirror of the ring heads (k_accept: one segment; k_act: two, back to back) */
   log_advance(e, GPX_SEG_ACC_BYTES(n_max, blob0_bytes + blob1_bytes) + (fused ? GPX_SEG_DEC_BYTES(n_max) : 0ull),
@@ -709,8 +731,8 @@ static int launch_accept(gpx_engine* e, bool fused, const gpx_accept_rec* d_recs
   return GPX_OK;
 }
 
-static int launch_tally(gpx_engine* e, const gpx_accept_reply_rec* d_replies, const uint32_t* n_ptr, uint32_t mult,
-                        uint32_t n_max, gpx_decision_rec* d_dec, cudaStream_t st) {
+static int launch_tally(gpx_engine* e, const PhaseOut& o, const gpx_accept_reply_rec* d_replies, const uint32_t* n_ptr,
+                        uint32_t mult, uint32_t n_max, gpx_decision_rec* d_dec, cudaStream_t st) {
   ls_settle(e, st);
   TallyArgs A;
   A.replies = d_replies;
@@ -718,7 +740,7 @@ static int launch_tally(gpx_engine* e, const gpx_accept_reply_rec* d_replies, co
   A.mult = mult;
   A.n_max = n_max;
   A.decisions = d_dec;
-  A.n_decisions = &e->d_ctl->n_decisions;
+  A.n_decisions = &o.ctl->n_decisions;
   if (mult > 1 && mult == e->cfg.n_lanes) { /* [ACCEPT][lane] layout of the phase pipeline: one thread per slot */
     GPX_DISPATCH_L(mult, k_tally_slots, cdiv(n_max / mult, GPX_BLOCK), st, e->S, A);
   } else
@@ -727,17 +749,17 @@ static int launch_tally(gpx_engine* e, const gpx_accept_reply_rec* d_replies, co
   return GPX_OK;
 }
 
-static int launch_commit(gpx_engine* e, const gpx_decision_rec* d_dec, const uint32_t* n_ptr, uint32_t n_max,
-                         gpx_exec_rec* d_exec, cudaStream_t st) {
+static int launch_commit(gpx_engine* e, const PhaseOut& o, const gpx_decision_rec* d_dec, const uint32_t* n_ptr,
+                         uint32_t n_max, gpx_exec_rec* d_exec, cudaStream_t st) {
   ls_settle(e, st);
   CommitArgs A;
   A.decisions = d_dec;
   A.n_ptr = n_ptr;
   A.n_max = n_max;
   A.exec = d_exec;
-  A.extra = e->d_extra;
-  A.extra_cap = e->extra_cap;
-  A.n_extra = &e->d_ctl->n_extra;
+  A.extra = o.extra;
+  A.extra_cap = o.extra_cap;
+  A.n_extra = &o.ctl->n_extra;
   log_advance(e, GPX_SEG_DEC_BYTES(n_max), true);
   GPX_DISPATCH_L(e->cfg.n_lanes, k_commit, cdiv(n_max, GPX_BLOCK), st, e->S, A);
   log_flip(e);
@@ -784,33 +806,27 @@ static void launch_round_t(uint32_t n, bool team, cudaStream_t st, const DevStat
   }
 }
 }
-static int launch_round(gpx_engine* e, const gpx_request_rec* d_reqs, const uint8_t* d_payload, uint64_t pal,
-                        uint32_t n, int32_t* d_status, gpx_exec_rec* d_exec, cudaStream_t st,
-                        RoundCtl* d_ctl = nullptr, gpx_exec_rec* d_extra = nullptr, uint32_t extra_cap = 0,
+/* the round counts into o.ctl, which the caller zeroed; a null o.ctl selects the engine's own blocks [0] / [1], which
+ * alternate (each round zeroes the one the next round uses), and launch_round leaves the one it used in o.ctl */
+static int launch_round(gpx_engine* e, PhaseOut& o, const gpx_request_rec* d_reqs, const uint8_t* d_payload,
+                        uint64_t pal, uint32_t n, int32_t* d_status, gpx_exec_rec* d_exec, cudaStream_t st,
                         gpx_exec_sum* d_sum = nullptr) {
-  /* the round counts into `working`: the engine's own blocks [0] / [1] alternate (each round zeroes the one the next
-   * round uses); a caller-provided block is zeroed by the caller */
   RoundCtl* ctl_zero = nullptr;
-  if (!d_ctl) {
-    d_ctl = e->d_rctl + e->rparity;
+  if (!o.ctl) {
+    o.ctl = e->d_rctl + e->rparity;
     ctl_zero = e->d_rctl + (e->rparity ^ 1u);
     e->rparity ^= 1u;
-  }
-  e->last_ctl = d_ctl;
-  if (!d_extra) {
-    d_extra = e->d_extra;
-    extra_cap = e->extra_cap;
   }
   RoundArgs RA;
   memset(&RA, 0, sizeof RA);
   RA.P.reqs = d_reqs;
   RA.P.n = n;
   RA.P.payload_bytes_al = pal;
-  RA.P.accepts = e->d_accepts;
+  RA.P.accepts = o.accepts;
   RA.P.status = d_status;
   RA.P.copy_tab = e->d_copy_tab;
   RA.P.copy_dst = e->d_copy_dst;
-  RA.P.ctl = d_ctl;
+  RA.P.ctl = o.ctl;
   RA.ctl_zero = ctl_zero;
   RA.sum = d_sum;
   RA.A.n_max = n;
@@ -821,14 +837,14 @@ static int launch_round(gpx_engine* e, const gpx_request_rec* d_reqs, const uint
   RA.A.decisions = e->d_decisions;
   RA.A.out_mask = e->d_out_mask;
   RA.A.exec = d_exec;
-  RA.A.extra = d_extra;
-  RA.A.extra_cap = extra_cap;
-  RA.A.n_extra = &d_ctl->n_extra;
+  RA.A.extra = o.extra;
+  RA.A.extra_cap = o.extra_cap;
+  RA.A.n_extra = &o.ctl->n_extra;
   RA.blob1w = e->d_blob1;
   RA.todo = e->d_todo;
   RA.todo_end = e->d_todo + e->cfg.max_batch_recs;
   RA.mark = e->d_mark;
-  RA.n_todo = &d_ctl->n_todo;
+  RA.n_todo = &o.ctl->n_todo;
   RA.blob1_res = round_blob1(e, n, pal);
   RA.A.blob1_bytes = RA.blob1_res;
   RA.pay_bytes = pal + RA.blob1_res;
@@ -844,9 +860,8 @@ static int launch_round(gpx_engine* e, const gpx_request_rec* d_reqs, const uint
   const uint32_t teams_per_block = (GPX_RBLOCK / 32u) * (32u / L); /* teams of L adjacent lanes */
   const uint32_t grid = cdiv((uint64_t)n, teams_per_block);
   RA.slow_grid = std::min<uint32_t>(grid, 2u * (uint32_t)e->n_sms);
-  RA.tail_launch = (e->round_mode == 2 || e->round_mode == 4) ? 0u : 1u; /* grid-stride over the todo list; all
-                                                                            * blocks resident (grid barriers) */
-  const bool team = e->round_mode >= 3;
+  RA.tail_launch = !e->round_slow_host; /* grid-stride over the todo list; all blocks resident (grid barriers) */
+  const bool team = e->round_team;
   switch (L) {
     case 1: launch_round_t<1, 1>(n, team, st, e->S, RA); break;
     case 2: launch_round_t<2, 2>(n, team, st, e->S, RA); break;
@@ -917,6 +932,19 @@ static int fetch_ctl(gpx_engine* e, const RoundCtl* src = nullptr) {
   CK(cudaStreamSynchronize(e->stream));
   return GPX_OK;
 }
+/* the EXEC rows beyond one per (record, lane) that a call appended to the engine's queue, `n_extra` of them, into the
+ * caller's buffer as far as both hold; synchronises when it copied, or always with `sync` (the caller's own copies
+ * are still in flight on `st`) */
+static int copy_extra(gpx_engine* e, uint32_t n_extra, gpx_exec_rec* out, uint32_t cap, cudaStream_t st,
+                      bool sync = false) {
+  const uint32_t cp = std::min(std::min(n_extra, cap), e->extra_cap);
+  if (cp && out) {
+    CK(cudaMemcpyAsync(out, e->d_extra, cp * sizeof(gpx_exec_rec), cudaMemcpyDeviceToHost, st));
+    sync = true;
+  }
+  if (sync) CK(cudaStreamSynchronize(st));
+  return GPX_OK;
+}
 
 /* ---- data path: host buffers -------------------------------------------------------- */
 int gpx_propose(gpx_engine* e, uint32_t n, const gpx_request_rec* reqs, const uint8_t* payload,
@@ -934,7 +962,7 @@ int gpx_propose(gpx_engine* e, uint32_t n, const gpx_request_rec* reqs, const ui
   CK(cudaMemsetAsync(e->d_ctl, 0, sizeof(RoundCtl), st));
   CK(cudaMemcpyAsync(e->d_reqs, reqs, n * sizeof(gpx_request_rec), cudaMemcpyHostToDevice, st));
   if (payload_bytes) CK(cudaMemcpyAsync(e->d_payload, payload, payload_bytes, cudaMemcpyHostToDevice, st));
-  rc = launch_propose(e, e->d_reqs, e->d_payload, pal, n, e->d_status, st);
+  rc = launch_propose(e, engine_out(e), e->d_reqs, e->d_payload, pal, n, e->d_status, st);
   if (rc) return rc;
   rc = fetch_ctl(e);
   if (rc) return rc;
@@ -971,21 +999,15 @@ int gpx_handle_accepts(gpx_engine* e, uint32_t n, const gpx_accept_rec* accepts,
   CK(cudaMemsetAsync(e->d_ctl, 0, sizeof(RoundCtl), st));
   CK(cudaMemcpyAsync(e->d_accepts, accepts, n * sizeof(gpx_accept_rec), cudaMemcpyHostToDevice, st));
   if (blob_bytes) CK(cudaMemcpyAsync(e->d_blob1, blob, blob_bytes, cudaMemcpyHostToDevice, st));
-  rc = launch_accept(e, false, e->d_accepts, nullptr, n, e->d_blob1, blob_bytes, nullptr, 0, nullptr, e->d_replies,
-                     nullptr, nullptr, st);
+  rc = launch_accept(e, engine_out(e), false, e->d_accepts, nullptr, n, e->d_blob1, blob_bytes, nullptr, 0, nullptr,
+                     e->d_replies, nullptr, nullptr, st);
   if (rc) return rc;
   CK(cudaMemcpyAsync(out_replies, e->d_replies, (size_t)n * L * sizeof(gpx_accept_reply_rec), cudaMemcpyDeviceToHost,
                      st));
   rc = fetch_ctl(e);
   if (rc) return rc;
-  uint32_t nx = e->h_ctl->n_extra;
-  if (n_extra) *n_extra = nx;
-  uint32_t cp = std::min(std::min(nx, extra_cap), e->extra_cap);
-  if (cp && out_extra_exec) {
-    CK(cudaMemcpyAsync(out_extra_exec, e->d_extra, cp * sizeof(gpx_exec_rec), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
-  return GPX_OK;
+  if (n_extra) *n_extra = e->h_ctl->n_extra;
+  return copy_extra(e, e->h_ctl->n_extra, out_extra_exec, extra_cap, st);
 }
 
 int gpx_handle_accept_replies(gpx_engine* e, uint32_t n, const gpx_accept_reply_rec* replies,
@@ -998,7 +1020,7 @@ int gpx_handle_accept_replies(gpx_engine* e, uint32_t n, const gpx_accept_reply_
   cudaStream_t st = e->stream;
   CK(cudaMemsetAsync(e->d_ctl, 0, sizeof(RoundCtl), st));
   CK(cudaMemcpyAsync(e->d_replies, replies, n * sizeof(gpx_accept_reply_rec), cudaMemcpyHostToDevice, st));
-  int rc = launch_tally(e, e->d_replies, nullptr, 1, n, e->d_decisions, st);
+  int rc = launch_tally(e, engine_out(e), e->d_replies, nullptr, 1, n, e->d_decisions, st);
   if (rc) return rc;
   rc = fetch_ctl(e);
   if (rc) return rc;
@@ -1024,19 +1046,13 @@ int gpx_handle_decisions(gpx_engine* e, uint32_t n, const gpx_decision_rec* deci
   const uint32_t L = e->cfg.n_lanes;
   CK(cudaMemsetAsync(e->d_ctl, 0, sizeof(RoundCtl), st));
   CK(cudaMemcpyAsync(e->d_decisions, decisions, n * sizeof(gpx_decision_rec), cudaMemcpyHostToDevice, st));
-  rc = launch_commit(e, e->d_decisions, nullptr, n, e->d_exec, st);
+  rc = launch_commit(e, engine_out(e), e->d_decisions, nullptr, n, e->d_exec, st);
   if (rc) return rc;
   CK(cudaMemcpyAsync(out_exec, e->d_exec, (size_t)n * L * sizeof(gpx_exec_rec), cudaMemcpyDeviceToHost, st));
   rc = fetch_ctl(e);
   if (rc) return rc;
-  uint32_t nx = e->h_ctl->n_extra;
-  if (n_extra) *n_extra = nx;
-  uint32_t cp = std::min(std::min(nx, extra_cap), e->extra_cap);
-  if (cp && out_extra_exec) {
-    CK(cudaMemcpyAsync(out_extra_exec, e->d_extra, cp * sizeof(gpx_exec_rec), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
-  return GPX_OK;
+  if (n_extra) *n_extra = e->h_ctl->n_extra;
+  return copy_extra(e, e->h_ctl->n_extra, out_extra_exec, extra_cap, st);
 }
 
 /* phase 1a at the acceptors: PISM.handlePrepare for a batch of PREPAREs, host buffers */
@@ -1126,8 +1142,8 @@ int gpx_handle_accepts_fused(gpx_engine* e, uint32_t n, const gpx_accept_rec* ac
   CK(cudaMemsetAsync(e->d_ctl, 0, sizeof(RoundCtl), st));
   CK(cudaMemcpyAsync(e->d_accepts, accepts, n * sizeof(gpx_accept_rec), cudaMemcpyHostToDevice, st));
   if (blob_bytes) CK(cudaMemcpyAsync(e->d_blob1, blob, blob_bytes, cudaMemcpyHostToDevice, st));
-  rc = launch_accept(e, true, e->d_accepts, nullptr, n, e->d_blob1, blob_bytes, nullptr, 0, nullptr, e->d_replies,
-                     e->d_decisions, e->d_exec, st);
+  rc = launch_accept(e, engine_out(e), true, e->d_accepts, nullptr, n, e->d_blob1, blob_bytes, nullptr, 0, nullptr,
+                     e->d_replies, e->d_decisions, e->d_exec, st);
   if (rc) return rc;
   /* replies consumed by a local coordinator never reach HBM: out_mask says which reply slots were written */
   e->h_out_mask.resize(n);
@@ -1151,30 +1167,31 @@ int gpx_handle_accepts_fused(gpx_engine* e, uint32_t n, const gpx_accept_rec* ac
         r.slot = accepts[i].h.slot;
         r.who = GPX_WHO(0xffu, 0xffu, GPX_F_VOID);
       }
-  uint32_t nx = e->h_ctl->n_extra;
-  if (n_extra) *n_extra = nx;
-  uint32_t cp = std::min(std::min(nx, extra_cap), e->extra_cap);
-  if (cp && out_extra_exec) {
-    CK(cudaMemcpyAsync(out_extra_exec, e->d_extra, cp * sizeof(gpx_exec_rec), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-  }
-  return GPX_OK;
+  if (n_extra) *n_extra = e->h_ctl->n_extra;
+  return copy_extra(e, e->h_ctl->n_extra, out_extra_exec, extra_cap, st);
 }
 
-/* one round on device pointers.  fused: k_propose -> k_act (replies, decisions and rows stay in registers);
- * phases: k_propose -> k_accept -> k_tally -> k_commit (inter-replica records go through HBM) */
-static int round_on_stream(gpx_engine* e, bool fused, const gpx_request_rec* d_reqs, const uint8_t* d_payload,
+/* one round on device pointers.  fused: the round kernel (launch_round), one EXEC row per request;
+ * phases: k_propose -> k_accept -> k_tally -> k_commit (inter-replica records go through HBM);
+ * compact: k_propose -> k_act (replies, decisions and rows stay in registers), one EXEC row per ACCEPT */
+enum class RoundForm { fused, phases, compact };
+/* *ctl: the control block the round counted into */
+static int round_on_stream(gpx_engine* e, RoundForm form, const gpx_request_rec* d_reqs, const uint8_t* d_payload,
                            uint64_t payload_bytes, uint32_t n, int32_t* d_status, gpx_exec_rec* d_exec,
-                           cudaStream_t st) {
+                           cudaStream_t st, const RoundCtl** ctl = nullptr) {
   const uint64_t pal = (payload_bytes + 15) & ~15ull;
   const uint32_t L = e->cfg.n_lanes;
   const bool tm = e->timing;
+  const bool fused = form == RoundForm::fused;
+  PhaseOut o = engine_out(e);
   if (!fused || !round_uses_ls(e)) ls_settle(e, st); /* outside the timed window */
-  if (!fused) CK(cudaMemsetAsync(e->d_ctl, 0, sizeof(RoundCtl), st)); /* the fused kernels keep their own block zero */
+  if (!fused) CK(cudaMemsetAsync(o.ctl, 0, sizeof(RoundCtl), st)); /* the fused kernels keep their own block zero */
   if (tm) cudaEventRecord(e->ev[0], st);
   if (fused) { /* the whole round is ONE kernel */
-    int rc1 = launch_round(e, d_reqs, d_payload, pal, n, d_status, d_exec, st);
+    o.ctl = nullptr; /* it counts into the round kernels' own blocks */
+    int rc1 = launch_round(e, o, d_reqs, d_payload, pal, n, d_status, d_exec, st);
     if (rc1) return rc1;
+    if (ctl) *ctl = o.ctl;
     if (tm) {
       cudaEventRecord(e->ev[1], st);
       cudaEventSynchronize(e->ev[1]);
@@ -1185,23 +1202,25 @@ static int round_on_stream(gpx_engine* e, bool fused, const gpx_request_rec* d_r
     }
     return GPX_OK;
   }
-  int rc = launch_propose(e, d_reqs, d_payload, pal, n, d_status, st);
+  const bool compact = form == RoundForm::compact;
+  int rc = launch_propose(e, o, d_reqs, d_payload, pal, n, d_status, st);
   if (rc) return rc;
   if (tm) cudaEventRecord(e->ev[1], st);
   /* the ACCEPT segment mirrors the payload arena plus the constructed blobs actually used */
-  rc = launch_accept(e, e->compact_fused, e->d_accepts, &e->d_ctl->n_accepts, n, d_payload, pal, e->d_blob1, 0,
-                     &e->d_ctl->blob1_used, e->d_replies, e->d_decisions, d_exec, st);
+  rc = launch_accept(e, o, compact, o.accepts, &o.ctl->n_accepts, n, d_payload, pal, e->d_blob1, 0,
+                     &o.ctl->blob1_used, e->d_replies, e->d_decisions, d_exec, st);
   if (rc) return rc;
   if (tm) cudaEventRecord(e->ev[2], st);
-  if (!e->compact_fused) {
-    rc = launch_tally(e, e->d_replies, &e->d_ctl->n_accepts, L, n * L, e->d_decisions, st);
+  if (!compact) {
+    rc = launch_tally(e, o, e->d_replies, &o.ctl->n_accepts, L, n * L, e->d_decisions, st);
     if (rc) return rc;
   }
   if (tm) cudaEventRecord(e->ev[3], st);
-  if (!e->compact_fused) {
-    rc = launch_commit(e, e->d_decisions, &e->d_ctl->n_decisions, n, d_exec, st);
+  if (!compact) {
+    rc = launch_commit(e, o, e->d_decisions, &o.ctl->n_decisions, n, d_exec, st);
     if (rc) return rc;
   }
+  if (ctl) *ctl = o.ctl;
   if (tm) {
     cudaEventRecord(e->ev[4], st);
     cudaEventSynchronize(e->ev[4]);
@@ -1221,9 +1240,8 @@ static int round_on_stream(gpx_engine* e, bool fused, const gpx_request_rec* d_r
 
 int gpx_set_round_mode(gpx_engine* e, int mode) {
   if (!e) return fail(GPX_EINVAL, "null argument");
-  if (mode < 0 || mode > 4)
+  if (!set_round_mode(e, mode))
     return fail(GPX_EINVAL, "round mode: 0 / 1 device tail launch, 2 host-launched pair, 3 / 4 the same with k_round");
-  e->round_mode = mode;
   return GPX_OK;
 }
 
@@ -1244,19 +1262,19 @@ static int round_host(gpx_engine* e, bool fused, uint32_t n, const gpx_request_r
   const uint32_t L = e->cfg.n_lanes;
   CK(cudaMemcpyAsync(e->d_reqs, reqs, n * sizeof(gpx_request_rec), cudaMemcpyHostToDevice, st));
   if (payload_bytes) CK(cudaMemcpyAsync(e->d_payload, payload, payload_bytes, cudaMemcpyHostToDevice, st));
-  rc = round_on_stream(e, fused, e->d_reqs, e->d_payload, payload_bytes, n, e->d_status, e->d_exec, st);
+  const RoundCtl* ctl = nullptr;
+  rc = round_on_stream(e, fused ? RoundForm::fused : RoundForm::phases, e->d_reqs, e->d_payload, payload_bytes, n,
+                       e->d_status, e->d_exec, st, &ctl);
   if (rc) return rc;
   CK(cudaMemcpyAsync(status, e->d_status, n * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  rc = fetch_ctl(e, fused ? e->last_ctl : nullptr);
+  rc = fetch_ctl(e, ctl);
   if (rc) return rc;
   /* fused: one EXEC row per REQUEST index (VOID where the request carries no ACCEPT); phases: one per DECISION */
   const uint32_t rows = fused ? n : e->h_ctl->n_decisions;
   const uint32_t nx = e->h_ctl->n_extra;
   if (rows) CK(cudaMemcpyAsync(out_exec, e->d_exec, (size_t)rows * L * sizeof(gpx_exec_rec), cudaMemcpyDeviceToHost, st));
-  uint32_t cp = std::min(std::min(nx, extra_cap), e->extra_cap);
-  if (cp && out_extra_exec)
-    CK(cudaMemcpyAsync(out_extra_exec, e->d_extra, cp * sizeof(gpx_exec_rec), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
+  rc = copy_extra(e, nx, out_extra_exec, extra_cap, st, true);
+  if (rc) return rc;
   *n_exec_slots = rows * L;
   if (n_extra) *n_extra = nx;
   return GPX_OK;
@@ -1280,8 +1298,8 @@ int gpx_round_device(gpx_engine* e, const gpx_dev_round_bufs* b, void* stream) {
   if (b->n == 0) return GPX_OK;
   int rc = check_batch(e, b->n, b->payload_bytes);
   if (rc) return rc;
-  return round_on_stream(e, true, b->reqs, b->payload, b->payload_bytes, b->n, b->status, b->exec,
-                         stream ? (cudaStream_t)stream : e->stream);
+  return round_on_stream(e, RoundForm::fused, b->reqs, b->payload, b->payload_bytes, b->n, b->status, b->exec,
+                         call_stream(e, stream));
 }
 /* k_propose (ACCEPTs compacted at the front: one record, log image and EXEC row per ACCEPT, no per-request holes) +
  * k_act (accept -> tally -> commit per ACCEPT in registers): the form for batches in which most requests share a
@@ -1291,49 +1309,27 @@ int gpx_round_device_compact(gpx_engine* e, const gpx_dev_round_bufs* b, void* s
   if (b->n == 0) return GPX_OK;
   int rc = check_batch(e, b->n, b->payload_bytes);
   if (rc) return rc;
-  e->compact_fused = true;
-  rc = round_on_stream(e, false, b->reqs, b->payload, b->payload_bytes, b->n, b->status, b->exec,
-                       stream ? (cudaStream_t)stream : e->stream);
-  e->compact_fused = false;
-  return rc;
+  return round_on_stream(e, RoundForm::compact, b->reqs, b->payload, b->payload_bytes, b->n, b->status, b->exec,
+                         call_stream(e, stream));
 }
 int gpx_round_device_phases(gpx_engine* e, const gpx_dev_round_bufs* b, void* stream) {
   if (!e || !b) return fail(GPX_EINVAL, "null argument");
   if (b->n == 0) return GPX_OK;
   int rc = check_batch(e, b->n, b->payload_bytes);
   if (rc) return rc;
-  return round_on_stream(e, false, b->reqs, b->payload, b->payload_bytes, b->n, b->status, b->exec,
-                         stream ? (cudaStream_t)stream : e->stream);
+  return round_on_stream(e, RoundForm::phases, b->reqs, b->payload, b->payload_bytes, b->n, b->status, b->exec,
+                         call_stream(e, stream));
 }
 
 /* ---- device-resident phase calls (spread placement) -------------------------------------- */
 static_assert(sizeof(gpx_dev_ctl) == sizeof(RoundCtl), "gpx_dev_ctl mirrors RoundCtl");
-namespace {
-/* the launch helpers count into / append to engine-owned scratch; point them at the caller's buffers for the
- * duration of one call (the engine is single-submitter) */
-struct ScratchSwap {
-  gpx_engine* e;
-  RoundCtl* ctl0;
-  gpx_accept_rec* acc0;
-  gpx_exec_rec* ex0;
-  uint32_t cap0;
-  ScratchSwap(gpx_engine* e_, gpx_dev_ctl* ctl, gpx_accept_rec* acc, gpx_exec_rec* extra, uint32_t extra_cap)
-      : e(e_), ctl0(e_->d_ctl), acc0(e_->d_accepts), ex0(e_->d_extra), cap0(e_->extra_cap) {
-    if (ctl) e->d_ctl = reinterpret_cast<RoundCtl*>(ctl);
-    if (acc) e->d_accepts = acc;
-    if (extra) {
-      e->d_extra = extra;
-      e->extra_cap = extra_cap;
-    }
-  }
-  ~ScratchSwap() {
-    e->d_ctl = ctl0;
-    e->d_accepts = acc0;
-    e->d_extra = ex0;
-    e->extra_cap = cap0;
-  }
-};
-}  // namespace
+/* the outputs of a call on the caller's buffers: its control block, and its ACCEPT records and extra-EXEC queue where
+ * it passes them (null: the engine's) */
+static PhaseOut caller_out(const gpx_engine* e, gpx_dev_ctl* ctl, gpx_accept_rec* accepts, gpx_exec_rec* extra,
+                           uint32_t extra_cap) {
+  return {reinterpret_cast<RoundCtl*>(ctl), accepts ? accepts : e->d_accepts, extra ? extra : e->d_extra,
+          extra ? extra_cap : e->extra_cap};
+}
 
 int gpx_propose_device(gpx_engine* e, const gpx_request_rec* reqs, const uint8_t* payload, uint64_t payload_bytes,
                        uint32_t n, int32_t* status, gpx_accept_rec* out_accepts, gpx_dev_ctl* ctl, void* stream) {
@@ -1342,9 +1338,8 @@ int gpx_propose_device(gpx_engine* e, const gpx_request_rec* reqs, const uint8_t
   if (!reqs || !status || !out_accepts || (!payload && payload_bytes)) return fail(GPX_EINVAL, "null argument");
   int rc = check_batch(e, n, payload_bytes);
   if (rc) return rc;
-  ScratchSwap sw(e, ctl, out_accepts, nullptr, 0);
-  return launch_propose(e, reqs, payload, (payload_bytes + 15) & ~15ull, n, status,
-                        stream ? (cudaStream_t)stream : e->stream);
+  return launch_propose(e, caller_out(e, ctl, out_accepts, nullptr, 0), reqs, payload, (payload_bytes + 15) & ~15ull, n,
+                        status, call_stream(e, stream));
 }
 int gpx_propose_device_heads(gpx_engine* e, const gpx_request_rec* reqs, const uint8_t* payload, uint64_t payload_bytes,
                              uint32_t n, int32_t* status, gpx_accept_rec* out_accepts, uint32_t* out_head,
@@ -1354,9 +1349,8 @@ int gpx_propose_device_heads(gpx_engine* e, const gpx_request_rec* reqs, const u
   if (!reqs || !status || !out_accepts || !out_head || (!payload && payload_bytes)) return fail(GPX_EINVAL, "null argument");
   int rc = check_batch(e, n, payload_bytes);
   if (rc) return rc;
-  ScratchSwap sw(e, ctl, out_accepts, nullptr, 0);
-  return launch_propose(e, reqs, payload, (payload_bytes + 15) & ~15ull, n, status,
-                        stream ? (cudaStream_t)stream : e->stream, out_head);
+  return launch_propose(e, caller_out(e, ctl, out_accepts, nullptr, 0), reqs, payload, (payload_bytes + 15) & ~15ull, n,
+                        status, call_stream(e, stream), out_head);
 }
 
 int gpx_route_device(gpx_engine* e, uint32_t kind, const void* recs, const uint32_t* n_ptr, uint32_t n_max,
@@ -1386,7 +1380,7 @@ int gpx_route_device(gpx_engine* e, uint32_t kind, const void* recs, const uint3
   A.blob_cap = blob_cap;
   A.out_blob_units = out_blob_units;
   A.dropped = dropped;
-  k_route<<<cdiv(n_max, GPX_BLOCK), GPX_BLOCK, 0, stream ? (cudaStream_t)stream : e->stream>>>(e->S, A);
+  k_route<<<cdiv(n_max, GPX_BLOCK), GPX_BLOCK, 0, call_stream(e, stream)>>>(e->S, A);
   CK(cudaGetLastError());
   return GPX_OK;
 }
@@ -1403,7 +1397,7 @@ int gpx_accepts_device(gpx_engine* e, gpx_accept_rec* recs, uint32_t n, const ui
   if (n > e->cfg.max_batch_recs) return fail(GPX_ERANGE, "n > max_batch_recs");
   int rc = ring_fits(e, acc_bound(n, blob_bytes));
   if (rc) return rc;
-  cudaStream_t st = stream ? (cudaStream_t)stream : e->stream;
+  cudaStream_t st = call_stream(e, stream);
   {
     IngestArgs R;
     memset(&R, 0, sizeof R);
@@ -1417,9 +1411,8 @@ int gpx_accepts_device(gpx_engine* e, gpx_accept_rec* recs, uint32_t n, const ui
     }
     k_ingest<<<cdiv(n, GPX_BLOCK), GPX_BLOCK, 0, st>>>(e->S, R);
   }
-  ScratchSwap sw(e, ctl, nullptr, out_extra, out_extra ? extra_cap : 0);
-  return launch_accept(e, false, recs, nullptr, n, blob, blob_bytes, nullptr, 0, nullptr, out_replies, nullptr, nullptr,
-                       st);
+  return launch_accept(e, caller_out(e, ctl, nullptr, out_extra, extra_cap), false, recs, nullptr, n, blob, blob_bytes,
+                       nullptr, 0, nullptr, out_replies, nullptr, nullptr, st);
 }
 
 int gpx_replies_device(gpx_engine* e, const gpx_accept_reply_rec* replies, uint32_t n,
@@ -1427,8 +1420,8 @@ int gpx_replies_device(gpx_engine* e, const gpx_accept_reply_rec* replies, uint3
   if (!e || !ctl) return fail(GPX_EINVAL, "null argument");
   if (n == 0) return GPX_OK;
   if (!replies || !out_decisions) return fail(GPX_EINVAL, "null argument");
-  ScratchSwap sw(e, ctl, nullptr, nullptr, 0);
-  return launch_tally(e, replies, nullptr, 1, n, out_decisions, stream ? (cudaStream_t)stream : e->stream);
+  return launch_tally(e, caller_out(e, ctl, nullptr, nullptr, 0), replies, nullptr, 1, n, out_decisions,
+                      call_stream(e, stream));
 }
 
 int gpx_decisions_device(gpx_engine* e, gpx_decision_rec* decisions, uint32_t n, gpx_exec_rec* out_exec,
@@ -1439,7 +1432,7 @@ int gpx_decisions_device(gpx_engine* e, gpx_decision_rec* decisions, uint32_t n,
   if (n > e->cfg.max_batch_recs) return fail(GPX_ERANGE, "n > max_batch_recs");
   int rc = ring_fits(e, GPX_SEG_DEC_BYTES(n));
   if (rc) return rc;
-  cudaStream_t st = stream ? (cudaStream_t)stream : e->stream;
+  cudaStream_t st = call_stream(e, stream);
   {
     IngestArgs R;
     memset(&R, 0, sizeof R);
@@ -1448,8 +1441,7 @@ int gpx_decisions_device(gpx_engine* e, gpx_decision_rec* decisions, uint32_t n,
     R.n = n;
     k_ingest<<<cdiv(n, GPX_BLOCK), GPX_BLOCK, 0, st>>>(e->S, R);
   }
-  ScratchSwap sw(e, ctl, nullptr, out_extra, out_extra ? extra_cap : 0);
-  return launch_commit(e, decisions, nullptr, n, out_exec, st);
+  return launch_commit(e, caller_out(e, ctl, nullptr, out_extra, extra_cap), decisions, nullptr, n, out_exec, st);
 }
 
 /* ---- pipelined rounds ---------------------------------------------------------------- */
@@ -1518,14 +1510,15 @@ int gpx_round_submit(gpx_engine* e, const gpx_round_io* io, uint64_t* ticket) {
     k_unpack_expand<<<nb, GPX_BLOCK, 0, e->stream>>>(e->S, ps.d_packed, n, ps.d_bsum, ps.d_reqs);
     CK(cudaGetLastError());
   }
-  rc = launch_round(e, ps.d_reqs, ps.d_payload, pal, n, ps.d_status, ps.d_exec, e->stream, ps.d_ctl, ps.d_extra,
-                    (uint32_t)std::min<uint64_t>((uint64_t)e->cfg.max_batch_recs * (L + 1), 0xffffffffull),
+  PhaseOut o{ps.d_ctl, e->d_accepts, ps.d_extra,
+             (uint32_t)std::min<uint64_t>((uint64_t)e->cfg.max_batch_recs * (L + 1), 0xffffffffull)};
+  rc = launch_round(e, o, ps.d_reqs, ps.d_payload, pal, n, ps.d_status, ps.d_exec, e->stream,
                     compact ? ps.d_sum : nullptr);
   if (rc) return rc;
   CK(cudaEventRecord(ps.ev_k, e->stream));
   /* stream 3: results */
   CK(cudaStreamWaitEvent(e->s_d2h, ps.ev_k, 0));
-  CK(cudaMemcpyAsync(ps.h_ctl, e->last_ctl, sizeof(RoundCtl), cudaMemcpyDeviceToHost, e->s_d2h));
+  CK(cudaMemcpyAsync(ps.h_ctl, ps.d_ctl, sizeof(RoundCtl), cudaMemcpyDeviceToHost, e->s_d2h));
   if (compact) {
     CK(cudaMemcpyAsync(io->sum, ps.d_sum, n * sizeof(gpx_exec_sum), cudaMemcpyDeviceToHost, e->s_d2h));
   } else {
@@ -1731,7 +1724,7 @@ int gpx_log_drain_async(gpx_engine* e, uint32_t lane, void* dst, uint64_t cap, u
   *from = f;
   *n_bytes = nb;
   if (!nb) return GPX_OK;
-  CK(cudaEventRecord(e->ev_drain, after_stream ? (cudaStream_t)after_stream : e->stream));
+  CK(cudaEventRecord(e->ev_drain, call_stream(e, after_stream)));
   CK(cudaStreamWaitEvent(e->s_drain, e->ev_drain, 0));
   const uint64_t pos = f & (rc_ - 1), first = std::min<uint64_t>(nb, rc_ - pos);
   CK(cudaMemcpyAsync(dst, e->S.ring[lane] + pos, first, cudaMemcpyDeviceToHost, e->s_drain));
