@@ -49,6 +49,7 @@ static int fail(int code, const std::string& msg) {
 static inline uint32_t cdiv(uint64_t a, uint32_t b) { return (uint32_t)((a + b - 1) / b); }
 
 #include "gpx_wire_seq.h"
+#include "gpx_state_seq.h"
 
 struct gpx_engine {
   gpx_config cfg;
@@ -1083,45 +1084,6 @@ int gpx_handle_prepares(gpx_engine* e, uint32_t n, const gpx_pvalue_hdr* prepare
   return GPX_OK;
 }
 
-/* phase 1b for a batch of elections: one launch of k_prepare_tally (gpx_phase1b.cuh) */
-int gpx_handle_prepare_replies(gpx_engine* e, uint32_t n, const gpx_election_rec* elections, uint32_t n_reply_recs,
-                               const gpx_prepare_reply_rec* replies, gpx_election_out* out) {
-  if (!e) return fail(GPX_EINVAL, "null argument");
-  if (n == 0) return GPX_OK;
-  if (!elections || !out || (!replies && n_reply_recs)) return fail(GPX_EINVAL, "null argument");
-  {
-    std::vector<uint32_t> gids(n);
-    for (uint32_t i = 0; i < n; i++) {
-      if ((uint64_t)elections[i].first_reply + elections[i].n_replies > n_reply_recs)
-        return fail(GPX_ERANGE, "election refers to replies beyond n_reply_recs");
-      gids[i] = elections[i].gid;
-    }
-    std::sort(gids.begin(), gids.end());
-    if (std::adjacent_find(gids.begin(), gids.end()) != gids.end())
-      return fail(GPX_EINVAL, "more than one election for a group in one call");
-  }
-  const size_t el_bytes = (size_t)n * sizeof(gpx_election_rec);
-  const size_t rep_bytes = (size_t)n_reply_recs * sizeof(gpx_prepare_reply_rec);
-  const size_t out_bytes = (size_t)n * sizeof(gpx_election_out);
-  int rc = e->ensure_misc(el_bytes + rep_bytes + out_bytes);
-  if (rc) return rc;
-  cudaStream_t st = e->stream;
-  uint8_t* base = (uint8_t*)e->d_misc;
-  CK(cudaMemcpyAsync(base, elections, el_bytes, cudaMemcpyHostToDevice, st));
-  if (rep_bytes) CK(cudaMemcpyAsync(base + el_bytes, replies, rep_bytes, cudaMemcpyHostToDevice, st));
-  Phase1bArgs A;
-  A.els = (const gpx_election_rec*)base;
-  A.n = n;
-  A.replies = (const gpx_prepare_reply_rec*)(base + el_bytes);
-  A.out = (gpx_election_out*)(base + el_bytes + rep_bytes);
-  ls_settle(e, st);
-  k_prepare_tally<<<cdiv(n, GPX_P1B_BLOCK), GPX_P1B_BLOCK, 0, st>>>(e->S, A);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out, A.out, out_bytes, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return GPX_OK;
-}
-
 /* handleAccept + loopback tally + commit per ACCEPT (k_act), host buffers */
 int gpx_handle_accepts_fused(gpx_engine* e, uint32_t n, const gpx_accept_rec* accepts, const uint8_t* blob,
                              uint64_t blob_bytes, gpx_accept_reply_rec* out_replies, gpx_decision_rec* out_decisions,
@@ -1605,105 +1567,6 @@ int gpx_log_read(gpx_engine* e, uint32_t lane, uint64_t from, void* dst, uint64_
   return GPX_OK;
 }
 
-/* the journal's index as a scan: k_log_dir -> k_log_scan -> k_log_hits (gpx_logfind.cuh) */
-int gpx_log_find(gpx_engine* e, uint32_t lane, uint64_t from, uint32_t n, const gpx_log_want* wants, gpx_log_hit* out) {
-  if (!e) return fail(GPX_EINVAL, "null argument");
-  if (lane >= e->cfg.n_lanes) return fail(GPX_ERANGE, "lane");
-  if (n == 0) return GPX_OK;
-  if (!wants || !out) return fail(GPX_EINVAL, "null argument");
-  if (from & 31) return fail(GPX_EINVAL, "from is not a segment boundary");
-  for (uint32_t i = 0; i < n; i++) {
-    if (wants[i].n_slots > GPX_LOG_SPAN) return fail(GPX_ERANGE, "n_slots > GPX_LOG_SPAN");
-    if (i && wants[i - 1].gid >= wants[i].gid) return fail(GPX_EINVAL, "wants must be sorted by gid, one per group");
-  }
-  CK(cudaDeviceSynchronize()); /* rounds may have been issued on a caller's stream; the head is read on the device */
-  const size_t cells = (size_t)n * GPX_LOG_SPAN;
-  /* a segment is at least GPX_SEG_DEC_BYTES(1) = 96 bytes; a directory of 2^20 entries (32 MiB) covers every ring the
-   * launches of this engine can fill with fewer segments than that, else LOGF_TOO_MANY */
-  const uint64_t seg_cap64 = std::min<uint64_t>(e->cfg.log_ring_bytes / GPX_SEG_DEC_BYTES(1) + 2, 1ull << 20);
-  const size_t want_bytes = ((size_t)n * sizeof(gpx_log_want) + 31) & ~(size_t)31;
-  const size_t seg_bytes = (size_t)seg_cap64 * sizeof(LogSeg);
-  const size_t best_bytes = 2 * cells * 8;
-  const size_t hit_bytes = cells * sizeof(gpx_log_hit);
-  int rc = e->ensure_misc(want_bytes + seg_bytes + 32 + best_bytes + hit_bytes);
-  if (rc) return rc;
-  cudaStream_t st = e->stream;
-  uint8_t* base = (uint8_t*)e->d_misc;
-  LogFindArgs A;
-  A.lane = lane;
-  A.n = n;
-  A.from = from;
-  A.wants = (const gpx_log_want*)base;
-  A.segs = (LogSeg*)(base + want_bytes);
-  A.seg_cap = (uint32_t)seg_cap64;
-  A.ctl = (unsigned long long*)(base + want_bytes + seg_bytes);
-  A.best = A.ctl + 4;
-  A.hits = (gpx_log_hit*)(base + want_bytes + seg_bytes + 32 + best_bytes);
-  CK(cudaMemcpyAsync(base, wants, (size_t)n * sizeof(gpx_log_want), cudaMemcpyHostToDevice, st));
-  CK(cudaMemsetAsync(A.ctl, 0, 32 + best_bytes, st));
-  k_log_dir<<<1, 32, 0, st>>>(e->S, A);
-  int sms = e->n_sms;
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->cfg.device);
-  k_log_scan<<<(unsigned)sms * 8u, GPX_LOGF_BLOCK, 0, st>>>(e->S, A);
-  k_log_hits<<<cdiv(cells, GPX_LOGF_BLOCK), GPX_LOGF_BLOCK, 0, st>>>(e->S, A);
-  CK(cudaGetLastError());
-  unsigned long long ctl[4];
-  CK(cudaMemcpyAsync(ctl, A.ctl, sizeof ctl, cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(out, A.hits, hit_bytes, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  if (ctl[LOGF_ERR] == LOGF_OVERWRITTEN) return fail(GPX_ERANGE, "bytes from `from` on were already overwritten");
-  if (ctl[LOGF_ERR] == LOGF_CORRUPT) return fail(GPX_EINVAL, "`from` is not a segment boundary");
-  if (ctl[LOGF_ERR] == LOGF_TOO_MANY) return fail(GPX_ERANGE, "more log segments than the scan's directory holds");
-  return GPX_OK;
-}
-
-/* the bodies of a batch of hits in one copy: k_log_gather (gpx_logfind.cuh) packs them into a staging buffer */
-int gpx_log_gather(gpx_engine* e, uint32_t lane, uint32_t n, const gpx_log_range* ranges, void* dst, uint64_t dst_bytes) {
-  if (!e) return fail(GPX_EINVAL, "null argument");
-  if (lane >= e->cfg.n_lanes) return fail(GPX_ERANGE, "lane");
-  if (n == 0) return GPX_OK;
-  if (!ranges || !dst) return fail(GPX_EINVAL, "null argument");
-  CK(cudaDeviceSynchronize());
-  unsigned long long lp[2 * GPX_MAX_LANES];
-  CK(cudaMemcpy(lp, e->S.log_pos + (size_t)e->S.lp * 2 * GPX_MAX_LANES, sizeof lp, cudaMemcpyDeviceToHost));
-  const uint64_t head = lp[2 * lane], cap = e->S.ring_cap;
-  std::vector<uint32_t> first(n + 1);
-  uint64_t chunks = 0, top = 0;
-  for (uint32_t i = 0; i < n; i++) {
-    const uint64_t nc = ((uint64_t)ranges[i].len + 15) >> 4;
-    if ((ranges[i].pos & 15) || (ranges[i].dst_off & 15)) return fail(GPX_EINVAL, "range not on a 16-byte boundary");
-    if (ranges[i].pos + 16 * nc > head || head - ranges[i].pos > cap) return fail(GPX_ERANGE, "range outside the live ring bytes");
-    if ((ranges[i].pos & (cap - 1)) + 16 * nc > cap) return fail(GPX_ERANGE, "range straddles the ring end");
-    if ((uint64_t)ranges[i].dst_off + 16 * nc > dst_bytes) return fail(GPX_ERANGE, "range beyond dst");
-    first[i] = (uint32_t)chunks;
-    chunks += nc;
-    top = std::max<uint64_t>(top, (uint64_t)ranges[i].dst_off + 16 * nc);
-    if (chunks > 0xffffffffull) return fail(GPX_ERANGE, "too many bytes for one gather");
-  }
-  first[n] = (uint32_t)chunks;
-  if (chunks == 0) return GPX_OK;
-  const size_t r_bytes = ((size_t)n * sizeof(gpx_log_range) + 15) & ~(size_t)15;
-  const size_t f_bytes = ((size_t)(n + 1) * 4 + 15) & ~(size_t)15;
-  int rc = e->ensure_misc(r_bytes + f_bytes + top);
-  if (rc) return rc;
-  cudaStream_t st = e->stream;
-  uint8_t* base = (uint8_t*)e->d_misc;
-  CK(cudaMemcpyAsync(base, ranges, (size_t)n * sizeof(gpx_log_range), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(base + r_bytes, first.data(), (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, st));
-  LogGatherArgs A;
-  A.lane = lane;
-  A.n = n;
-  A.ranges = (const gpx_log_range*)base;
-  A.first_chunk = (const uint32_t*)(base + r_bytes);
-  A.out = (int4*)(base + r_bytes + f_bytes);
-  CK(cudaMemsetAsync(A.out, 0, top, st)); /* gaps between ranges read as zero */
-  k_log_gather<<<cdiv(chunks, GPX_LOGF_BLOCK), GPX_LOGF_BLOCK, 0, st>>>(e->S, A);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(dst, A.out, top, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return GPX_OK;
-}
-
 /* Asynchronous drain (SQLPaxosLogger.journal :965-1036 appends the batch to the journal file; here the caller's
  * page-locked buffer stands for the file's write buffer).  Everything is enqueued: the copy runs on the engine's
  * drain stream behind the work already enqueued on `after_stream` (NULL = the engine's stream) and overlaps later
@@ -1807,127 +1670,93 @@ int gpx_get_group_flags(gpx_engine* e, uint32_t lane, uint32_t n, const uint32_t
   return GPX_OK;
 }
 
+#include "gpx_spread_host.inc"
+#include "gpx_wire_host.inc"
+#include "gpx_respcache_host.inc"
+
+/* ---- group-state and log-index calls: the engine's duties around the sequences of gpx_state_seq.h ------------------- */
+/* the CUDA executor of gpx_state_seq.h: gpx_wire_seq.h's on the engine's stream, the lockstep settle, and the
+ * group-management scratch (*buf is e->d_misc) */
+extern "C++" {
+struct StateCuda : WireCuda {
+  gpx_engine* e;
+  int settle() {
+    ls_settle(e, st);
+    return GPX_OK;
+  }
+  int grow(void**, size_t*, size_t bytes, size_t) { return e->ensure_misc(bytes); }
+};
+}
+static StateCuda state_cuda(gpx_engine* e) { return StateCuda{{e->stream}, e}; }
+static StateEnv state_env(gpx_engine* e) { return StateEnv{e->S, &e->d_misc, &e->misc_bytes}; }
+
+/* the log readers run once the rounds issued on any stream (gpx_round_device) are done */
+struct LogFindCall {
+  int begin() {
+    CK(cudaDeviceSynchronize());
+    return GPX_OK;
+  }
+};
+struct LogGatherCall {
+  const gpx_engine* e;
+  uint32_t lane;
+  uint64_t head = 0;
+  int begin() {
+    CK(cudaDeviceSynchronize());
+    unsigned long long lp[2 * GPX_MAX_LANES];
+    CK(cudaMemcpy(lp, e->S.log_pos + (size_t)e->S.lp * 2 * GPX_MAX_LANES, sizeof lp, cudaMemcpyDeviceToHost));
+    head = lp[2 * lane];
+    return GPX_OK;
+  }
+};
+
+/* the journal's index as a scan: k_log_dir -> k_log_scan -> k_log_hits (gpx_logfind.cuh) */
+int gpx_log_find(gpx_engine* e, uint32_t lane, uint64_t from, uint32_t n, const gpx_log_want* wants, gpx_log_hit* out) {
+  if (!e) return fail(GPX_EINVAL, "null argument");
+  int sms = e->n_sms;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, e->cfg.device);
+  StateCuda ex = state_cuda(e);
+  LogFindCall call;
+  return log_find(ex, call, state_env(e), lane, from, n, wants, out, (uint32_t)sms * 8u * GPX_LOGF_BLOCK);
+}
+
+/* the bodies of a batch of hits in one copy: k_log_gather (gpx_logfind.cuh) packs them into a staging buffer */
+int gpx_log_gather(gpx_engine* e, uint32_t lane, uint32_t n, const gpx_log_range* ranges, void* dst, uint64_t dst_bytes) {
+  if (!e) return fail(GPX_EINVAL, "null argument");
+  StateCuda ex = state_cuda(e);
+  LogGatherCall call{e, lane};
+  return log_gather(ex, call, state_env(e), lane, n, ranges, dst, dst_bytes);
+}
+
 /* the slow-path list / the candidates of a sweep: one launch of k_select_groups over all gids (gpx_pause.cuh) */
 int gpx_select_groups(gpx_engine* e, uint32_t lane, uint32_t mask, uint32_t value, uint32_t* out_gids, uint32_t cap,
                       uint32_t* n_found) {
-  if (!e || !n_found || (!out_gids && cap)) return fail(GPX_EINVAL, "null argument");
-  if (lane >= e->cfg.n_lanes) return fail(GPX_ERANGE, "lane");
-  int rc = e->ensure_misc(16 + (size_t)cap * 4);
-  if (rc) return rc;
-  cudaStream_t st = e->stream;
-  uint8_t* base = (uint8_t*)e->d_misc;
-  SelectArgs A;
-  A.lane = lane;
-  A.mask = mask;
-  A.value = value;
-  A.cap = cap;
-  A.n_found = (unsigned long long*)base;
-  A.gids = (uint32_t*)(base + 16);
-  CK(cudaMemsetAsync(base, 0, 16, st));
-  ls_settle(e, st);
-  k_select_groups<<<cdiv(e->cfg.max_groups, GPX_PAUSE_BLOCK), GPX_PAUSE_BLOCK, 0, st>>>(e->S, A);
-  CK(cudaGetLastError());
-  unsigned long long found = 0;
-  CK(cudaMemcpyAsync(&found, A.n_found, 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  const uint32_t got = (uint32_t)std::min<unsigned long long>(found, cap);
-  if (got) {
-    CK(cudaMemcpyAsync(out_gids, A.gids, (size_t)got * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    std::sort(out_gids, out_gids + got);
-  }
-  *n_found = (uint32_t)std::min<unsigned long long>(found, 0xffffffffull);
-  return GPX_OK;
+  if (!e) return fail(GPX_EINVAL, "null argument");
+  StateCuda ex = state_cuda(e);
+  return select_groups(ex, state_env(e), lane, mask, value, out_gids, cap, n_found);
 }
 
 /* the fields of a SYNC_DECISIONS_REQUEST for a batch of groups: one launch of k_missing_decisions (gpx_pause.cuh) */
 int gpx_missing_decisions(gpx_engine* e, uint32_t lane, uint32_t n, const uint32_t* gids, int32_t size_limit,
                           int32_t too_much_gap, gpx_missing_rec* out) {
-  if (!e || ((!gids || !out) && n)) return fail(GPX_EINVAL, "null argument");
-  if (lane >= e->cfg.n_lanes) return fail(GPX_ERANGE, "lane");
-  if (n == 0) return GPX_OK;
-  const size_t gid_bytes = ((size_t)n * 4 + 15) & ~(size_t)15;
-  int rc = e->ensure_misc(gid_bytes + (size_t)n * sizeof(gpx_missing_rec));
-  if (rc) return rc;
-  cudaStream_t st = e->stream;
-  uint8_t* base = (uint8_t*)e->d_misc;
-  CK(cudaMemcpyAsync(base, gids, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  MissingArgs A;
-  A.lane = lane;
-  A.n = n;
-  A.gids = (const uint32_t*)base;
-  A.size_limit = size_limit;
-  A.too_much_gap = too_much_gap;
-  A.out = (gpx_missing_rec*)(base + gid_bytes);
-  ls_settle(e, st);
-  k_missing_decisions<<<cdiv(n, GPX_PAUSE_BLOCK), GPX_PAUSE_BLOCK, 0, st>>>(e->S, A);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out, A.out, (size_t)n * sizeof(gpx_missing_rec), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return GPX_OK;
+  if (!e) return fail(GPX_EINVAL, "null argument");
+  StateCuda ex = state_cuda(e);
+  return missing_decisions(ex, state_env(e), lane, n, gids, size_limit, too_much_gap, out);
 }
 
 int gpx_clear_group_flags(gpx_engine* e, uint32_t lane, uint32_t n, const uint32_t* gids, uint32_t mask) {
-  if (!e || (!gids && n)) return fail(GPX_EINVAL, "null argument");
-  if (lane >= e->cfg.n_lanes) return fail(GPX_ERANGE, "lane");
-  if (n == 0) return GPX_OK;
-  { /* two threads must not read-modify-write the same word */
-    std::vector<uint32_t> g(gids, gids + n);
-    std::sort(g.begin(), g.end());
-    if (std::adjacent_find(g.begin(), g.end()) != g.end()) return fail(GPX_EINVAL, "a gid appears twice in the batch");
-  }
-  int rc = e->ensure_misc((size_t)n * 4);
-  if (rc) return rc;
-  CK(cudaMemcpyAsync(e->d_misc, gids, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
-  ls_settle(e, e->stream);
-  k_clear_flags<<<cdiv(n, 128), 128, 0, e->stream>>>(e->S, lane, (const uint32_t*)e->d_misc, n, mask);
-  CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(e->stream));
-  return GPX_OK;
+  if (!e) return fail(GPX_EINVAL, "null argument");
+  StateCuda ex = state_cuda(e);
+  return clear_group_flags(ex, state_env(e), lane, n, gids, mask);
 }
 
 /* the deactivation sweep: one launch of k_pause_groups (gpx_pause.cuh) */
 int gpx_pause_groups(gpx_engine* e, uint32_t n, const uint32_t* gids, gpx_row* out_rows, uint8_t* out_paused) {
   if (!e) return fail(GPX_EINVAL, "null argument");
-  if (n == 0) return GPX_OK;
-  if (!gids || !out_rows || !out_paused) return fail(GPX_EINVAL, "null argument");
-  {
-    std::vector<uint32_t> g(gids, gids + n);
-    std::sort(g.begin(), g.end());
-    if (std::adjacent_find(g.begin(), g.end()) != g.end()) return fail(GPX_EINVAL, "a gid appears twice in the batch");
-  }
-  const uint32_t L = e->cfg.n_lanes;
-  const size_t gid_bytes = ((size_t)n * 4 + 15) & ~(size_t)15;
-  const size_t row_bytes = (size_t)n * L * sizeof(gpx_row);
-  const size_t flag_off = gid_bytes + ((row_bytes + 15) & ~(size_t)15);
-  int rc = e->ensure_misc(flag_off + n);
+  StateCuda ex = state_cuda(e);
+  int rc = pause_groups(ex, state_env(e), n, gids, out_rows, out_paused);
   if (rc) return rc;
-  cudaStream_t st = e->stream;
-  uint8_t* base = (uint8_t*)e->d_misc;
-  CK(cudaMemcpyAsync(base, gids, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  PauseArgs A;
-  A.gids = (const uint32_t*)base;
-  A.n = n;
-  A.rows = (gpx_row*)(base + gid_bytes);
-  A.paused = base + flag_off;
-  ls_settle(e, st);
-  k_pause_groups<<<cdiv(n, GPX_PAUSE_BLOCK), GPX_PAUSE_BLOCK, 0, st>>>(e->S, A);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out_paused, A.paused, n, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  /* only the rows of the paused groups were written: copy those (runs of consecutive paused entries) */
-  for (uint32_t i = 0; i < n;) {
-    if (!out_paused[i]) {
-      i++;
-      continue;
-    }
-    uint32_t j = i;
-    while (j < n && out_paused[j]) j++;
-    CK(cudaMemcpyAsync(out_rows + (size_t)i * L, A.rows + (size_t)i * L, (size_t)(j - i) * L * sizeof(gpx_row),
-                       cudaMemcpyDeviceToHost, st));
-    i = j;
-  }
-  CK(cudaStreamSynchronize(st));
+  const uint32_t L = e->cfg.n_lanes;
   for (uint32_t i = 0; i < n; i++) { /* version and paxosID hash live on the host (as in gpx_dump_rows / _destroy_groups) */
     if (!out_paused[i] || gids[i] >= e->cfg.max_groups) continue;
     for (uint32_t l = 0; l < L; l++) {
@@ -1939,8 +1768,12 @@ int gpx_pause_groups(gpx_engine* e, uint32_t n, const uint32_t* gids, gpx_row* o
   return names_drop(e, n, gids, out_paused);
 }
 
-#include "gpx_spread_host.inc"
-#include "gpx_wire_host.inc"
-#include "gpx_respcache_host.inc"
+/* phase 1b for a batch of elections: one launch of k_prepare_tally (gpx_phase1b.cuh) */
+int gpx_handle_prepare_replies(gpx_engine* e, uint32_t n, const gpx_election_rec* elections, uint32_t n_reply_recs,
+                               const gpx_prepare_reply_rec* replies, gpx_election_out* out) {
+  if (!e) return fail(GPX_EINVAL, "null argument");
+  StateCuda ex = state_cuda(e);
+  return prepare_replies(ex, state_env(e), n, elections, n_reply_recs, replies, out);
+}
 
 } /* extern "C" */

@@ -1,64 +1,33 @@
 /*
- * logfind_emu.cpp -- k_log_dir / k_log_scan / k_log_hits (gigapaxos_b200/csrc/gpx_logfind.cuh, the source the GPU runs)
- * compiled for the host over cuda_emu.h; see p1b_emu.cpp.  The caller hands in one lane's ring as the device holds it
+ * logfind_emu.cpp -- k_log_dir / k_log_scan / k_log_hits and k_log_gather (gigapaxos_b200/csrc/gpx_logfind.cuh, the
+ * source the GPU runs) compiled for the host over cuda_emu.h, driven by the product's own host sequences (log_find and
+ * log_gather in gpx_state_seq.h) on the CPU executor.  The caller hands in one lane's ring as the device holds it
  * (ring_cap bytes, positions taken modulo ring_cap) and the head.  Test infrastructure only.
  */
-#include "cuda_emu.h"
+#include "state_exec.h"
 
-#include "gpx_logfind.cuh"
+/* the head the engine reads once the rounds are done */
+struct EmuHead {
+  uint64_t head;
+  int begin() { return GPX_OK; }
+};
 
-#include <cstring>
-#include <vector>
-
+/* gpx_log_find; k_log_scan runs grid x block threads.  Returns 1 (k_log_dir's launch) or the GPX_* error. */
 extern "C" int emu_log_find(uint8_t* ring, uint64_t ring_cap, uint64_t head, uint64_t from, uint32_t lane, uint32_t n,
-                            const gpx_log_want* wants, gpx_log_hit* hits, uint32_t seg_cap, uint32_t grid, uint32_t block,
-                            uint64_t* ctl_out) {
-  if (lane >= GPX_MAX_LANES || (ring_cap & (ring_cap - 1))) return -1;
-  std::vector<unsigned long long> ctr((size_t)GPX_CTR_STRIPES * C_NCTR, 0ull);
-  std::vector<unsigned long long> log_pos((size_t)2 * GPX_MAX_LANES * 2, 0ull);
-  DevState S;
-  memset(&S, 0, sizeof S);
-  S.L = lane + 1;
-  S.ring[lane] = ring;
-  S.ring_cap = ring_cap;
-  S.lp = 1; /* the copy the next launch would read */
-  log_pos[((size_t)S.lp * GPX_MAX_LANES + lane) * 2] = head;
-  S.log_pos = log_pos.data();
-  S.ctr = ctr.data();
-  const size_t cells = (size_t)n * GPX_LOG_SPAN;
-  std::vector<LogSeg> segs(seg_cap);
-  std::vector<unsigned long long> ctl(4 + 2 * cells, 0ull);
-  LogFindArgs A;
-  A.lane = lane;
-  A.n = n;
-  A.from = from;
-  A.wants = wants;
-  A.segs = segs.data();
-  A.seg_cap = seg_cap;
-  A.ctl = ctl.data();
-  A.best = ctl.data() + 4;
-  A.hits = hits;
-  emu_launch(k_log_dir, 1, 32, S, A);
-  emu_launch(k_log_scan, grid, block, S, A);
-  emu_launch(k_log_hits, (unsigned)((cells + block - 1) / block), block, S, A);
-  for (int i = 0; i < 4; i++) ctl_out[i] = ctl[i];
-  return (int)ctr[C_KERNEL_LAUNCHES];
+                            const gpx_log_want* wants, gpx_log_hit* hits, uint32_t grid, uint32_t block) {
+  EmuWorld w(0, lane + 1, 0, 0, 0, nullptr, nullptr, nullptr, block);
+  if (!w.ok || (ring_cap & (ring_cap - 1))) return -100;
+  w.ring(lane, ring, ring_cap, head);
+  EmuCall call;
+  return w.done(log_find(w.ex, call, w.env(), lane, from, n, wants, hits, grid * block));
 }
 
-extern "C" int emu_log_gather(uint8_t* ring, uint64_t ring_cap, uint32_t lane, uint32_t n, const gpx_log_range* ranges,
-                              const uint32_t* first_chunk, uint8_t* out, uint32_t block) {
-  if (lane >= GPX_MAX_LANES || (ring_cap & (ring_cap - 1)) || block == 0) return -1;
-  DevState S;
-  memset(&S, 0, sizeof S);
-  S.L = lane + 1;
-  S.ring[lane] = ring;
-  S.ring_cap = ring_cap;
-  LogGatherArgs A;
-  A.lane = lane;
-  A.n = n;
-  A.ranges = ranges;
-  A.first_chunk = first_chunk;
-  A.out = reinterpret_cast<int4*>(out);
-  emu_launch(k_log_gather, (first_chunk[n] + block - 1) / block + 1, block, S, A);
-  return 0;
+/* gpx_log_gather into out[out_bytes]; returns 0 or the GPX_* error */
+extern "C" int emu_log_gather(uint8_t* ring, uint64_t ring_cap, uint64_t head, uint32_t lane, uint32_t n,
+                              const gpx_log_range* ranges, uint8_t* out, uint64_t out_bytes, uint32_t block) {
+  EmuWorld w(0, lane + 1, 0, 0, 0, nullptr, nullptr, nullptr, block);
+  if (!w.ok || (ring_cap & (ring_cap - 1))) return -100;
+  w.ring(lane, ring, ring_cap, head);
+  EmuHead call{head};
+  return w.done(log_gather(w.ex, call, w.env(), lane, n, ranges, out, out_bytes));
 }

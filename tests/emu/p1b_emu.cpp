@@ -1,57 +1,21 @@
 /*
  * p1b_emu.cpp -- k_prepare_tally (gigapaxos_b200/csrc/gpx_phase1b.cuh, the source the GPU runs) compiled for the host
- * over cuda_emu.h.  The caller (tests/test_phase1b.py) lays the engine's state arrays out as DevState describes them
- * ([L][G] rows, [L][W][G] windows, [L][Rcap][G] nodeSlotNumbers), this file fills the DevState / MsetInfo structs of
- * gpx_dev.cuh itself, runs the kernel thread by thread and leaves outputs and state where the kernel wrote them.
- * Test infrastructure only.
+ * over cuda_emu.h, driven by the product's own host sequence (prepare_replies in gpx_state_seq.h) on the CPU executor,
+ * in the world of state_exec.h.  Outputs and state are left where the kernel wrote them.  Test infrastructure only.
  */
-#include "cuda_emu.h"
+#include "state_exec.h"
 
-#include "gpx_phase1b.cuh"
-
-#include <cstring>
-#include <vector>
-
+/* gpx_handle_prepare_replies; returns the kernel launches the call counted, or its GPX_* error */
 extern "C" int emu_prepare_tally(uint32_t G, uint32_t L, uint32_t W, uint32_t Rcap, uint32_t R, const int32_t* members,
                                  const int32_t* lane_node, const uint8_t* live, int32_t* coord_row, uint32_t* acc_aux,
                                  int32_t* node_slots, int32_t* prop_win, uint32_t n, const gpx_election_rec* els,
-                                 const gpx_prepare_reply_rec* replies, gpx_election_out* out, uint32_t block) {
-  if (R > GPX_MAX_GROUP_SIZE || L > GPX_MAX_LANES || block == 0) return -1;
-  MsetInfo ms;
-  memset(&ms, 0, sizeof ms);
-  memset(ms.lane_of_idx, 0xff, sizeof ms.lane_of_idx);
-  memset(ms.idx_of_lane, 0xff, sizeof ms.idx_of_lane);
-  ms.R = (uint8_t)R;
-  for (uint32_t m = 0; m < R; m++) {
-    ms.nodes[m] = members[m];
-    for (uint32_t l = 0; l < L; l++)
-      if (lane_node[l] == members[m]) {
-        ms.lane_of_idx[m] = (uint8_t)l;
-        ms.idx_of_lane[l] = (uint8_t)m;
-        ms.lane_mask |= (uint16_t)(1u << l);
-      }
-  }
-  std::vector<uint32_t> meta(G);
-  for (uint32_t g = 0; g < G; g++) meta[g] = 0u | (R << 16) | (live[g] ? GPX_META_LIVE : 0u);
-  std::vector<unsigned long long> ctr((size_t)GPX_CTR_STRIPES * C_NCTR, 0ull);
-  DevState S;
-  memset(&S, 0, sizeof S);
-  S.G = G;
-  S.L = L;
-  S.W = W;
-  S.Rcap = Rcap;
-  S.acc_aux = acc_aux;
-  S.coord_row = reinterpret_cast<int4*>(coord_row);
-  S.node_slots = node_slots;
-  S.prop_win = reinterpret_cast<int4*>(prop_win);
-  S.grp_meta = meta.data();
-  S.msets = &ms;
-  S.ctr = ctr.data();
-  Phase1bArgs A;
-  A.els = els;
-  A.n = n;
-  A.replies = replies;
-  A.out = out;
-  emu_launch(k_prepare_tally, (n + block - 1) / block, block, S, A);
-  return (int)ctr[C_KERNEL_LAUNCHES];
+                                 uint32_t n_reply_recs, const gpx_prepare_reply_rec* replies, gpx_election_out* out,
+                                 uint32_t block) {
+  EmuWorld w(G, L, W, Rcap, R, members, lane_node, live, block);
+  if (!w.ok) return -100;
+  w.S.acc_aux = acc_aux;
+  w.S.coord_row = reinterpret_cast<int4*>(coord_row);
+  w.S.node_slots = node_slots;
+  w.S.prop_win = reinterpret_cast<int4*>(prop_win);
+  return w.done(prepare_replies(w.ex, w.env(), n, els, n_reply_recs, replies, out));
 }

@@ -1,105 +1,40 @@
 /*
- * pause_emu.cpp -- k_pause_groups (gigapaxos_b200/csrc/gpx_pause.cuh, the source the GPU runs) compiled for the host
- * over cuda_emu.h; see p1b_emu.cpp.  Test infrastructure only.
+ * pause_emu.cpp -- k_pause_groups, k_select_groups, k_missing_decisions and k_clear_flags (gigapaxos_b200/csrc/
+ * gpx_pause.cuh, the source the GPU runs) compiled for the host over cuda_emu.h, driven by the product's own host
+ * sequences (gpx_state_seq.h) on the CPU executor, in the world of state_exec.h.  Each returns the kernel launches the
+ * call counted, or its GPX_* error.  Test infrastructure only.
  */
-#include "cuda_emu.h"
+#include "state_exec.h"
 
-#include "gpx_pause.cuh"
+static void planes(EmuWorld& w, int journaling, int32_t* acc_row, uint32_t* acc_aux, int32_t* acc_win,
+                   int32_t* coord_row, int32_t* node_slots) {
+  w.S.journaling = journaling;
+  w.S.acc_row = reinterpret_cast<int4*>(acc_row);
+  w.S.acc_aux = acc_aux;
+  w.S.acc_win = reinterpret_cast<int4*>(acc_win);
+  w.S.coord_row = reinterpret_cast<int4*>(coord_row);
+  w.S.node_slots = node_slots;
+}
 
-#include <cstring>
-#include <vector>
-
+/* gpx_pause_groups up to the rows' version and name hash, which the engine keeps on the host */
 extern "C" int emu_pause_groups(uint32_t G, uint32_t L, uint32_t W, uint32_t Rcap, uint32_t R, const int32_t* members,
                                 const int32_t* lane_node, const uint8_t* live, int journaling, int32_t* acc_row,
                                 uint32_t* acc_aux, int32_t* acc_win, int32_t* coord_row, int32_t* node_slots, uint32_t n,
                                 const uint32_t* gids, gpx_row* rows, uint8_t* paused, uint32_t block) {
-  if (R > GPX_MAX_GROUP_SIZE || L > GPX_MAX_LANES || block == 0) return -1;
-  MsetInfo ms;
-  memset(&ms, 0, sizeof ms);
-  memset(ms.lane_of_idx, 0xff, sizeof ms.lane_of_idx);
-  memset(ms.idx_of_lane, 0xff, sizeof ms.idx_of_lane);
-  ms.R = (uint8_t)R;
-  for (uint32_t m = 0; m < R; m++) {
-    ms.nodes[m] = members[m];
-    for (uint32_t l = 0; l < L; l++)
-      if (lane_node[l] == members[m]) {
-        ms.lane_of_idx[m] = (uint8_t)l;
-        ms.idx_of_lane[l] = (uint8_t)m;
-        ms.lane_mask |= (uint16_t)(1u << l);
-      }
-  }
-  std::vector<uint32_t> meta(G);
-  for (uint32_t g = 0; g < G; g++) meta[g] = live[g] ? (0u | (R << 16) | GPX_META_LIVE) : 0u;
-  std::vector<unsigned long long> ctr((size_t)GPX_CTR_STRIPES * C_NCTR, 0ull);
-  DevState S;
-  memset(&S, 0, sizeof S);
-  S.G = G;
-  S.L = L;
-  S.W = W;
-  S.Rcap = Rcap;
-  S.journaling = journaling;
-  S.acc_row = reinterpret_cast<int4*>(acc_row);
-  S.acc_aux = acc_aux;
-  S.acc_win = reinterpret_cast<int4*>(acc_win);
-  S.coord_row = reinterpret_cast<int4*>(coord_row);
-  S.node_slots = node_slots;
-  S.grp_meta = meta.data();
-  S.msets = &ms;
-  S.ctr = ctr.data();
-  PauseArgs A;
-  A.gids = gids;
-  A.n = n;
-  A.rows = rows;
-  A.paused = paused;
-  emu_launch(k_pause_groups, (n + block - 1) / block, block, S, A);
-  return (int)ctr[C_KERNEL_LAUNCHES];
+  EmuWorld w(G, L, W, Rcap, R, members, lane_node, live, block);
+  if (!w.ok) return -100;
+  planes(w, journaling, acc_row, acc_aux, acc_win, coord_row, node_slots);
+  return w.done(pause_groups(w.ex, w.env(), n, gids, rows, paused));
 }
 
 extern "C" int emu_select_groups(uint32_t G, uint32_t L, uint32_t W, uint32_t Rcap, uint32_t R, const int32_t* members,
                                  const int32_t* lane_node, const uint8_t* live, int journaling, int32_t* acc_row,
                                  uint32_t* acc_aux, int32_t* acc_win, int32_t* coord_row, uint32_t lane, uint32_t mask,
-                                 uint32_t value, uint32_t* gids, uint32_t cap, unsigned long long* n_found, uint32_t block) {
-  if (R > GPX_MAX_GROUP_SIZE || L > GPX_MAX_LANES || block == 0) return -1;
-  MsetInfo ms;
-  memset(&ms, 0, sizeof ms);
-  memset(ms.lane_of_idx, 0xff, sizeof ms.lane_of_idx);
-  memset(ms.idx_of_lane, 0xff, sizeof ms.idx_of_lane);
-  ms.R = (uint8_t)R;
-  for (uint32_t m = 0; m < R; m++) {
-    ms.nodes[m] = members[m];
-    for (uint32_t l = 0; l < L; l++)
-      if (lane_node[l] == members[m]) {
-        ms.lane_of_idx[m] = (uint8_t)l;
-        ms.idx_of_lane[l] = (uint8_t)m;
-      }
-  }
-  std::vector<uint32_t> meta(G);
-  for (uint32_t g = 0; g < G; g++) meta[g] = live[g] ? (0u | (R << 16) | GPX_META_LIVE) : 0u;
-  std::vector<unsigned long long> ctr((size_t)GPX_CTR_STRIPES * C_NCTR, 0ull);
-  DevState S;
-  memset(&S, 0, sizeof S);
-  S.G = G;
-  S.L = L;
-  S.W = W;
-  S.Rcap = Rcap;
-  S.journaling = journaling;
-  S.acc_row = reinterpret_cast<int4*>(acc_row);
-  S.acc_aux = acc_aux;
-  S.acc_win = reinterpret_cast<int4*>(acc_win);
-  S.coord_row = reinterpret_cast<int4*>(coord_row);
-  S.grp_meta = meta.data();
-  S.msets = &ms;
-  S.ctr = ctr.data();
-  SelectArgs A;
-  A.lane = lane;
-  A.mask = mask;
-  A.value = value;
-  A.cap = cap;
-  A.gids = gids;
-  A.n_found = n_found;
-  *n_found = 0;
-  emu_launch(k_select_groups, (G + block - 1) / block, block, S, A);
-  return (int)ctr[C_KERNEL_LAUNCHES];
+                                 uint32_t value, uint32_t* gids, uint32_t cap, uint32_t* n_found, uint32_t block) {
+  EmuWorld w(G, L, W, Rcap, R, members, lane_node, live, block);
+  if (!w.ok) return -100;
+  planes(w, journaling, acc_row, acc_aux, acc_win, coord_row, nullptr);
+  return w.done(select_groups(w.ex, w.env(), lane, mask, value, gids, cap, n_found));
 }
 
 extern "C" int emu_missing_decisions(uint32_t G, uint32_t L, uint32_t W, uint32_t R, const int32_t* members,
@@ -107,44 +42,17 @@ extern "C" int emu_missing_decisions(uint32_t G, uint32_t L, uint32_t W, uint32_
                                      uint32_t* acc_aux, int32_t* acc_win, int32_t* coord_row, uint32_t lane, uint32_t n,
                                      const uint32_t* gids, int32_t size_limit, int32_t too_much_gap, gpx_missing_rec* out,
                                      uint32_t block) {
-  if (R > GPX_MAX_GROUP_SIZE || L > GPX_MAX_LANES || block == 0) return -1;
-  MsetInfo ms;
-  memset(&ms, 0, sizeof ms);
-  memset(ms.lane_of_idx, 0xff, sizeof ms.lane_of_idx);
-  memset(ms.idx_of_lane, 0xff, sizeof ms.idx_of_lane);
-  ms.R = (uint8_t)R;
-  for (uint32_t m = 0; m < R; m++) {
-    ms.nodes[m] = members[m];
-    for (uint32_t l = 0; l < L; l++)
-      if (lane_node[l] == members[m]) {
-        ms.lane_of_idx[m] = (uint8_t)l;
-        ms.idx_of_lane[l] = (uint8_t)m;
-      }
-  }
-  std::vector<uint32_t> meta(G);
-  for (uint32_t g = 0; g < G; g++) meta[g] = live[g] ? (0u | (R << 16) | GPX_META_LIVE) : 0u;
-  std::vector<unsigned long long> ctr((size_t)GPX_CTR_STRIPES * C_NCTR, 0ull);
-  DevState S;
-  memset(&S, 0, sizeof S);
-  S.G = G;
-  S.L = L;
-  S.W = W;
-  S.Rcap = R;
-  S.journaling = journaling;
-  S.acc_row = reinterpret_cast<int4*>(acc_row);
-  S.acc_aux = acc_aux;
-  S.acc_win = reinterpret_cast<int4*>(acc_win);
-  S.coord_row = reinterpret_cast<int4*>(coord_row);
-  S.grp_meta = meta.data();
-  S.msets = &ms;
-  S.ctr = ctr.data();
-  MissingArgs A;
-  A.lane = lane;
-  A.n = n;
-  A.gids = gids;
-  A.size_limit = size_limit;
-  A.too_much_gap = too_much_gap;
-  A.out = out;
-  emu_launch(k_missing_decisions, (n + block - 1) / block, block, S, A);
-  return (int)ctr[C_KERNEL_LAUNCHES];
+  EmuWorld w(G, L, W, R, R, members, lane_node, live, block);
+  if (!w.ok) return -100;
+  planes(w, journaling, acc_row, acc_aux, acc_win, coord_row, nullptr);
+  return w.done(missing_decisions(w.ex, w.env(), lane, n, gids, size_limit, too_much_gap, out));
+}
+
+extern "C" int emu_clear_group_flags(uint32_t G, uint32_t L, uint32_t W, uint32_t R, const int32_t* members,
+                                     const int32_t* lane_node, const uint8_t* live, uint32_t* acc_aux, uint32_t lane,
+                                     uint32_t n, const uint32_t* gids, uint32_t mask, uint32_t block) {
+  EmuWorld w(G, L, W, R, R, members, lane_node, live, block);
+  if (!w.ok) return -100;
+  w.S.acc_aux = acc_aux;
+  return w.done(clear_group_flags(w.ex, w.env(), lane, n, gids, mask));
 }

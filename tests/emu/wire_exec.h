@@ -1,8 +1,8 @@
 /*
- * wire_exec.h -- the CPU executor of gigapaxos_b200/csrc/gpx_wire_seq.h, so that the CPU tests run the product's own
- * host sequences (argument checks, scratch layouts, passes, sorts, scans, capacity decisions, early exits) over the
- * kernels compiled for the host by cuda_emu.h.  Only what the CUDA executor does with CUB and the CUDA runtime is done
- * here with the standard library.  Test infrastructure only.
+ * wire_exec.h -- the CPU executor of gigapaxos_b200/csrc/gpx_wire_seq.h and gpx_state_seq.h, so that the CPU tests run
+ * the product's own host sequences (argument checks, scratch layouts, passes, sorts, scans, capacity decisions, early
+ * exits) over the kernels compiled for the host by cuda_emu.h.  Only what the CUDA executor does with CUB and the CUDA
+ * runtime is done here with the standard library.  Test infrastructure only.
  */
 #pragma once
 #include "cuda_emu.h"
@@ -13,7 +13,12 @@
 #include <string>
 #include <vector>
 
-static int fail(int code, const std::string&) { return code; }
+static std::string emu_err; /* the message of the last refusal */
+static int fail(int code, const std::string& msg) {
+  emu_err = msg;
+  return code;
+}
+extern "C" const char* emu_last_error() { return emu_err.c_str(); }
 
 #include "gpx_wire_seq.h"
 
@@ -92,6 +97,7 @@ struct EmuExec {
   }
   int read(void* host, const void* src, size_t n) { return upload(host, src, n); }
   int sync() { return GPX_OK; }
+  int settle() { return GPX_OK; } /* no lockstep records here */
   /* a fresh buffer on every layout, its bytes past `keep` garbage: a pass that reads what an earlier one wrote finds it
    * only if the layout kept it */
   int grow(void** b, size_t* cap, size_t need, size_t keep) {

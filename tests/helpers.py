@@ -16,7 +16,7 @@ from gigapaxos_b200.abi import GpxError as GpxErrorT  # noqa: E402
 
 ORACLE_PATH = os.path.join(ROOT, "oracle", "libgpx_oracle.so")
 _oracle = None
-_wire_emu = None
+_emu = {}  # (source, defines) -> the emulated library (emu_libraries)
 
 
 def oracle_library() -> Library:
@@ -30,29 +30,49 @@ def oracle_library() -> Library:
     return _oracle
 
 
-def wire_emu_library(tmp_path_factory):
-    """tests/emu/wire_emu.cpp, the wire kernels' source compiled for the host (under AddressSanitizer + UBSan when
-    GPX_EMU_SANITIZE is set), built once per process; skips the test without the CUDA headers"""
-    global _wire_emu
-    if _wire_emu is None:
-        import ctypes as C
-        import subprocess
+def ptr(a):
+    """a numpy array's data as a ctypes pointer; None stays a null pointer"""
+    import ctypes as C
+    return None if a is None else a.ctypes.data_as(C.c_void_p)
 
-        import pytest
-        cuda_inc = "/usr/local/cuda/include"
-        if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-            pytest.skip("no CUDA headers")
-        sanitize = (["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"]
-                    if os.environ.get("GPX_EMU_SANITIZE") else [])
-        out = str(tmp_path_factory.mktemp("emu") / "libwire_emu.so")
-        subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *sanitize, "-I", cuda_inc,
-                               "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
-                               "-x", "c++", os.path.join(ROOT, "tests", "emu", "wire_emu.cpp"), "-o", out])
-        lib = C.CDLL(out)
-        lib.emu_wire_new.restype = C.c_void_p
-        lib.emu_wire_new.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p]
-        _wire_emu = lib
-    return _wire_emu
+
+def emu_libraries(tmp_path_factory, *sources, defines=()):
+    """tests/emu/<source>.cpp for each source, kernel sources compiled for the host with the -D `defines` (under
+    AddressSanitizer + UBSan when GPX_EMU_SANITIZE is set) -> {source: library}.  Each (source, defines) is built once
+    per process, the missing ones at the same time; skips the test without the CUDA headers."""
+    import ctypes as C
+    import subprocess
+
+    import pytest
+    cuda_inc = "/usr/local/cuda/include"
+    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
+        pytest.skip("no CUDA headers")
+    sanitize = (["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"]
+                if os.environ.get("GPX_EMU_SANITIZE") else [])
+    defines = tuple(defines)
+    jobs = []
+    for src in sources:
+        if (src, defines) not in _emu:
+            out = str(tmp_path_factory.mktemp("emu") / f"lib{src}.so")
+            jobs.append((src, out, subprocess.Popen(
+                ["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *sanitize, *(f"-D{d}" for d in defines),
+                 "-I", cuda_inc, "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
+                 "-x", "c++", os.path.join(ROOT, "tests", "emu", src + ".cpp"), "-o", out])))
+    for src, out, p in jobs:
+        assert p.wait() == 0, f"g++ {src}.cpp"
+        lib = _emu[(src, defines)] = C.CDLL(out)
+        lib.emu_set_order.argtypes = [C.c_char_p]
+        if hasattr(lib, "emu_last_error"):  # the libraries that run the engine's sequences
+            lib.emu_last_error.restype = C.c_char_p
+        if hasattr(lib, "emu_wire_new"):  # the wire libraries' world
+            lib.emu_wire_new.restype = C.c_void_p
+            lib.emu_wire_new.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p]
+    return {src: _emu[(src, defines)] for src in sources}
+
+
+def emu_library(tmp_path_factory, source, *defines):
+    """emu_libraries for one source"""
+    return emu_libraries(tmp_path_factory, source, defines=defines)[source]
 
 
 def make_config(lib: Library, **kw) -> abi.Config:

@@ -21,36 +21,14 @@ import time
 import numpy as np
 import pytest
 
-from helpers import ROOT, abi
+from helpers import ROOT, abi, emu_libraries, ptr
 
-CUDA_INC = "/usr/local/cuda/include"
 SHUFFLES = ("shuffle:1", "shuffle:20261018")
 ORDERS = ("desc",) + SHUFFLES
 MODULES = ("test_phase1b.py", "test_pause_batch.py", "test_log_find.py",
            "test_wire_dev.py", "test_wire_device.py", "test_wire_coord.py", "test_wire_forward.py",
            "test_wire_json.py", "test_wire_json_out.py", "test_wire_json_sweep.py",
            "test_rc_cpu.py", "test_journal_frames.py", "test_journal_gc.py")
-
-
-def ptr(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
-def compile_emus(tmp_path_factory, *sources):
-    """tests/emu/<source>.cpp compiled for the host, all at once -> {source: library}; skips without the CUDA headers"""
-    if not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime.h")):
-        pytest.skip("no CUDA headers")
-    d = tmp_path_factory.mktemp("emu_orders")
-    jobs = [(src, subprocess.Popen(
-        ["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", "-I", CUDA_INC, "-I", os.path.join(ROOT, "include"),
-         "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"), "-x", "c++", os.path.join(ROOT, "tests", "emu", src + ".cpp"),
-         "-o", str(d / (src + ".so"))])) for src in sources]
-    libs = {}
-    for src, p in jobs:
-        assert p.wait() == 0, src
-        lib = libs[src] = C.CDLL(str(d / (src + ".so")))
-        lib.emu_set_order.argtypes = [C.c_char_p]
-    return libs
 
 
 class order:
@@ -70,7 +48,7 @@ class order:
 
 @pytest.fixture(scope="module")
 def probe(tmp_path_factory):
-    lib = compile_emus(tmp_path_factory, "order_probe_emu")["order_probe_emu"]
+    lib = emu_libraries(tmp_path_factory, "order_probe_emu")["order_probe_emu"]
     lib.emu_probe_chain.argtypes = lib.emu_probe_append.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32]
     return lib
 
@@ -142,7 +120,7 @@ def child_command():
 @pytest.fixture(scope="module")
 def children(request):
     """one child pytest per order this session runs, all started at once: each is about two minutes of one core"""
-    if not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime.h")):
+    if not os.path.exists("/usr/local/cuda/include/cuda_runtime.h"):
         pytest.skip("no CUDA headers")
     wanted = [it.callspec.params["spec"] for it in request.session.items
               if it.module is request.module and it.originalname == "test_emulated_kernels_pass_in_order"]
@@ -191,14 +169,15 @@ SIGNATURES = {
     "emu_jgc_names": ([P, U32, P, P, P, P], None),
     "emu_jgc_compact": ([P, P, U64, P, U32, P, U32, P, U32, U32, P, P, P, P, U32], C.c_int),
     "emu_jgc_index": ([P, U64, U32, P, U32, P, P], C.c_int),
-    "emu_log_find": ([P, U64, U64, U64, U32, U32, P, P, U32, U32, U32, P], C.c_int),
+    "emu_log_find": ([P, U64, U64, U64, U32, U32, P, P, U32, U32], C.c_int),
+    "emu_log_gather": ([P, U64, U64, U32, U32, P, P, U64, U32], C.c_int),
 }
 
 
 @pytest.fixture(scope="module")
 def emus(tmp_path_factory):
     """every emulated entry point: source -> library"""
-    libs = compile_emus(tmp_path_factory, *SOURCES)
+    libs = emu_libraries(tmp_path_factory, *SOURCES)
     for lib in libs.values():
         for f, (args, res) in SIGNATURES.items():
             if hasattr(lib, f):
@@ -471,7 +450,7 @@ def test_prepare_tally_in_every_order(oracle_lib, emus):
         got = np.zeros(len(els), abi.election_out_dtype)
         got.view(np.uint8)[:] = 0xAB
         assert lib.emu_prepare_tally(G, R, W, R, R, ptr(members), ptr(members), ptr(live), ptr(crow), ptr(aux), ptr(nsl),
-                                     ptr(pwin), len(els), ptr(els), ptr(reps), ptr(got), 7) == 1
+                                     ptr(pwin), len(els), ptr(els), len(reps), ptr(reps), ptr(got), 7) == 1
         return [got, aux, crow, nsl, pwin]
     out = same_in_every_order(lib, run)
     verdicts = np.frombuffer(out[0][2], abi.election_out_dtype)["verdict"]
@@ -479,11 +458,10 @@ def test_prepare_tally_in_every_order(oracle_lib, emus):
 
 
 def test_pause_select_and_missing_in_every_order(oracle_lib, emus):
-    """emu_pause_groups (verdicts, rows, the state it leaves), emu_missing_decisions, and emu_select_groups, whose
-    kernel appends each match with one atomicAdd.  gpx.h promises gpx_select_groups' "out_gids[0 .. min(*n_found, cap))
-    in ascending order", and the engine sorts them on the host after the kernel; so the kernel's gids are compared as a
-    set, and with too small a buffer ("which `cap` of them were returned is unspecified") only their count and that
-    they match"""
+    """emu_pause_groups (verdicts, rows, the state it leaves), emu_missing_decisions, emu_clear_group_flags, and
+    emu_select_groups, whose kernel appends each match with one atomicAdd and whose gids the host sorts afterwards.
+    With too small a buffer ("which `cap` of them were returned is unspecified", gpx.h) only their count and that they
+    match are compared"""
     from test_pause_batch import NODES, busy_engine, pause_state
     lib = emus["pause_emu"]
     R, G, W = 3, 120, 8
@@ -502,12 +480,12 @@ def test_pause_select_and_missing_in_every_order(oracle_lib, emus):
         for lane, mask, value in sweeps:
             for cap in (G, 5):  # all matches fit, then too few
                 found = np.zeros(cap, np.uint32)
-                n = np.zeros(1, np.uint64)
+                n = np.zeros(1, np.uint32)
                 assert lib.emu_select_groups(G, R, W, R, R, ptr(nodes), ptr(nodes), ptr(live), 0, ptr(acc_row),
                                              ptr(acc_aux), ptr(acc_win), ptr(coord_row), lane, mask, value, ptr(found),
                                              cap, ptr(n), 7) == 1
                 if int(n[0]) <= cap:
-                    out.append(np.sort(found[: int(n[0])]))
+                    out.append(found[: int(n[0])])
                 else:
                     assert np.isin(found, out[-1]).all()
                     out.append(n)
@@ -518,6 +496,9 @@ def test_pause_select_and_missing_in_every_order(oracle_lib, emus):
                                              ptr(acc_aux), ptr(acc_win), ptr(coord_row), lane, len(gids), ptr(gids),
                                              400, 400, ptr(miss), 7) == 1
             out.append(miss)
+        for lane in range(R):
+            assert lib.emu_clear_group_flags(G, R, W, R, ptr(nodes), ptr(nodes), ptr(live), ptr(acc_aux), lane,
+                                             len(gids) - lane, ptr(gids), abi.GF_NEEDS_SYNC << lane % 2, 7) == 0
         rows = np.zeros((len(gids), R), abi.row_dtype)
         ok = np.full(len(gids), 7, np.uint8)
         assert lib.emu_pause_groups(G, R, W, R, R, ptr(nodes), ptr(nodes), ptr(live), 0, ptr(acc_row), ptr(acc_aux),
@@ -563,22 +544,20 @@ def test_log_find_and_gather_in_every_order(oracle_lib, emus):
         r["pos"], r["len"] = hits["blob_pos"], hits["accept"]["payload_len"]
         padded = (r["len"].astype(np.uint64) + 15) // 16 * 16
         r["dst_off"] = np.concatenate([[0], np.cumsum(padded)[:-1]])
-        first = np.concatenate([[0], np.cumsum(padded // 16)]).astype(np.uint32)
-        rings.append((ring, cap, len(buf), r, first, int(padded.sum()) + 64))
+        rings.append((ring, cap, len(buf), r, int(padded.sum()) + 64))
     eng.close()
 
     def run():
         out = []
-        for lane, (ring, cap, head, r, first, n_out) in enumerate(rings):
+        for lane, (ring, cap, head, r, n_out) in enumerate(rings):
             for grid, block in ((3, 7), (5, 64)):
                 hits = np.zeros((len(wants), abi.GPX_LOG_SPAN), abi.log_hit_dtype)
                 hits.view(np.uint8)[:] = 0xCD
-                ctl = np.zeros(4, np.uint64)
-                assert lib.emu_log_find(ptr(ring), cap, head, 0, lane, len(wants), ptr(wants), ptr(hits), 4096, grid,
-                                        block, ptr(ctl)) == 1
-                out += [hits, ctl]
+                assert lib.emu_log_find(ptr(ring), cap, head, 0, lane, len(wants), ptr(wants), ptr(hits), grid,
+                                        block) == 1
+                out.append(hits)
             gathered = np.full(n_out, 0xEE, np.uint8)
-            assert lib.emu_log_gather(ptr(ring), U64(cap), lane, len(r), ptr(r), ptr(first), ptr(gathered), 7) == 0
+            assert lib.emu_log_gather(ptr(ring), cap, head, lane, len(r), ptr(r), ptr(gathered), n_out, 7) == 0
             out.append(gathered)
         return out
     out = same_in_every_order(lib, run)

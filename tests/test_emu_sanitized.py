@@ -19,7 +19,7 @@ def test_emulated_kernels_are_clean_under_asan_and_ubsan():
     r = subprocess.run([sys.executable, "-m", "pytest", "-x", "-q", "-p", "no:cacheprovider",
                         os.path.join(ROOT, "tests", "test_phase1b.py"), os.path.join(ROOT, "tests", "test_pause_batch.py"),
                         os.path.join(ROOT, "tests", "test_log_find.py"),
-                        "-k", "kernel_source or run_away or absurd or select_kernel or missing_kernel"],
+                        "-k", "kernel_source or run_away or absurd or more_segments or select_kernel or missing_kernel"],
                        capture_output=True, text=True, env=env, cwd=ROOT, timeout=900)
     assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
     assert " passed" in r.stdout and "AddressSanitizer" not in r.stderr and "runtime error" not in r.stderr

@@ -16,25 +16,16 @@ import numpy as np
 import pytest
 
 from gigapaxos_b200 import journal
-from helpers import ROOT, abi, relay_into_small_ring
+from helpers import ROOT, abi, emu_library, ptr, relay_into_small_ring
 from test_log_find import logged_engine
 
-SANITIZE = ["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"] if os.environ.get("GPX_EMU_SANITIZE") else []
 BLOCKS = [1, 7, 64]
 I32, I64 = (-(1 << 31), (1 << 31) - 1), (-(1 << 63), (1 << 63) - 1)
 
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    cuda_inc = "/usr/local/cuda/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("no CUDA headers")
-    so = str(tmp_path_factory.mktemp("jfemu") / "libjournal_emu.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *SANITIZE, "-I", cuda_inc,
-                           "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
-                           "-I", os.path.join(ROOT, "tests", "emu"), "-x", "c++",
-                           os.path.join(ROOT, "tests", "emu", "journal_emu.cpp"), "-o", so])
-    lib = C.CDLL(so)
+    lib = emu_library(tmp_path_factory, "journal_emu")
     lib.emu_journal_new.restype = C.c_void_p
     lib.emu_journal_new.argtypes = [C.c_uint32, C.c_uint32]
     lib.emu_journal_free.argtypes = [C.c_void_p]
@@ -43,10 +34,6 @@ def lib(tmp_path_factory):
     lib.emu_log_frame.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint32,
                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]
     return lib
-
-
-def ptr(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
 def hard_names(G, rng):

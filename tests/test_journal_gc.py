@@ -17,26 +17,17 @@ import numpy as np
 import pytest
 
 from gigapaxos_b200 import journal, wire
-from helpers import ROOT, abi, relay_into_small_ring
+from helpers import ROOT, abi, emu_library, ptr, relay_into_small_ring
 from test_journal_frames import hard_names, log_drainer, make_meta, oracle_ring, requests_of
 from test_log_find import logged_engine
 
-SANITIZE = ["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"] if os.environ.get("GPX_EMU_SANITIZE") else []
 BLOCKS = [1, 7, 64]
 I32 = (-(1 << 31), (1 << 31) - 1)
 
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    cuda_inc = "/usr/local/cuda/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("no CUDA headers")
-    so = str(tmp_path_factory.mktemp("jgcemu") / "libjournal_gc_emu.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *SANITIZE, "-I", cuda_inc,
-                           "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
-                           "-I", os.path.join(ROOT, "tests", "emu"), "-x", "c++",
-                           os.path.join(ROOT, "tests", "emu", "journal_gc_emu.cpp"), "-o", so])
-    lib = C.CDLL(so)
+    lib = emu_library(tmp_path_factory, "journal_gc_emu")
     lib.emu_jgc_new.restype = C.c_void_p
     lib.emu_jgc_new.argtypes = [C.c_uint32]
     lib.emu_jgc_free.argtypes = [C.c_void_p]
@@ -46,10 +37,6 @@ def lib(tmp_path_factory):
                                     C.c_uint32]
     lib.emu_jgc_index.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
     return lib
-
-
-def ptr(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
 def index(lib, buf, base=0, cap=None):

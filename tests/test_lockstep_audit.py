@@ -8,8 +8,9 @@ settle is missing: the kernel answers from a slot one or more rounds old.  So ev
 function or macro it reaches, names a plane word is listed below with the reason it never sees a stale one, and a new
 such kernel, or a new launch of a listed one, fails this test until the table says how it is settled.
 
-For kernels that are settled, the test also checks each host function that launches them: an ls_settle call comes
-before the launch in that function, or the function is one of the launch helpers that settle (gpx_engine.cu).
+For kernels that are settled, the test also checks each host function that launches them: an ls_settle call, or in a
+host sequence of gpx_state_seq.h an ex.settle() call (ls_settle on the device), comes before the launch in that
+function, or the function is one of the launch helpers that settle (gpx_engine.cu).
 """
 import os
 import re
@@ -22,8 +23,8 @@ CSRC = os.path.join(ROOT, "gigapaxos_b200", "csrc")
 PLANE_WORDS = {"acc_row", "coord_row", "ns_u", "node_slots"}
 
 SETTLED, CURRENT, OWNER = "settled", "current", "owner"
-# kernel -> (reason, {host function that launches it: how the launch is settled}).  "settles": ls_settle comes
-# earlier in the same function; "<helper>": the launch is in a helper that settles first, or whose only callers do.
+# kernel -> (reason, {host function that launches it: how the launch is settled}).  "settles": ls_settle or
+# ex.settle comes earlier in the same function; "<helper>": the launch is in a helper that settles first, or whose only callers do.
 PLANE_KERNELS = {
     "k_propose": (SETTLED, {"launch_propose": "settles"}),
     "k_accept": (SETTLED, {"launch_accept": "settles"}),
@@ -37,11 +38,11 @@ PLANE_KERNELS = {
     "k_load_rows": (SETTLED, {"gpx_load_rows": "settles"}),
     "k_patch": (SETTLED, {"gpx_patch": "settles"}),
     "k_get_flags": (SETTLED, {"gpx_get_group_flags": "settles"}),
-    "k_select_groups": (SETTLED, {"gpx_select_groups": "settles"}),
-    "k_missing_decisions": (SETTLED, {"gpx_missing_decisions": "settles"}),
-    "k_pause_groups": (SETTLED, {"gpx_pause_groups": "settles"}),
+    "k_select_groups": (SETTLED, {"select_groups": "settles"}),
+    "k_missing_decisions": (SETTLED, {"missing_decisions": "settles"}),
+    "k_pause_groups": (SETTLED, {"pause_groups": "settles"}),
     "k_prepare": (SETTLED, {"gpx_handle_prepares": "settles"}),
-    "k_prepare_tally": (SETTLED, {"gpx_handle_prepare_replies": "settles"}),
+    "k_prepare_tally": (SETTLED, {"prepare_replies": "settles"}),
     "k_sp_tally": (SETTLED, {"spread_enqueue": "gpx_spread_round"}),
     "k_sp_commit": (SETTLED, {"spread_enqueue": "gpx_spread_round"}),
     "k_sp_accept": (SETTLED, {"spread_enqueue": "gpx_spread_round"}),
@@ -163,10 +164,10 @@ def plane_kernels():
 
 
 def host_functions():
-    """{host function: body} of gpx_engine.cu and the host files it includes"""
+    """{host function: body} of gpx_engine.cu, the host files it includes and the host sequences of gpx_state_seq.h"""
     out = {}
     for f in sorted(os.listdir(CSRC)):
-        if f.endswith((".cu", ".inc", ".cpp")):
+        if f.endswith((".cu", ".inc", ".cpp")) or f == "gpx_state_seq.h":
             _, src = macros(strip(open(os.path.join(CSRC, f)).read()))
             for name, _, body in functions(src):
                 out[name] = out.get(name, "") + body
@@ -205,8 +206,8 @@ def test_every_launch_of_a_plane_kernel_is_settled(kernel):
         if how == "settles":
             # textual order only: a settle on one branch and the launch on another would pass.  Every settling
             # function today settles unconditionally right before its launch; the GPU tests catch the rest.
-            s = body.find("ls_settle(")
-            assert 0 <= s < at, f"{fn} launches {kernel} without an ls_settle before it"
+            s = min((i for i in (body.find("ls_settle("), body.find("ex.settle(")) if i >= 0), default=-1)
+            assert 0 <= s < at, f"{fn} launches {kernel} without an ls_settle or ex.settle before it"
         elif how == "launch_round":
             lr = host["launch_round"]
             assert re.search(r"if \(round_uses_ls\(e\)\)\s*e->ls_live = true;\s*else\s*ls_settle\(e, st\);", lr), \
@@ -219,6 +220,12 @@ def test_every_launch_of_a_plane_kernel_is_settled(kernel):
             assert launch_sites(host, fn) == {"gpx_spread_round"}
         else:
             assert kernel == "k_ls_settle"
+
+
+def test_the_sequences_settle_with_ls_settle_on_the_device():
+    """ex.settle() in a sequence of gpx_state_seq.h is the CUDA executor's settle, which must be ls_settle"""
+    host = host_functions()
+    assert "ls_settle(e, st);" in host["settle"]
 
 
 def test_every_call_of_a_launch_helper_is_after_its_settle():

@@ -7,18 +7,13 @@ source (gigapaxos_b200/csrc/gpx_logfind.cuh) compiled for the host (tests/emu) o
 as they lie, and re-laid into a small ring that wraps (stale laps, skipped tails) the way the device lays them.  The GPU
 test is in tests/test_zz_phase1b_gpu.py."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 # GPX_EMU_SANITIZE=1 LD_PRELOAD=$(gcc -print-file-name=libasan.so) python -m pytest ... : the emulated kernels under
 # AddressSanitizer + UBSan (every heap buffer numpy hands them gets red zones; so do their local arrays)
-import os as _os
-EMU_SANITIZE = ["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"] if _os.environ.get("GPX_EMU_SANITIZE") else []
-
-from helpers import ROOT, Engine, abi, group_descs, make_config, make_requests, relay_into_small_ring
+from helpers import Engine, abi, emu_library, group_descs, make_config, make_requests, ptr, relay_into_small_ring
 
 NODES = [100, 101, 102]
 
@@ -164,30 +159,26 @@ def test_oracle_log_find_equals_a_walk_of_the_ring(oracle_lib, seed):
     assert np.any(h["accept"]["bnum"][ok] == row0["acc_bnum"].max())
 
 
-# ---- the CUDA kernels' own source on the host ---------------------------------------------------------------------------
+# ---- the CUDA kernels' own source on the host, driven by the engine's own sequences (gpx_state_seq.h) ----------------------
 @pytest.fixture(scope="module")
 def emu_lib(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu") / "liblogfind_emu.so")
-    cuda_inc = "/usr/local/cuda/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("no CUDA headers")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *EMU_SANITIZE, "-I", cuda_inc,
-                           "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
-                           "-x", "c++", os.path.join(ROOT, "tests", "emu", "logfind_emu.cpp"), "-o", out])
-    lib = C.CDLL(out)
-    lib.emu_log_find.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
-                                 C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]
+    lib = emu_library(tmp_path_factory, "logfind_emu")
+    lib.emu_log_find.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p,
+                                 C.c_void_p, C.c_uint32, C.c_uint32]
+    lib.emu_log_gather.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
+                                   C.c_uint64, C.c_uint32]
     return lib
 
 
-def emu_find(emu_lib, ring, cap, head, start, lane, wants, seg_cap=4096, grid=3, block=64):
+def emu_find(emu_lib, ring, cap, head, start, lane, wants, grid=3, block=64, rc=1, error=None):
+    """gpx_log_find on the ring image; rc: 1 (k_log_dir's launch) or the GPX_* error expected, with `error` in its
+    message"""
     hits = np.zeros((len(wants), abi.GPX_LOG_SPAN), dtype=abi.log_hit_dtype)
     hits.view(np.uint8)[:] = 0xCD
-    ctl = np.zeros(4, dtype=np.uint64)
-    ptr = lambda a: a.ctypes.data_as(C.c_void_p)
-    rc = emu_lib.emu_log_find(ptr(ring), cap, head, start, lane, len(wants), ptr(wants), ptr(hits), seg_cap, grid, block, ptr(ctl))
-    assert rc == 1  # k_log_dir counts the launch
-    return hits, ctl
+    assert emu_lib.emu_log_find(ptr(ring), cap, head, start, lane, len(wants), ptr(wants), ptr(hits), grid, block) == rc
+    if error:
+        assert error in emu_lib.emu_last_error().decode()
+    return hits
 
 
 @pytest.mark.parametrize("seed,grid,block", [(3, 3, 64), (4, 1, 1), (5, 7, 256)])
@@ -203,15 +194,28 @@ def test_kernel_source_on_the_host_equals_oracle(oracle_lib, emu_lib, seed, grid
         for start in (0, heads[lane][len(heads[lane]) // 3]):
             wants = random_wants(G, rng)
             want = eng.log_find(lane, wants, start)
-            got, ctl = emu_find(emu_lib, ring, cap, head, start, lane, wants, grid=grid, block=block)
-            assert int(ctl[2]) == 0 and int(ctl[3]) == head and int(ctl[0]) > 5
+            got = emu_find(emu_lib, ring, cap, head, start, lane, wants, grid=grid, block=block)
             assert got.tobytes() == want.tobytes()
-    # a directory that is too small, bytes that were overwritten: reported, nothing found
+    # bytes that were overwritten: reported, nothing found
     wants = random_wants(G, rng)
-    got, ctl = emu_find(emu_lib, ring, cap, head, 0, 2, wants, seg_cap=3)
-    assert int(ctl[2]) == 3 and np.all(got["decision"]["flags"] == abi.F_VOID) and np.all(got["accept"]["flags"] == abi.F_VOID)
-    got, ctl = emu_find(emu_lib, ring, cap, head + 2 * cap, 0, 2, wants)
-    assert int(ctl[2]) == 1
+    got = emu_find(emu_lib, ring, cap, head + 2 * cap, 0, 2, wants, rc=abi.GPX_ERANGE, error="already overwritten")
+    assert np.all(got["decision"]["flags"] == abi.F_VOID) and np.all(got["accept"]["flags"] == abi.F_VOID)
+
+
+def test_more_segments_than_the_directory_holds(emu_lib):
+    """the directory holds ring_cap / GPX_SEG_DEC_BYTES(1) + 2 segments, more than any launch of the engine fills the
+    ring with; a ring of 64-byte segments that carry no slot (no launch writes those) overfills it: reported, nothing
+    found"""
+    cap = 1 << 10
+    ring = np.zeros(cap, dtype=np.uint8)
+    hdr = ring.view(abi.seg_hdr_dtype)
+    hdr["magic"], hdr["type"], hdr["rec_bytes"], hdr["ring_off"] = abi.SEG_MAGIC, abi.F_DECISION, 32, np.arange(0, cap, 64)
+    wants = np.zeros(1, dtype=abi.log_want_dtype)
+    wants["n_slots"] = 4
+    got = emu_find(emu_lib, ring, cap, 12 * 64, 0, 0, wants)  # 12 segments: as many as it holds
+    assert np.all(got["decision"]["flags"] == abi.F_VOID)
+    got = emu_find(emu_lib, ring, cap, 13 * 64, 0, 0, wants, rc=abi.GPX_ERANGE, error="more log segments")
+    assert np.all(got["decision"]["flags"] == abi.F_VOID) and np.all(got["accept"]["flags"] == abi.F_VOID)
 
 
 @pytest.mark.parametrize("seed", [6, 7])
@@ -232,8 +236,7 @@ def test_kernel_source_on_a_ring_that_wraps(oracle_lib, emu_lib, seed):
         assert 0 < first < len(call_pos) - 1
         wants = random_wants(G, rng, max_slot=16)
         want = eng.log_find(lane, wants, hs[first])
-        got, ctl = emu_find(emu_lib, ring, cap, head, call_pos[first], lane, wants)
-        assert int(ctl[2]) == 0
+        got = emu_find(emu_lib, ring, cap, head, call_pos[first], lane, wants)
         for f in ("decision", "accept"):
             assert got[f].tobytes() == want[f].tobytes(), f
         assert ((want["accept"]["flags"] & abi.F_VOID) == 0).any()
@@ -247,8 +250,7 @@ def test_kernel_source_on_a_ring_that_wraps(oracle_lib, emu_lib, seed):
             gp = int(got[i, k]["blob_pos"]) % cap
             assert bytes(ring[gp: gp + n]) == bytes(buf[ob: ob + n])
         # one call too far back: its bytes are gone
-        got, ctl = emu_find(emu_lib, ring, cap, head, call_pos[0], lane, wants)
-        assert int(ctl[2]) == 1
+        emu_find(emu_lib, ring, cap, head, call_pos[0], lane, wants, rc=abi.GPX_ERANGE, error="already overwritten")
 
 
 def test_a_header_with_absurd_sizes_is_not_followed(emu_lib):
@@ -262,8 +264,8 @@ def test_a_header_with_absurd_sizes_is_not_followed(emu_lib):
     wants["n_slots"] = 4
     for pb in ((1 << 64) - 64, 1 << 40):
         ring[:64].view(abi.seg_hdr_dtype)[0]["payload_bytes"] = pb
-        got, ctl = emu_find(emu_lib, ring, cap, 2048, 0, 0, wants)
-        assert int(ctl[2]) == 2 and np.all(got["decision"]["flags"] == abi.F_VOID)
+        got = emu_find(emu_lib, ring, cap, 2048, 0, 0, wants, rc=abi.GPX_EINVAL, error="`from` is not a segment boundary")
+        assert np.all(got["decision"]["flags"] == abi.F_VOID)
 
 
 # ---- gpx_log_gather: the bodies of a batch of hits in one copy ---------------------------------------------------------------
@@ -291,16 +293,36 @@ def test_log_gather_oracle_and_kernel_source(oracle_lib, emu_lib):
         r = np.zeros(len(pos), dtype=abi.log_range_dtype)
         r["pos"], r["len"] = pos, ln
         padded = (ln.astype(np.uint64) + 15) // 16 * 16
-        r["dst_off"] = np.concatenate([[0], np.cumsum(padded)[:-1]])
-        first = np.concatenate([[0], np.cumsum(padded // 16)]).astype(np.uint32)
-        out = np.full(int(padded.sum()) + 64, 0xEE, dtype=np.uint8)
-        ptr = lambda a: a.ctypes.data_as(C.c_void_p)
+        gaps = np.arange(len(r), dtype=np.uint64) % 3 * 16  # bytes between the ranges read as zero
+        r["dst_off"] = np.concatenate([[0], np.cumsum(padded + gaps)[:-1]]) + gaps
+        top = int(r["dst_off"][-1] + padded[-1])
+        out = np.full(top + 64, 0xEE, dtype=np.uint8)
         for block in (1, 64, 256):
             out[:] = 0xEE
-            assert emu_lib.emu_log_gather(ptr(ring), C.c_uint64(cap), lane, len(r), ptr(r), ptr(first), ptr(out), block) == 0
+            assert emu_lib.emu_log_gather(ptr(ring), cap, head, lane, len(r), ptr(r), ptr(out), len(out), block) == 0
+            written = np.zeros(len(out), dtype=bool)
             for o, n, b in zip(r["dst_off"], ln, want):
                 assert bytes(out[int(o): int(o) + int(n)]) == b
-            assert np.all(out[int(padded.sum()):] == 0xEE)  # nothing written past the last chunk
+                written[int(o): int(o) + int(n)] = True
+            assert not out[:top][~written[:top]].any()  # gaps and padding are zero
+            assert np.all(out[top:] == 0xEE)  # nothing written past the last chunk
+    # the range checks, on a ring of 256 bytes whose head has wrapped to 304: each refused, nothing written
+    ring = np.arange(256, dtype=np.uint8)
+    out = np.full(64, 0xEE, dtype=np.uint8)
+    for pos, ln, dst_off, rc, error in ((56, 4, 0, abi.GPX_EINVAL, "16-byte boundary"),
+                                        (48, 4, 8, abi.GPX_EINVAL, "16-byte boundary"),
+                                        (288, 32, 0, abi.GPX_ERANGE, "outside the live ring bytes"),
+                                        (32, 16, 0, abi.GPX_ERANGE, "outside the live ring bytes"),
+                                        (240, 32, 0, abi.GPX_ERANGE, "straddles the ring end"),
+                                        (256, 16, 64, abi.GPX_ERANGE, "range beyond dst")):
+        r = np.zeros(2, dtype=abi.log_range_dtype)
+        r["pos"], r["len"], r["dst_off"] = [256, pos], [16, ln], [16, dst_off]
+        assert emu_lib.emu_log_gather(ptr(ring), 256, 304, 0, 2, ptr(r), ptr(out), len(out), 7) == rc, error
+        assert error in emu_lib.emu_last_error().decode() and np.all(out == 0xEE)
+    r["pos"], r["len"], r["dst_off"] = [256, 288], [16, 16], [16, 48]  # both live: [16, 32) and [48, 64), zeros around
+    assert emu_lib.emu_log_gather(ptr(ring), 256, 304, 0, 2, ptr(r), ptr(out), len(out), 7) == 0
+    assert not out[:16].any() and list(out[16:32]) == list(range(16)) and not out[32:48].any()
+    assert list(out[48:]) == list(range(32, 48))
     with pytest.raises(abi.GpxError):
         eng.log_gather(0, [8], [4])  # not on a 16-byte boundary
     with pytest.raises(abi.GpxError):

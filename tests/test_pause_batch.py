@@ -4,20 +4,14 @@ pause(Map, dequeue) :2327-2366 over PISM.tryPause :2004-2035).
 CPU: the oracle's entry point against the per-group path it replaces (gpx_get_group_flags x lanes + gpx_dump_rows x lanes
 + gpx_destroy_groups), through the host mirror; and k_pause_groups' own source (gigapaxos_b200/csrc/gpx_pause.cuh)
 compiled for the host (tests/emu) against the oracle.  The GPU test is in tests/test_zz_phase1b_gpu.py."""
-import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 # GPX_EMU_SANITIZE=1 LD_PRELOAD=$(gcc -print-file-name=libasan.so) python -m pytest ... : the emulated kernels under
 # AddressSanitizer + UBSan (every heap buffer numpy hands them gets red zones; so do their local arrays)
-import os as _os
-EMU_SANITIZE = ["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"] if _os.environ.get("GPX_EMU_SANITIZE") else []
-
 from gigapaxos_b200.paxos_manager import HashChainApp, PaxosManager
-from helpers import ROOT, Engine, abi, group_descs, make_config, make_requests
+from helpers import Engine, abi, emu_library, group_descs, make_config, make_requests, ptr
 
 NODES = [100, 101, 102]
 
@@ -128,17 +122,10 @@ def test_mirror_pause_batch(oracle_lib):
     assert a.apps[0].state == b.apps[0].state and a.num_decisions == b.num_decisions
 
 
-# ---- the CUDA kernel's own source on the host -------------------------------------------------------------------------
+# ---- the CUDA kernels' own source on the host, driven by the engine's own sequences (gpx_state_seq.h) -------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def emu_lib(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("emu") / "libpause_emu.so")
-    cuda_inc = "/usr/local/cuda/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("no CUDA headers")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *EMU_SANITIZE, "-I", cuda_inc,
-                           "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
-                           "-x", "c++", os.path.join(ROOT, "tests", "emu", "pause_emu.cpp"), "-o", out])
-    return C.CDLL(out)
+    return emu_library(tmp_path_factory, "pause_emu")
 
 
 def pause_state(eng, R, G, W, journaling, rng):
@@ -194,7 +181,6 @@ def test_kernel_source_on_the_host_equals_oracle(oracle_lib, emu_lib, journaling
     want_rows, want_ok = eng.pause_groups(gids)
     got_rows = np.zeros((len(gids), R), dtype=abi.row_dtype)
     got_ok = np.full(len(gids), 7, dtype=np.uint8)
-    ptr = lambda a: a.ctypes.data_as(C.c_void_p)
     nodes_a = np.array(nodes, dtype=np.int32)
     rc = emu_lib.emu_pause_groups(G, R, W, R, R, ptr(nodes_a), ptr(nodes_a), ptr(live), int(journaling), ptr(acc_row), ptr(acc_aux),
                                   ptr(acc_win), ptr(coord_row), ptr(node_slots), len(gids), ptr(gids), ptr(got_rows), ptr(got_ok),
@@ -206,6 +192,13 @@ def test_kernel_source_on_the_host_equals_oracle(oracle_lib, emu_lib, journaling
             continue
         assert np.array_equal(got_rows[f][want_ok], want_rows[f][want_ok]), f
     assert not got_rows[~want_ok].view(np.uint8).any()  # rows of groups that did not pause are not written
+    # a gid twice in the batch: refused before anything runs
+    aux0, rows0 = acc_aux.copy(), got_rows.copy()
+    dup = np.array([gids[0], gids[1], gids[0]], dtype=np.uint32)
+    assert emu_lib.emu_pause_groups(G, R, W, R, R, ptr(nodes_a), ptr(nodes_a), ptr(live), int(journaling), ptr(acc_row),
+                                    ptr(acc_aux), ptr(acc_win), ptr(coord_row), ptr(node_slots), len(dup), ptr(dup),
+                                    ptr(got_rows), ptr(got_ok), block) == abi.GPX_EINVAL
+    assert b"twice" in emu_lib.emu_last_error() and np.array_equal(acc_aux, aux0) and np.array_equal(got_rows, rows0)
     after = [eng.dump_rows(all_g, l) for l in range(R)]
     for l in range(R):
         freed = after[l]["state"] == abi.ST_FREE
@@ -285,22 +278,24 @@ def test_select_kernel_source_on_the_host_equals_oracle(oracle_lib, emu_lib, jou
         livepv = busy & (why == 2)
         acc_win[l, 3, :, 0] = np.where(livepv, r["acc_gc_slot"] + 2, acc_win[l, 3, :, 0])
         flags[l] = (flags[l] & abi.GF_NOT_CAUGHT_UP) | sticky.astype(np.uint8)
-    ptr = lambda a: a.ctypes.data_as(C.c_void_p)
     nodes_a = np.array(nodes, dtype=np.int32)
     for lane in range(R):
         active = np.isin(rows[lane]["state"], (abi.ST_ACTIVE_1, abi.ST_ACTIVE_2))
         for mask, value in ((abi.GF_NOT_CAUGHT_UP, 0), (abi.GF_NEEDS_SYNC, abi.GF_NEEDS_SYNC),
                             (abi.GF_NEEDS_SYNC | abi.GF_NOT_CAUGHT_UP, abi.GF_NOT_CAUGHT_UP), (0, 0)):
             want = all_g[active & ((flags[lane] & mask) == value)]
-            for cap in (G, max(len(want) - 2, 0)):
+            for cap, spec in ((G, b"asc"), (G, b"desc"), (max(len(want) - 2, 0), b"desc")):
                 out = np.full(max(cap, 1), 0xFFFFFFFF, dtype=np.uint32)
-                found = np.zeros(1, dtype=np.uint64)
+                found = np.zeros(1, dtype=np.uint32)
+                emu_lib.emu_set_order(spec)  # the kernel appends in thread order; the host sorts what it appended
                 rc = emu_lib.emu_select_groups(G, R, W, R, R, ptr(nodes_a), ptr(nodes_a), ptr(live), int(journaling), ptr(acc_row),
                                                ptr(acc_aux), ptr(acc_win), ptr(coord_row), lane, mask, value, ptr(out), cap,
                                                ptr(found), block)
+                emu_lib.emu_set_order(None)
                 assert rc == 1 and int(found[0]) == len(want)
-                got = np.sort(out[: min(cap, len(want))])
+                got = out[: min(cap, len(want))]  # sorted on the host
                 assert np.array_equal(got, want) if cap >= len(want) else np.all(np.isin(got, want))
+                assert np.all(np.diff(got.astype(np.int64)) > 0) and np.all(out[len(got):] == 0xFFFFFFFF)
 
 
 # ---- the slow-path list end to end: a replica that missed decisions is named by the engine, caught up, taken off the list ---
@@ -460,7 +455,6 @@ def test_missing_kernel_source_on_the_host_equals_the_model(emu_lib, seed, block
                 acc_win[l, w, g, 7] = 0 if k == 2 else 1
     gids = rng.permutation(G + 3).astype(np.uint32)
     nodes = np.array(NODES, dtype=np.int32)
-    ptr = lambda a: a.ctypes.data_as(C.c_void_p)
     for lane in range(L):
         for size_limit, gap_th in ((400, 400), (3, 400), (400, 4), (400, 1)):
             out = np.zeros(len(gids), dtype=abi.missing_dtype)
@@ -480,3 +474,31 @@ def test_missing_kernel_source_on_the_host_equals_the_model(emu_lib, seed, block
                 assert int(r["slot"]) == slot and int(r["max_decision_slot"]) == max_c, (lane, g)
                 assert list(r["missing"][: int(r["n_missing"])]) == missing and bool(r["missing_too_much"]) == too, (lane, g)
                 assert not r["missing"][int(r["n_missing"]):].any()
+
+
+@pytest.mark.parametrize("seed,block", [(41, 128), (42, 3)])
+def test_clear_flags_kernel_source_on_the_host(emu_lib, seed, block):
+    """gpx_clear_group_flags: only the OVERFLOW / NEEDS_SYNC bits of the mask, only this lane, only these gids (those
+    beyond max_groups are skipped); a gid twice or a lane beyond the engine's is refused and nothing changes"""
+    rng = np.random.default_rng(seed)
+    G, L, W, R = 150, 3, 8, 3
+    nodes = np.array(NODES, dtype=np.int32)
+    live = np.ones(G, dtype=np.uint8)
+    aux = rng.integers(0, 1 << 32, size=(L, G), dtype=np.uint64).astype(np.uint32)
+    for lane in range(L):
+        for mask in (abi.GF_NEEDS_SYNC, abi.GF_OVERFLOW | abi.GF_NEEDS_SYNC | abi.GF_NOT_CAUGHT_UP, 0):
+            gids = rng.choice(G + 5, size=60, replace=False).astype(np.uint32)
+            want = aux.copy()
+            ok = gids[gids < G]
+            want[lane, ok] &= ~np.uint32((mask & (abi.GF_OVERFLOW | abi.GF_NEEDS_SYNC)) << 24)
+            assert emu_lib.emu_clear_group_flags(G, L, W, R, ptr(nodes), ptr(nodes), ptr(live), ptr(aux), lane,
+                                                 len(gids), ptr(gids), mask, block) == 0
+            assert np.array_equal(aux, want)
+    before = aux.copy()
+    dup = np.array([4, 9, 4], dtype=np.uint32)
+    assert emu_lib.emu_clear_group_flags(G, L, W, R, ptr(nodes), ptr(nodes), ptr(live), ptr(aux), 0, 3, ptr(dup),
+                                         abi.GF_NEEDS_SYNC, block) == abi.GPX_EINVAL
+    assert b"twice" in emu_lib.emu_last_error()
+    assert emu_lib.emu_clear_group_flags(G, L, W, R, ptr(nodes), ptr(nodes), ptr(live), ptr(aux), L, 2, ptr(dup),
+                                         abi.GF_NEEDS_SYNC, block) == abi.GPX_ERANGE
+    assert np.array_equal(aux, before)

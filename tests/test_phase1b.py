@@ -8,11 +8,8 @@ import pytest
 
 # GPX_EMU_SANITIZE=1 LD_PRELOAD=$(gcc -print-file-name=libasan.so) python -m pytest ... : the emulated kernels under
 # AddressSanitizer + UBSan (every heap buffer numpy hands them gets red zones; so do their local arrays)
-import os as _os
-EMU_SANITIZE = ["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"] if _os.environ.get("GPX_EMU_SANITIZE") else []
-
 from gigapaxos_b200.paxos_manager import NoopPaxosApp, PaxosManager
-from helpers import abi
+from helpers import abi, emu_library, ptr
 from p1b_cases import NODES5, assert_same_out, dump_all, make_engine, preconditions, random_elections
 
 
@@ -127,24 +124,14 @@ def test_elected_coordinator_proposes_the_plan(oracle_lib):
 
 # ---- the CUDA kernel's own source, run on the host ---------------------------------------------------------------------
 # tests/emu/ compiles gigapaxos_b200/csrc/gpx_phase1b.cuh (k_prepare_tally as the GPU runs it: a scalar kernel over
-# gpx_dev.cuh's structs and index helpers) with g++ and runs it thread by thread.  State goes in as the arrays DevState
+# gpx_dev.cuh's structs and index helpers) with g++ and runs it thread by thread, driven by the engine's own host sequence
+# (prepare_replies in gpx_state_seq.h: its checks, scratch layout, copies).  State goes in as the arrays DevState
 # describes, taken from the oracle engine's rows before the call; outputs and the state the kernel leaves are held
-# against the oracle's.  What this cannot see is the launch glue in gpx_engine.cu -- that is the GPU test's job
+# against the oracle's.  What this cannot see is the CUDA executor and the launch itself -- that is the GPU test's job
 # (tests/test_zz_phase1b_gpu.py).
 @pytest.fixture(scope="module")
 def emu_lib(tmp_path_factory):
-    import ctypes
-    import subprocess
-    from helpers import ROOT
-    import os
-    out = str(tmp_path_factory.mktemp("emu") / "libp1b_emu.so")
-    cuda_inc = "/usr/local/cuda/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("no CUDA headers")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *EMU_SANITIZE, "-I", cuda_inc,
-                           "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
-                           "-x", "c++", os.path.join(ROOT, "tests", "emu", "p1b_emu.cpp"), "-o", out])
-    return ctypes.CDLL(out)
+    return emu_library(tmp_path_factory, "p1b_emu")
 
 
 def _state_arrays(rows, R, G, W, Rcap, rng):
@@ -171,13 +158,11 @@ def _state_arrays(rows, R, G, W, Rcap, rng):
                                                           (5, 14, True, 7, None), (1, 15, False, 64, None), (4, 16, False, 33, None),
                                                           (3, 17, False, 64, [102]), (5, 18, True, 16, [101, 104])])
 def test_kernel_source_on_the_host_equals_oracle(oracle_lib, emu_lib, R, seed, wrap, block, lane_nodes):
-    import ctypes as C
     G, W = 160, 8
     Rcap = R
     rng = np.random.default_rng(seed)
     eng = make_engine(oracle_lib, R, G, lane_nodes)
     L = eng.n_lanes
-    ptr = lambda a: a.ctypes.data_as(C.c_void_p)
     for rnd in range(3):
         preconditions(eng, R, G, rng)
         els, reps = random_elections(R, G, rng, wrap, lane_nodes)
@@ -191,9 +176,23 @@ def test_kernel_source_on_the_host_equals_oracle(oracle_lib, emu_lib, R, seed, w
         members = np.array(NODES5[:R], dtype=np.int32)
         hosted = members if lane_nodes is None else np.array(lane_nodes, dtype=np.int32)
         launches = emu_lib.emu_prepare_tally(G, L, W, Rcap, R, ptr(members), ptr(hosted), ptr(live), ptr(crow), ptr(aux),
-                                             ptr(nsl), ptr(pwin), len(els), ptr(els), ptr(reps), ptr(got), block)
+                                             ptr(nsl), ptr(pwin), len(els), ptr(els), len(reps), ptr(reps), ptr(got),
+                                             block)
         assert launches == 1
         assert_same_out(got, want)
+        if rnd == 0:  # the engine's refusals, before anything runs: replies beyond n_reply_recs, two elections of a group
+            for k, (e2, n_reps, rc, error) in enumerate(((els, len(reps) - 1, abi.GPX_ERANGE, b"beyond n_reply_recs"),
+                                                        (np.concatenate([els, els[:1]]), len(reps), abi.GPX_EINVAL,
+                                                         b"more than one election"))):
+                st = [a.copy() for a in (crow, aux, nsl, pwin)]
+                if k == 0:
+                    e2 = e2[np.argsort(e2["first_reply"] + e2["n_replies"])]  # the last reply is referred to
+                bad = np.zeros(len(e2), dtype=abi.election_out_dtype)
+                assert emu_lib.emu_prepare_tally(G, L, W, Rcap, R, ptr(members), ptr(hosted), ptr(live), ptr(st[0]),
+                                                 ptr(st[1]), ptr(st[2]), ptr(st[3]), len(e2), ptr(e2), n_reps, ptr(reps),
+                                                 ptr(bad), block) == rc
+                assert error in emu_lib.emu_last_error() and not bad.view(np.uint8).any()
+                assert all(np.array_equal(x, y) for x, y in zip(st, (crow, aux, nsl, pwin)))
         after = dump_all(eng, R, G)
         won = {int(o["gid"]): (int(e["lane"]), (int(e["bnum"]), int(e["bcoord"])))
                for o, e in zip(want, els) if int(o["verdict"]) == abi.EL_MAJORITY}
@@ -298,7 +297,6 @@ def test_slots_half_the_int_range_apart_do_not_run_away(oracle_lib, emu_lib):
     """a (hostile or garbage) reply pair whose recorded minimum and carried-over maximum are exactly 2^31 apart: the
     reference's fill loop `curSlot - maxCarryoverSlot <= 0` :408 would never end on it; oracle, twin and kernel count the
     slots instead and agree that there is nothing to fill"""
-    import ctypes as C
     R, G = 2, 4
     INT_MIN = -(1 << 31)
     eng, twin_eng = make_engine(oracle_lib, R, G), make_engine(oracle_lib, R, G)
@@ -322,9 +320,8 @@ def test_slots_half_the_int_range_apart_do_not_run_away(oracle_lib, emu_lib):
     rng = np.random.default_rng(0)
     aux, crow, nsl, pwin = _state_arrays(rows, R, G, 8, R, rng)
     got = np.zeros(1, dtype=abi.election_out_dtype)
-    ptr = lambda a: a.ctypes.data_as(C.c_void_p)
     members = np.array(NODES5[:R], dtype=np.int32)
     live = np.ones(G, dtype=np.uint8)
     assert emu_lib.emu_prepare_tally(G, R, 8, R, R, ptr(members), ptr(members), ptr(live), ptr(crow), ptr(aux), ptr(nsl), ptr(pwin),
-                                     1, ptr(els), ptr(reps), ptr(got), 64) == 1
+                                     1, ptr(els), len(reps), ptr(reps), ptr(got), 64) == 1
     assert got[0].tobytes() == out.tobytes()

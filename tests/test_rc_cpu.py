@@ -12,28 +12,15 @@ import sys
 import numpy as np
 import pytest
 
-from helpers import ROOT, abi
+from helpers import ROOT, abi, emu_library, ptr
 from rc_cases import CELLS, Cache, Names, cell_dtype, ip_word, random_case, random_keys, random_requests, rc_hash
 
-SANITIZE = ["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"] if os.environ.get("GPX_EMU_SANITIZE") else []
 NONE = 0xFFFFFFFF
-
-
-def ptr(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    cuda_inc = "/usr/local/cuda/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("no CUDA headers")
-    so = str(tmp_path_factory.mktemp("rcemu") / "librc_emu.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *SANITIZE, "-I", cuda_inc,
-                           "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
-                           "-I", os.path.join(ROOT, "tests", "emu"), "-x", "c++",
-                           os.path.join(ROOT, "tests", "emu", "rc_emu.cpp"), "-o", so])
-    lib = C.CDLL(so)
+    lib = emu_library(tmp_path_factory, "rc_emu")
     lib.emu_rc_hash.restype = C.c_uint64
     lib.emu_rc_hash.argtypes = [C.c_uint32, C.c_uint32, C.c_int64, C.c_uint32, C.c_uint16]
     lib.emu_rc_cell_bytes.restype = C.c_uint32

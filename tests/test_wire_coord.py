@@ -18,7 +18,7 @@ import sys
 import numpy as np
 import pytest
 
-from helpers import ROOT, abi, wire_emu_library
+from helpers import ROOT, abi, emu_library, ptr
 from test_wire_dev import ENC_ACCEPTS, Emu
 from wire_coord_cases import (NOW_MS, check_requests, expected_accepts, malformed_request_packets, propose_blob,
                               random_accepts, random_request_packets)
@@ -27,13 +27,9 @@ from wire_dev_cases import random_world
 from gigapaxos_b200 import wire
 
 
-def ptr(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    return wire_emu_library(tmp_path_factory)
+    return emu_library(tmp_path_factory, "wire_emu")
 
 
 def decode_requests(e: Emu, pkts, block=64):

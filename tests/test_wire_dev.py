@@ -12,7 +12,7 @@ import sys
 import numpy as np
 import pytest
 
-from helpers import ROOT, abi, wire_emu_library
+from helpers import ROOT, abi, emu_library, ptr
 from wire_dev_cases import (World, check_decode, expected_encode_decisions, expected_encode_replies, malformed_packets,
                             random_decisions, random_packets, random_replies, random_world)
 
@@ -22,13 +22,9 @@ GOLD = json.load(open(os.path.join(ROOT, "tests", "golden", "wire_vectors.json")
 ENC_REPLIES, ENC_DECISIONS, ENC_ACCEPTS = 0, 1, 2  # the encoders of emu_wire_encode
 
 
-def ptr(a):
-    return a.ctypes.data_as(C.c_void_p)
-
-
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    return wire_emu_library(tmp_path_factory)
+    return emu_library(tmp_path_factory, "wire_emu")
 
 
 class Emu:

@@ -9,14 +9,14 @@ import sys
 import numpy as np
 import pytest
 
-from helpers import ROOT, wire_emu_library
+from helpers import ROOT, emu_library
 from test_wire_dev import ENC_DECISIONS, Emu
 from wire_dev_cases import expected_encode_decisions, random_decisions, random_world
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    return wire_emu_library(tmp_path_factory)
+    return emu_library(tmp_path_factory, "wire_emu")
 
 
 def encode_counted(e: Emu, recs, count, n_max, block):

@@ -18,7 +18,7 @@ import sys
 import numpy as np
 import pytest
 
-from helpers import ROOT, abi
+from helpers import ROOT, abi, emu_library, ptr
 from test_wire_dev import Emu
 from wire_coord_cases import NOW_MS, random_request_packets
 from wire_dev_cases import random_world
@@ -26,27 +26,10 @@ from wire_fwd_cases import expected_forwards, forward_case, json_wrappers, malfo
 
 from gigapaxos_b200 import wire
 
-SANITIZE = ["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"] if os.environ.get("GPX_EMU_SANITIZE") else []
-
-
-def ptr(a):
-    return a.ctypes.data_as(C.c_void_p)
-
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    cuda_inc = "/usr/local/cuda/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("no CUDA headers")
-    so = str(tmp_path_factory.mktemp("femu") / "libwire_fwd_emu.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *SANITIZE, "-I", cuda_inc,
-                           "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
-                           "-I", os.path.join(ROOT, "tests", "emu"), "-x", "c++",
-                           os.path.join(ROOT, "tests", "emu", "wire_fwd_emu.cpp"), "-o", so])
-    lib = C.CDLL(so)
-    lib.emu_wire_new.restype = C.c_void_p
-    lib.emu_wire_new.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p]
-    return lib
+    return emu_library(tmp_path_factory, "wire_fwd_emu")
 
 
 # ---- the decoders, on arenas ----------------------------------------------------------------------------------------

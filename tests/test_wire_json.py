@@ -12,41 +12,23 @@ import sys
 import numpy as np
 import pytest
 
-from helpers import ROOT, abi
+from helpers import ROOT, abi, emu_library, ptr
 from test_wire_dev import Emu
 from wire_dev_cases import random_world
 from wire_json_cases import as_bytes, as_json, group_into_packets, malformed_corpus, model_batch, random_logical
 
 from gigapaxos_b200 import packets_json as pj, wire
 
-SANITIZE = ["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"] if os.environ.get("GPX_EMU_SANITIZE") else []
 CHUNKS = [1, 7, 16, 64]
-
-
-def ptr(a):
-    return a.ctypes.data_as(C.c_void_p)
 
 
 @pytest.fixture(scope="module")
 def libs(tmp_path_factory):
-    cuda_inc = "/usr/local/cuda/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("no CUDA headers")
-    out = {}
-    d = tmp_path_factory.mktemp("jemu")
-    for ch in CHUNKS:
-        so = str(d / f"libwire_json_emu_{ch}.so")
-        subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *SANITIZE, f"-DGPX_JSON_CHUNK={ch}u",
-                               "-I", cuda_inc, "-I", os.path.join(ROOT, "include"),
-                               "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"), "-I", os.path.join(ROOT, "tests", "emu"),
-                               "-x", "c++", os.path.join(ROOT, "tests", "emu", "wire_json_emu.cpp"), "-o", so])
-        lib = C.CDLL(so)
-        lib.emu_wire_new.restype = C.c_void_p
-        lib.emu_wire_new.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p]
+    out = {ch: emu_library(tmp_path_factory, "wire_json_emu", f"GPX_JSON_CHUNK={ch}u") for ch in CHUNKS}
+    for lib in out.values():
         for f in ("emu_wire_free", "emu_wire_group", "emu_wire_names", "emu_wire_names_remove", "emu_wire_names_rehash",
                   "emu_wire_decode", "emu_wire_encode", "emu_wire_decode_json"):
             getattr(lib, f).argtypes = None
-        out[ch] = lib
     return out
 
 

@@ -13,7 +13,7 @@ import sys
 import numpy as np
 import pytest
 
-from helpers import ROOT, abi
+from helpers import ROOT, abi, emu_library, ptr
 from test_wire_dev import Emu
 from test_wire_json import decode_json
 from wire_dev_cases import World
@@ -22,28 +22,12 @@ from wire_json_out_cases import (MAX_MEMBER, WRAP_OVERHEAD, coordinator_commit_w
 
 from gigapaxos_b200 import packets_json as pj, wire
 
-SANITIZE = ["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"] if os.environ.get("GPX_EMU_SANITIZE") else []
 NODES = [100, 101, 102, 98, 99, 97, 96, 95]  # 103 and 104 stay remote
-
-
-def ptr(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    cuda_inc = "/usr/local/cuda/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("no CUDA headers")
-    so = str(tmp_path_factory.mktemp("joemu") / "libwire_json_out_emu.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *SANITIZE, "-I", cuda_inc,
-                           "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
-                           "-I", os.path.join(ROOT, "tests", "emu"), "-x", "c++",
-                           os.path.join(ROOT, "tests", "emu", "wire_json_out_emu.cpp"), "-o", so])
-    lib = C.CDLL(so)
-    lib.emu_wire_new.restype = C.c_void_p
-    lib.emu_wire_new.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p]
-    return lib
+    return emu_library(tmp_path_factory, "wire_json_out_emu")
 
 
 def encode_json(e: Emu, rep, dec, n_dec=None, wrap=0, block=64, sizes=None):

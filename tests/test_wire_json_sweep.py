@@ -14,7 +14,7 @@ import sys
 import numpy as np
 import pytest
 
-from helpers import ROOT, abi
+from helpers import ROOT, abi, emu_library, ptr
 from test_wire_dev import Emu
 from test_wire_forward import decode_json_requests, decode_members, decode_requests, encode_forwards, arena_of
 from test_wire_json_out import NODES, as_tuples, encode_json
@@ -25,37 +25,16 @@ from wire_json_sweep_cases import coordinator_world, expected_sweep, forward_cut
 
 from gigapaxos_b200 import packets_json as pj, wire
 
-SANITIZE = ["-fsanitize=address,undefined", "-fno-sanitize-recover=undefined", "-g"] if os.environ.get("GPX_EMU_SANITIZE") else []
-
-
-def ptr(a):
-    return None if a is None else a.ctypes.data_as(C.c_void_p)
-
-
-def build(tmp_path_factory, src):
-    cuda_inc = "/usr/local/cuda/include"
-    if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
-        pytest.skip("no CUDA headers")
-    so = str(tmp_path_factory.mktemp("jsemu") / f"lib{src}.so")
-    subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w", *SANITIZE, "-I", cuda_inc,
-                           "-I", os.path.join(ROOT, "include"), "-I", os.path.join(ROOT, "gigapaxos_b200", "csrc"),
-                           "-I", os.path.join(ROOT, "tests", "emu"), "-x", "c++",
-                           os.path.join(ROOT, "tests", "emu", src + ".cpp"), "-o", so])
-    lib = C.CDLL(so)
-    lib.emu_wire_new.restype = C.c_void_p
-    lib.emu_wire_new.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p]
-    return lib
-
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    return build(tmp_path_factory, "wire_json_sweep_emu")
+    return emu_library(tmp_path_factory, "wire_json_sweep_emu")
 
 
 @pytest.fixture(scope="module")
 def fwd_lib(tmp_path_factory):
     """the forwards encoder and the requests decoders, for the comparisons"""
-    return build(tmp_path_factory, "wire_fwd_emu")
+    return emu_library(tmp_path_factory, "wire_fwd_emu")
 
 
 def set_rows(e: Emu, rows: Rows):
