@@ -64,6 +64,10 @@ assert req_meta_dtype.itemsize == 32
 rc_key_dtype = np.dtype([("gid", "<u4"), ("handle", "<i4"), ("req_id", "<i8"), ("client_ip", "u1", (4,)),
                          ("client_port", "<u2"), ("pad", "<u2")])
 assert rc_key_dtype.itemsize == 24
+# gpx_wire_peer: the connection a client's packet came in on (gpx_wire_decode_client_requests_device); port 0 = unknown
+wire_peer_dtype = np.dtype([("sender_ip", "u1", (4,)), ("sender_port", "<u2"), ("receiver_port", "<u2"),
+                            ("receiver_ip", "u1", (4,)), ("pad", "<u4")])
+assert wire_peer_dtype.itemsize == 16
 # gpx_wire_member: one member of a JSON packet (gpx_wire_decode_json_device)
 wire_member_dtype = np.dtype([("pkt", "<u4"), ("off", "<u4"), ("len", "<u4"), ("status", "<i4")])
 # gpx_wire_encode_json_device: a wrapper's default and largest size, its head + tail, the largest member object

@@ -101,11 +101,10 @@ __device__ __forceinline__ uint32_t jg_be32(const uint8_t* p) {
 
 /* the keys of a journaled DECISION (journal.decision_json) and PREPARE (journal.prepare_json), up to 8 ISO-8859-1
  * characters packed little-endian */
-#define JK8(a, b, c, d, e, f, g, h) (JK(a, b, c, d, e) | ((uint64_t)(f) << 40) | ((uint64_t)(g) << 48) | ((uint64_t)(h) << 56))
 enum { JG_K_TYPE, JG_K_PT, JG_K_ID, JG_K_V, JG_K_B, JG_K_S, JG_K_GC_S, JG_K_QID, JG_K_ET, JG_K_E, JG_K_PREP, JG_K_N };
 struct JgcKeys {
   enum { N = JG_K_N, PP = -2 }; /* no array to jump over */
-  __device__ __forceinline__ static int id(const JStr& s) {
+  __device__ __forceinline__ static int id(const JStr& s, const JRd&, uint32_t) {
     if (s.wide) return -1;
     switch (s.len) {
       case 1:

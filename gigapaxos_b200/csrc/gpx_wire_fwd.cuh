@@ -10,9 +10,15 @@
  *                 sends its forwards as JSON members of BATCHED_PAXOS_PACKETs (PaxosPacketBatcher.process :270-277),
  *                 which gpx_wire_decode_json_device lists as GPX_WS_UNHANDLED; the REQUEST members among them become
  *                 proposals, as k_wire_req_decode makes them of the byte form.  One thread per member.
+ *   k_json_client the same decoder over a client's own packets (gpx_wire_decode_client_requests_device): a gigapaxos
+ *                 client sends each RequestPacket as a bare JSON object (PaxosClientAsync.sendRequest :165-172) with
+ *                 no "CA", so the client address comes from the receiver's stamp or the connection.  One thread per
+ *                 packet.
  * Both are scalar, like the kernels they sit beside, so tests/emu compiles this file for the host.
  */
 #pragma once
+#include <type_traits>
+
 #include "gpx_wire_json.cuh"
 
 /* ---- forwarded REQUEST packets (gpx_wire_encode_forwards_device) -------------------------------------------------- */
@@ -194,8 +200,29 @@ __device__ __forceinline__ int json_req_key(const JStr& s) {
 }
 struct JsonReqKeys {
   enum { N = JQ_N, PP = -2 };
-  __device__ __forceinline__ static int id(const JStr& s) { return json_req_key(s); }
+  __device__ __forceinline__ static int id(const JStr& s, const JRd&, uint32_t) { return json_req_key(s); }
 };
+/* ... and the receiver's stamps of a packet that came in over a socket (MessageExtractor.stampAddressIntoJSONObject
+ * :348-376): the connection's remote and local address, read where "CA" / "LA" are absent (RequestPacket(JSONObject)
+ * :530-536, JSONNIOTransport.getSenderAddress / getReceiverAddress).  A client's own request carries no "CA". */
+enum { JQ_SNDR = JQ_N, JQ_RCVR, JQ_CN };
+struct JsonClientKeys {
+  enum { N = JQ_CN, PP = -2 };
+  __device__ __forceinline__ static int id(const JStr& s, const JRd& J, uint32_t at) {
+    if (s.len != 13u || s.wide) return json_req_key(s);
+    if (s.head == JK8('_', 'S', 'N', 'D', 'R', '_', 'A', 'D') && json_key_rest(J, at, s, "DRESS", 5)) return JQ_SNDR;
+    if (s.head == JK8('_', 'R', 'C', 'V', 'R', '_', 'A', 'D') && json_key_rest(J, at, s, "DRESS", 5)) return JQ_RCVR;
+    return -1;
+  }
+};
+/* a request object's address keys: a stamp stands in for an absent "CA" / "LA", as the reference reads it */
+template <class Keys>
+__device__ __forceinline__ void json_req_stamps(uint32_t* pos) {
+  if constexpr (Keys::N > JQ_N) {
+    if (!pos[JQ_CA]) pos[JQ_CA] = pos[JQ_SNDR];
+    if (!pos[JQ_LA]) pos[JQ_LA] = pos[JQ_RCVR];
+  }
+}
 
 /* the fields of one request object */
 struct JsonReq {
@@ -310,6 +337,38 @@ struct WireJsonReqArgs {
   int emit;
 };
 
+/* a client's own packets (gpx_wire_decode_client_requests_device): the members are the whole packets, peers[k] the
+ * transport address of packet k's connection (nullptr: none) */
+static_assert(sizeof(gpx_wire_peer) == 16, "gpx_wire_peer is 16 bytes");
+struct WireClientReqArgs : WireJsonReqArgs {
+  const gpx_wire_peer* peers;
+};
+
+/* the first byte after leading whitespace opens a JSON object (a byteified packet's first byte is its type) */
+__device__ __forceinline__ bool json_object_at(JRd J) {
+  jr_ws(J);
+  return jr_peek(J) == '{';
+}
+
+/* an outer request with neither "CA" nor a stamp takes the connection's address, "LA" the local one; an unknown port
+ * (0) leaves the request to the host.  Entries of its BATCH take none: each is read from its own object (:541-552). */
+__device__ __forceinline__ int32_t json_req_peer(const gpx_wire_peer* peers, uint32_t k, const uint32_t* pos,
+                                                 JsonReq& f, int32_t st) {
+  if (!peers || st == GPX_WS_MALFORMED) return st;
+  const gpx_wire_peer p = peers[k];
+  if (!pos[JQ_CA]) {
+    if (!p.sender_port) return GPX_WS_UNHANDLED;
+    for (int b = 0; b < 4; b++) f.ca_ip[b] = p.sender_ip[b];
+    f.ca_port = p.sender_port;
+  }
+  if (!pos[JQ_LA]) {
+    if (!p.receiver_port) return GPX_WS_UNHANDLED;
+    for (int b = 0; b < 4; b++) f.la_ip[b] = p.receiver_ip[b];
+    f.la_port = p.receiver_port;
+  }
+  return st;
+}
+
 /* one request with its value unescaped: k_wire_req_decode's record (wire_put_request) for the same RequestPacket */
 __device__ __forceinline__ void json_put_request(const WireJsonReqArgs& A, WireReqTo& t, const JRd& J0,
                                                  const JsonReq& f) {
@@ -334,15 +393,16 @@ __device__ __forceinline__ void json_put_request(const WireJsonReqArgs& A, WireR
   }
 }
 
-/* one thread per member.  Pass 0 (emit == 0): a member listed GPX_WS_UNHANDLED that is a REQUEST object (PT 1) is
- * parsed and validated with its BATCH, its name, version and receiving node looked up: its status and output sizes;
- * every other member's status is copied.  Pass 1 parses the OK members again and writes their requests, meta and
- * values at the scanned offsets. */
-__global__ void k_json_req(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
-                           const __grid_constant__ WireJsonReqArgs A) {
-  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= A.n) return;
-  const gpx_wire_member mb = A.mem[i];
+/* one member (k_json_req: a member listed GPX_WS_UNHANDLED; k_json_client: a whole packet, Client).  Pass 0
+ * (emit == 0): a REQUEST object (PT 1) is parsed and validated with its BATCH, its name, version and receiving node
+ * looked up: its status and output sizes; every other member's status is copied.  Pass 1 parses the OK members again
+ * and writes their requests, meta and values at the scanned offsets.  A client's packet is decoded when it is an
+ * object: anything else, and JSON of another type, is the host's (GPX_WS_UNHANDLED); its addresses fall back to the
+ * stamps and then to the connection (json_req_peer). */
+template <bool Client, typename Args>
+__device__ __forceinline__ void json_req_run(const DevState& S, const WireNames& W, const Args& A, uint32_t i,
+                                             const gpx_wire_member mb) {
+  using Keys = typename std::conditional<Client, JsonClientKeys, JsonReqKeys>::type;
   if (A.emit && (A.status[i] != GPX_WS_OK || mb.status != GPX_WS_UNHANDLED)) return; /* a copied OK has no request */
   int32_t st = mb.status;
   uint32_t nreq = 0, pay = 0, gid = GPX_NAME_NONE, lane = 0;
@@ -352,17 +412,22 @@ __global__ void k_json_req(const __grid_constant__ DevState S, const __grid_cons
   J.n = mb.off;
   J.end = mb.off + mb.len;
   J.ok = true;
-  uint32_t pos[JQ_N], ppc = GPX_JSON_NONE;
+  uint32_t pos[Keys::N], ppc = GPX_JSON_NONE;
   JsonReq f;
   if (st == GPX_WS_UNHANDLED) {
     int32_t type = 0, pt = 0, ver = 0;
     if ((uint64_t)mb.off + mb.len > A.n_bytes || mb.pkt >= A.n_pkts) {
       st = GPX_WS_MALFORMED;
+    } else if (Client && !json_object_at(J)) {
+      /* the byte form, or no JSON object: the host's */
     } else {
-      json_keys_t<JsonReqKeys>(J, pos, nullptr, &ppc);
+      json_keys_t<Keys>(J, pos, nullptr, &ppc);
       jr_ws(J);
-      if (!J.ok || J.n != J.end || !json_get_i32(J, pos[JQ_TYPE], &type) || type != GPX_PT_PAXOS_PACKET ||
-          !json_get_i32(J, pos[JQ_PT], &pt))
+      if (!J.ok || J.n != J.end || !json_get_i32(J, pos[JQ_TYPE], &type))
+        st = GPX_WS_MALFORMED;
+      else if (Client && type != GPX_PT_PAXOS_PACKET) /* a client's other JSON */
+        st = GPX_WS_UNHANDLED;
+      else if (type != GPX_PT_PAXOS_PACKET || !json_get_i32(J, pos[JQ_PT], &pt))
         st = GPX_WS_MALFORMED;
       else if (pt != GPX_PT_REQUEST)
         st = GPX_WS_UNHANDLED;
@@ -370,7 +435,9 @@ __global__ void k_json_req(const __grid_constant__ DevState S, const __grid_cons
         st = pos[JQ_ID] && J.b[pos[JQ_ID]] == '"' && json_get_i32(J, pos[JQ_V], &ver) ? GPX_WS_OK : GPX_WS_MALFORMED;
     }
     if (st == GPX_WS_OK) {
+      json_req_stamps<Keys>(pos);
       st = json_req_fields(J, pos, f);
+      if constexpr (Client) st = json_req_peer(A.peers, i, pos, f, st);
       nreq = 1;
       pay = (f.qv_len + 15u) & ~15u;
       if (st != GPX_WS_MALFORMED && pos[JQ_BATCH]) { /* one level of latched requests (RequestBatcher) */
@@ -381,11 +448,12 @@ __global__ void k_json_req(const __grid_constant__ DevState S, const __grid_cons
         if (ok && jr_peek(B) == ']') {
         } else {
           while (ok) {
-            uint32_t sp[JQ_N];
-            json_keys_t<JsonReqKeys>(B, sp, nullptr, &ppc);
+            uint32_t sp[Keys::N];
+            json_keys_t<Keys>(B, sp, nullptr, &ppc);
             ok = B.ok && !sp[JQ_BATCH];
             if (!ok) break;
             JsonReq g;
+            json_req_stamps<Keys>(sp);
             const int32_t s = json_req_fields(B, sp, g);
             if (s == GPX_WS_MALFORMED) {
               ok = false;
@@ -433,13 +501,31 @@ __global__ void k_json_req(const __grid_constant__ DevState S, const __grid_cons
   jr_ws(B);
   if (jr_peek(B) == ']') return;
   for (;;) {
-    uint32_t sp[JQ_N];
-    json_keys_t<JsonReqKeys>(B, sp, nullptr, &ppc);
+    uint32_t sp[Keys::N];
+    json_keys_t<Keys>(B, sp, nullptr, &ppc);
     JsonReq g;
+    json_req_stamps<Keys>(sp);
     json_req_fields(B, sp, g);
     json_put_request(A, t, B, g);
     jr_ws(B);
     if (jr_peek(B) != ',') return;
     B.n++;
   }
+}
+
+/* one thread per member of gpx_wire_decode_json_requests_device */
+__global__ void k_json_req(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                           const __grid_constant__ WireJsonReqArgs A) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= A.n) return;
+  json_req_run<false>(S, W, A, i, A.mem[i]);
+}
+
+/* one thread per packet of gpx_wire_decode_client_requests_device: the packet is the member */
+__global__ void k_json_client(const __grid_constant__ DevState S, const __grid_constant__ WireNames W,
+                              const __grid_constant__ WireClientReqArgs A) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= A.n) return;
+  const gpx_wire_ref r = A.pkts[i];
+  json_req_run<true>(S, W, A, i, gpx_wire_member{i, r.off, r.len, GPX_WS_UNHANDLED});
 }

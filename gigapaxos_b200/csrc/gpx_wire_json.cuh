@@ -471,6 +471,7 @@ __device__ void jr_skip(JRd& J) {
 
 /* the keys the schema knows, as up to 8 ISO-8859-1 characters packed little-endian */
 #define JK(a, b, c, d, e) ((uint64_t)(a) | ((uint64_t)(b) << 8) | ((uint64_t)(c) << 16) | ((uint64_t)(d) << 24) | ((uint64_t)(e) << 32))
+#define JK8(a, b, c, d, e, f, g, h) (JK(a, b, c, d, e) | ((uint64_t)(f) << 40) | ((uint64_t)(g) << 48) | ((uint64_t)(h) << 56))
 enum { JK_TYPE, JK_PT, JK_ID, JK_V, JK_SNDR, JK_B, JK_S, JK_CP_S, JK_QID, JK_NACK, JK_SLOTS, JK_GC_S, JK_GROUP, JK_PP, JK_N };
 __device__ __forceinline__ int json_key(const JStr& s) {
   if (s.wide) return -1;
@@ -501,11 +502,23 @@ __device__ __forceinline__ int json_key(const JStr& s) {
   }
 }
 
-/* the key table of the packets and members above: json_key, JK_N of them, JK_PP the array a top level jumps over */
+/* the key table of the packets and members above: json_key, JK_N of them, JK_PP the array a top level jumps over.
+ * A table's id() sees the key's JStr, and the reader and the key's opening quote for a key longer than JStr.head. */
 struct JsonPktKeys {
   enum { N = JK_N, PP = JK_PP };
-  __device__ __forceinline__ static int id(const JStr& s) { return json_key(s); }
+  __device__ __forceinline__ static int id(const JStr& s, const JRd&, uint32_t) { return json_key(s); }
 };
+/* the key string at `at` (JStr s) goes on after its first 8 characters with the n characters of rest */
+__device__ __forceinline__ bool json_key_rest(const JRd& J0, uint32_t at, const JStr& s, const char* rest, uint32_t n) {
+  if (s.len != 8u + n) return false;
+  JRd J = J0;
+  J.n = at + 1u;
+  for (uint32_t q = 0; q < s.len; q++) {
+    uint32_t u = 0;
+    if (jr_unit(J, &u) != 0 || (q >= 8u && u != (uint8_t)rest[q - 8u])) return false;
+  }
+  return true;
+}
 
 /* the PP jump of a packet's top level: PP's '[' at p closes at the first depth-1 close after p */
 struct JsonJump {
@@ -529,12 +542,13 @@ __device__ __forceinline__ void json_keys_t(JRd& J, uint32_t* pos, const JsonJum
   }
   while (J.ok) {
     jr_ws(J);
+    const uint32_t kat = J.n;
     const JStr key = jr_string(J);
     jr_ws(J);
     jr_eat(J, ':');
     jr_ws(J);
     if (!J.ok) return;
-    const int kid = Keys::id(key);
+    const int kid = Keys::id(key, J, kat);
     if (kid == JK_PP && *pp_close != GPX_JSON_NONE) { /* a duplicated PP: validate the jumped one, the last counts */
       JRd V = J;
       V.n = pos[JK_PP];

@@ -481,6 +481,28 @@ static int wire_decode_json_requests(Ex& ex, C& call, const WireEnv& E, uint32_t
   return wire_requests_run(ex, call, E, k_json_req, A, o, reqs, meta, payload);
 }
 
+/* gpx_wire_decode_client_requests_device: the packets are the members */
+template <class Ex, class C>
+static int wire_decode_client_requests(Ex& ex, C& call, const WireEnv& E, uint32_t n, const uint8_t* bytes,
+                                       uint64_t n_bytes, const gpx_wire_ref* pkts, const gpx_wire_peer* peers,
+                                       int64_t now_ms, int32_t* status, gpx_request_rec* reqs, gpx_wire_req_meta* meta,
+                                       uint32_t* n_reqs, uint8_t* payload, uint64_t* payload_bytes) {
+  WireOut o[] = {{n_reqs, reqs && meta}, {payload_bytes, payload != nullptr}};
+  int rc = wire_args(wire_packets_given(n, bytes, n_bytes, pkts, status), n_bytes, o);
+  if (rc || n == 0) return rc;
+  WireClientReqArgs A;
+  memset(&A, 0, sizeof A);
+  A.bytes = bytes;
+  A.pkts = pkts;
+  A.peers = peers;
+  A.n_bytes = n_bytes;
+  A.n_pkts = n;
+  A.n = n;
+  A.now_ms = now_ms;
+  A.status = status;
+  return wire_requests_run(ex, call, E, k_json_client, A, o, reqs, meta, payload);
+}
+
 /* ---- forwards: a non-coordinator's REQUEST packets (gpx_wire_fwd.cuh) ------------------------------------------------ */
 template <class Ex, class C>
 static int wire_encode_forwards(Ex& ex, C& call, const WireEnv& E, const gpx_request_rec* reqs,

@@ -255,6 +255,83 @@ def request_json(r, pt: int = PT_REQUEST) -> bytes:
     return _dumps(_request_smart(r, pt))
 
 
+def _org_quote(s: str) -> str:
+    """org.json JSONObject.quote: '"', '\\\\' and '/' after '<' escaped, \\b \\t \\n \\f \\r, every other character below
+    U+0020, U+0080-U+009F and U+2000-U+20FF as \\uXXXX"""
+    out, prev = ['"'], ""
+    for c in s:
+        if c in '"\\':
+            out.append("\\" + c)
+        elif c == "/":
+            out.append("\\/" if prev == "<" else "/")
+        elif c in "\b\t\n\f\r":
+            out.append({"\b": "\\b", "\t": "\\t", "\n": "\\n", "\f": "\\f", "\r": "\\r"}[c])
+        elif c < " " or "\x80" <= c < "\xa0" or "\u2000" <= c < "\u2100":
+            out.append("\\u%04x" % ord(c))
+        else:
+            out.append(c)
+        prev = c
+    return "".join(out + ['"'])
+
+
+def _org_value(v) -> str:
+    if isinstance(v, bool):
+        return "true" if v else "false"
+    if isinstance(v, int):
+        return str(v)
+    if isinstance(v, str):
+        return _org_quote(v)
+    if isinstance(v, list):
+        return "[" + ",".join(_org_value(x) for x in v) + "]"
+    return "{" + ",".join(_org_quote(k) + ":" + _org_value(x) for k, x in v.items()) + "}"
+
+
+def _request_org(r, pt: int) -> dict:
+    """PaxosPacket.toJSONObject :478-494 over RequestPacket.toJSONObjectImpl :652-694, keys in the order they are put"""
+    d = _base(pt, r.paxos_id, r.version)
+    d.update({"QID": int(r.request_id), "QV": bytes(r.value).decode(CHARSET)})
+    if r.response:
+        d["RV"] = bytes(r.response).decode(CHARSET)
+    d["ET"] = int(r.entry_time)
+    if r.forward_count > 0:
+        d["NFWDS"] = int(r.forward_count)
+    if r.stop:
+        d["STOP"] = True
+    d["E"] = int(r.entry_replica)
+    for key, a in (("CA", r.client), ("LA", r.listen)):
+        if a is not None:
+            d[key] = f"/{a[0]}:{int(a[1])}"  # the InetSocketAddress, written by its toString()
+    if r.should_return:
+        d["QF"] = True
+    if r.batched:
+        d["BATCH"] = [_request_org(b, PT_REQUEST) for b in r.batched]
+    if r.broadcasted:
+        d["BC"] = True
+    if r.digest:
+        d["DIG"] = bytes(r.digest).decode(CHARSET)
+    return d
+
+
+def client_request_json(r, sender=None, receiver=None, smart: bool = False) -> bytes:
+    """What a gigapaxos client sends for a wire.Request (PaxosClientAsync.sendRequest :165-172: request.toJSONObject()),
+    a bare JSON object in org.json's form: keys in toJSONObjectImpl order, strings quoted as JSONObject.quote does,
+    ISO-8859-1 bytes.  A client's own request has no clientAddress, so r.client is normally None and there is no "CA".
+    smart: the json-smart form instead (request_json's object).
+    sender / receiver ((ip, port)): the stamps a receiver adds (MessageExtractor.stampAddressIntoJSONObject :348-376)
+    unless the key is present: org.json "_SNDR_ADDRESS":"a.b.c.d:port" (with the deprecated "_SNDR_IP" / "_SNDR_PORT")
+    and "_RCVR_ADDRESS", json-smart the InetSocketAddress.toString() form "/a.b.c.d:port"."""
+    d = _request_smart(r, PT_REQUEST) if smart else _request_org(r, PT_REQUEST)
+    if sender is not None:
+        d.setdefault("_SNDR_ADDRESS", f"/{sender[0]}:{int(sender[1])}" if smart else f"{sender[0]}:{int(sender[1])}")
+        if not smart:
+            d.setdefault("_SNDR_IP", str(sender[0]))
+            d.setdefault("_SNDR_PORT", int(sender[1]))
+    if receiver is not None:
+        d.setdefault("_RCVR_ADDRESS",
+                     f"/{receiver[0]}:{int(receiver[1])}" if smart else f"{receiver[0]}:{int(receiver[1])}")
+    return _dumps(d) if smart else _org_value(d).encode(CHARSET)
+
+
 def accepted_pvalue_obj(paxos_id: str, version: int, pv, blob: bytes, entry_replica: int = -1, entry_time: int = 0,
                         pt: int = PT_ACCEPT) -> dict:
     """One entry of ACC_MAP: the PValuePacket JSON (PaxosPacket.toJSONObject :478-494 + PValuePacket.toJSONObjectImpl

@@ -587,3 +587,39 @@ def decode_json_requests_device(engine, arena, refs, members, n_members: int, no
                 C.c_uint32(int(refs.shape[0])), _dptr(members), C.c_int64(now_ms), _dptr(status), _dptr(o[0]),
                 _dptr(o[1]), sz[0], _dptr(o[2]), sz[1], st))
     return RequestsOut(status[:n], reqs[: caps[0]], meta[: caps[0]], pay[: caps[1]], caps)
+
+
+# ---- a client's own requests: bare JSON REQUEST packets, addressed by their connection ---------------------------------
+def wire_peers(peers) -> np.ndarray:
+    """[(sender, receiver)] -> abi.wire_peer_dtype rows; an address is (ip, port) or None (port 0: unknown)"""
+    out = np.zeros(len(peers), abi.wire_peer_dtype)
+    for k, (snd, rcv) in enumerate(peers):
+        for pre, a in (("sender", snd), ("receiver", rcv)):
+            if a is not None:
+                out[k][pre + "_ip"] = [int(x) for x in a[0].split(".")]
+                out[k][pre + "_port"] = a[1]
+    return out
+
+
+def decode_client_requests_device(engine, arena, refs, peers, now_ms: int, caps, stream=None) -> RequestsOut:
+    """gpx_wire_decode_client_requests_device: the bare JSON REQUEST packets a client sends, refs[n] of `arena` (the
+    refs' node column names the receiving node), peers [n, 16] (abi.wire_peer_dtype rows on the device: each packet's
+    connection, the fallback client and listen address; None: no fallback).  caps = (requests, payload bytes);
+    GPX_ERANGE as in decode_batch_device.  Returns status int32 [n] (byteified packets and other JSON types
+    WS_UNHANDLED), reqs [k, 32] and meta [k, 32] grouped by gid (propose_device's input form, client = the packet
+    index), the payload arena and the two host sizes."""
+    import torch
+    n, dev = int(refs.shape[0]), refs.device
+    L, st = engine.L, stream_handle(stream)
+    with _on(stream):
+        status = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+        (reqs, meta, pay), caps = _sized(
+            engine, caps, (C.c_uint32, C.c_uint64),
+            lambda c: (torch.empty((max(c[0], 1), 32), dtype=torch.uint8, device=dev),
+                       torch.empty((max(c[0], 1), 32), dtype=torch.uint8, device=dev),
+                       torch.empty(max(c[1], 16), dtype=torch.uint8, device=dev)),
+            lambda o, sz: L.fn("wire_decode_client_requests_device")(
+                engine.handle, C.c_uint32(n), _dptr(arena), C.c_uint64(arena.numel()), _dptr(refs),
+                _dptr(peers), C.c_int64(now_ms), _dptr(status), _dptr(o[0]),
+                _dptr(o[1]), sz[0], _dptr(o[2]), sz[1], st))
+    return RequestsOut(status[:n], reqs[: caps[0]], meta[: caps[0]], pay[: caps[1]], caps)

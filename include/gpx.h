@@ -1327,6 +1327,51 @@ int gpx_wire_decode_json_requests_device(gpx_engine* e, uint32_t n_members, cons
                                          gpx_wire_req_meta* meta, uint32_t* n_reqs, uint8_t* payload,
                                          uint64_t* payload_bytes, void* stream);
 
+/* ---- a client's own requests: bare JSON REQUEST packets, addressed by the connection they came in on ------------
+ * A gigapaxos client sends each RequestPacket as a bare JSON object, PaxosPacket.toJSONObject :478-494 ("type", "PT",
+ * "ID", "V") over toJSONObjectImpl :652-694, neither as bytes nor inside a BATCHED_PAXOS_PACKET
+ * (PaxosClientAsync.sendRequest :165-172).  Its clientAddress is null, so it carries no "CA": the reference takes the
+ * client address from the connection.  On receipt MessageExtractor.stampAddressIntoJSONObject :348-376 adds
+ * "_SNDR_ADDRESS" and "_RCVR_ADDRESS" (the socket's remote and local address) unless the keys are there already, and
+ * RequestPacket(JSONObject) :530-536 uses "CA" if present, else the sender stamp; "LA" likewise with the receiver's.
+ * The host's socket layer knows those two addresses for every packet it hands to the device: gpx_wire_peer. */
+typedef struct gpx_wire_peer { /* 16 B */
+  uint8_t sender_ip[4];   /* the connection's remote address (IPv4) */
+  uint16_t sender_port;   /* 0 = unknown: no fallback address */
+  uint16_t receiver_port; /* the local listen address the packet came in on; 0 = unknown */
+  uint8_t receiver_ip[4];
+  uint32_t pad;
+} gpx_wire_peer;
+
+/* Decode n bare JSON REQUEST packets from clients into proposals.  pkts[k] is packet k in the arena, pkts[k].node the
+ * node that received it, peers[k] its connection.  bytes, pkts, peers, status, reqs, meta and payload are device
+ * pointers; peers may be NULL (no fallback address: an absent one is all zeros, as in
+ * gpx_wire_decode_json_requests_device).
+ *   Which packets: a packet whose first byte after leading whitespace is '{' and whose object is "type":90, "PT":1.
+ *     A byteified packet, and JSON of any other type or PT, is GPX_WS_UNHANDLED, so a node that receives both forms
+ *     calls this and gpx_wire_decode_requests_device over the same arena.
+ *   Schema, strictness, BATCH and the GPX_WS_* rules: gpx_wire_decode_json_requests_device's for a member, in the
+ *     org.json form a client writes and the json-smart form alike, with the receiving node pkts[k].node.  A packet
+ *     that is not one JSON object with an int "type", or whose "type" 90 comes without an int "PT", is
+ *     GPX_WS_MALFORMED.
+ *   Addresses, in the reference's order: client address = "CA" if the key is present, else "_SNDR_ADDRESS" if present,
+ *     else peers[k].sender_*; listen address = "LA", else "_RCVR_ADDRESS", else peers[k].receiver_*.  A stamp is read
+ *     in both forms the reference writes: "a.b.c.d:port" (org.json) and "[host]/a.b.c.d:port" (json-smart).  A present
+ *     string that is not a literal IPv4 address with a port of 1-65535, or a fallback whose port is 0, makes the packet
+ *     GPX_WS_UNHANDLED: the host decides (IPv6 and hostnames need a lookup).  A BATCH entry takes its own "CA" / "LA",
+ *     else its own stamps, else no address (all zeros): RequestPacket(JSONObject) :541-552 builds each entry from its
+ *     own object, which the receiver never stamps.
+ *   reqs, meta, payload: byte-identical to gpx_wire_decode_json_requests_device's for the same RequestPacket with the
+ *     resolved "CA" / "LA" written out, client = the packet index; an "E" of -1 becomes the receiving node and now_ms.
+ *     Grouped by gid, packet order within a gid: the input of gpx_response_cache_match_device and gpx_propose_device.
+ * One thread handles one packet, its BATCH included.  *n_reqs and *payload_bytes are HOST pointers, capacities in /
+ * sizes out; GPX_ERANGE reports the sizes and writes nothing else.  Stream-ordered on `stream` (NULL = the engine's
+ * stream) with the other wire calls' scratch; one synchronisation reads the totals. */
+int gpx_wire_decode_client_requests_device(gpx_engine* e, uint32_t n, const uint8_t* bytes, uint64_t n_bytes,
+                                           const gpx_wire_ref* pkts, const gpx_wire_peer* peers, int64_t now_ms,
+                                           int32_t* status, gpx_request_rec* reqs, gpx_wire_req_meta* meta,
+                                           uint32_t* n_reqs, uint8_t* payload, uint64_t* payload_bytes, void* stream);
+
 /* Encode a node's whole non-digest sweep as a loaded Java node sends it: gpx_wire_encode_json_device's replies and
  * decisions, and the requests gpx_wire_encode_forwards_device forwards, as REQUEST members of the same
  * BATCHED_PAXOS_PACKET wrappers (BATCHED_REQUESTS and BATCH_ACROSS_GROUPS, both on by default: PaxosPacketBatcher
